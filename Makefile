@@ -1,17 +1,11 @@
-# Builds libb2f.so (hand-written sm_100a kernels + C ABI) in-tree.
+# Builds libb2f.so (hand-written sm_90a kernels + C ABI) in-tree.
 NVCC      ?= /usr/local/cuda/bin/nvcc
-ARCH      := -gencode arch=compute_100a,code=sm_100a
+ARCH      := -gencode arch=compute_90a,code=sm_90a
 NVFLAGS   := $(ARCH) -O3 -std=c++17 -lineinfo -Xcompiler -fPIC -Xcompiler -Wall -cudart shared \
              --expt-relaxed-constexpr -Xptxas -v
 CSRC      := gpt_image_edit_b200/csrc
 LIBDIR    := gpt_image_edit_b200/lib
-# attention_experiments.cu (alternative kernel structures kept for the record, DESIGN.md section 7) is not part of
-# the product library: `make EXPERIMENTS=1` links it and enables B2F_ATTN_VARIANT 10-12 / 30-32 / 40-42 / 60-62.
-SRCS      := $(filter-out $(CSRC)/attention_experiments.cu,$(wildcard $(CSRC)/*.cu))
-ifeq ($(EXPERIMENTS),1)
-SRCS      += $(CSRC)/attention_experiments.cu
-NVFLAGS   += -DB2F_WITH_EXPERIMENTS
-endif
+SRCS      := $(wildcard $(CSRC)/*.cu)
 OBJS      := $(patsubst $(CSRC)/%.cu,build/%.o,$(SRCS))
 HDRS      := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/b2f.h
 

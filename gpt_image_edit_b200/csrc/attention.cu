@@ -1,42 +1,21 @@
-// Fused non-causal / causal softmax attention for sm_100a, head_dim 128, bf16 in/out.
+// Fused non-causal / causal softmax attention for sm_90a, head_dim 128, bf16 in/out.
 //
 //   O[b, q, h, :] = softmax(Q[b, q, h, :] · K[b, :, hk, :]^T * scale) · V[b, :, hk, :]
 //
-// One CTA owns TWO 128-row query tiles of one (batch, head) and streams K/V in 128-row blocks:
-//   warp 0 (1 lane)  TMA producer: Q tiles once, K/V blocks through a 4-slot 32 KB ring
-//   warp 1 (1 lane)  tcgen05.mma issuer:  S_t = Q_t·K_j^T (SS),  O_t += P_t·V_j (A = P from TMEM)
-//   warps 2..5       softmax warpgroup of tile 0   } one thread per query row: tcgen05.ld S,
-//   warps 6..9       softmax warpgroup of tile 1   } online max/sum, exp2, P -> TMEM (bf16) over S
-// TMEM (512 cols): S0|P0 [0,128)  S1|P1 [128,256)  O0 [256,384)  O1 [384,512).
-// While one warpgroup runs softmax on its tile, the tensor core works on the other tile.
-// O is rescaled lazily (only when the running max grows by more than 2^8), by the softmax
-// warpgroup itself, between "S ready" (which also proves the previous P·V finished) and "P ready".
-//
-// Kernels in this file (B2F_ATTN_VARIANT selects at run time; all parity-green, tests/test_attention_gpu.py):
-//   54 (default)  attn_fwd_kernel_2cta_nr<3>: the same two-tile structure as a CTA PAIR (cta_group::2, M = 256 MMAs, each
-//                 CTA stores half of every K / V tile) for non-causal, bias-free calls with >= 512 query rows (the FLUX
-//                 joint attention).  Warps 0-3 are a light warpgroup (TMA, MMA issue, TMEM allocator) that hands its
-//                 registers to the eight softmax warps with setmaxnreg (80 / 208: no spills); a third of the
-//                 exponentials run as a polynomial on the FMA pipe.  53 / 56: a quarter / none of them.
-//   51            attn_fwd_kernel_2cta<4>: the pair kernel with warps 2.. as softmax warps at the 168 registers the launch
-//                 bounds give (3 warps per sub-partition): 3-5 % slower
-//   1             attn_fwd_kernel<4>: the single-CTA two-tile kernel described above (causal, GQA, bias, short): what
-//                 the pair kernels do not cover falls through to it
-//   0,2,5,6       other fractions of exponentials on the FMA pipe;  50/52 the same for the 168-register pair kernel
-//   10-12, 30-32, 40-42, 60-62   experiments kept for the record in attention_experiments.cu (`make EXPERIMENTS=1`);
-//                 round-2 structural experiments (column-split pair, one tile per CTA with double / triple buffered S and
-//                 register prefetch) were measured and removed, see DESIGN.md section 7 and profiles/r02_attn_variants_*.json
+// One CTA owns a 128-row query tile of one (batch, head) and streams K/V in 128-row blocks:
+//   warpgroup 0 (1 lane)   TMA producer: Q once, K_j and V_j through two double-buffered 32 KB slots
+//   warpgroups 1, 2        64 query rows each:  S = Q·K_j^T (wgmma, both operands in smem, S in registers),
+//                          online softmax in registers (base 2), P packed to bf16 in registers,
+//                          O += P·V_j (wgmma with A = P from registers, B = V_j MN-major in smem)
+// The two consumer warpgroups run independently, so one warpgroup's softmax overlaps the other's MMAs.
+// Causal calls (Sq == Skv) stop streaming at the tile's last query row; GQA maps head h to K/V head h / (H / Hkv);
+// the BIAS kernel adds a bf16 score bias (T5 relative positions) before the softmax.
 //
 // Replaces F.scaled_dot_product_attention as reached by diffusers FluxAttnProcessor2_0
 // (SURVEY.md A.2; reference call site univa/utils/flux_pipeline.py:1067) and flash_attn as reached
 // through transformers' attn_implementation="flash_attention_2" (univa/serve/cli.py:40).
 #include <atomic>
 #include <cmath>
-#include <cstdlib>
-
-#ifndef B2F_ATTN_DEFAULT_VARIANT
-#define B2F_ATTN_DEFAULT_VARIANT 54
-#endif
 
 #include "attention_common.cuh"
 
@@ -46,702 +25,183 @@ extern std::atomic<uint64_t> g_launch_count;
 
 using namespace attn;
 
-#ifndef B2F_WITH_EXPERIMENTS
-namespace attn {
-bool experimental_variant(int, Variant*) { return false; }   // `make EXPERIMENTS=1` links attention_experiments.cu
-}  // namespace attn
-#endif
-
 namespace {
 
-// POLY: one pair of exponentials in every POLY pairs goes to the polynomial (0 = never).
-// TURNS: the two softmax warpgroups take turns on the exp section (forces anti-phase).
-// ABL: timing ablations (wrong results), see attention_fwd.  BIAS: additive bf16 score bias (T5 relative
-// position bias); the bias kernel folds the score scale into the bias step and runs with scale_log2 = log2(e).
-template <int POLY, bool TURNS, int ABL = 0, bool BIAS = false>
+// BIAS: additive bf16 score bias; the bias kernel folds the score scale into the bias step and runs with
+// scale_log2 = log2(e).
+template <bool BIAS>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
                                              ~uintptr_t(1023));
-  uint8_t* q_smem = smem;                       // 2 tiles
-  uint8_t* kv_smem = smem + 2 * TILE_BYTES;     // KV_SLOTS tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (2 + KV_SLOTS) * TILE_BYTES);
-  uint64_t* q_full = bars;            // 1
-  uint64_t* kv_full = bars + 1;       // KV_SLOTS
-  uint64_t* kv_empty = kv_full + KV_SLOTS;
-  uint64_t* s_full = kv_empty + KV_SLOTS;  // 2
-  uint64_t* p_full = s_full + 2;           // [tile][half] = 4: P columns [0,64) and [64,128) handed over separately
-  uint64_t* o_done = p_full + 4;           // 2
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(o_done + 2);
+  uint8_t* q_smem = smem;
+  uint8_t* k_smem = smem + TILE_BYTES;                      // KV_SLOTS tiles
+  uint8_t* v_smem = k_smem + KV_SLOTS * TILE_BYTES;         // KV_SLOTS tiles
+  uint64_t* bars = reinterpret_cast<uint64_t*>(v_smem + KV_SLOTS * TILE_BYTES);
+  uint64_t* q_full = bars;                 // 1
+  uint64_t* k_full = bars + 1;             // KV_SLOTS
+  uint64_t* k_empty = k_full + KV_SLOTS;
+  uint64_t* v_full = k_empty + KV_SLOTS;
+  uint64_t* v_empty = v_full + KV_SLOTS;
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int qpair = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
+  const int wg = __shfl_sync(0xffffffffu, int(threadIdx.x >> 7), 0);   // warp-uniform for the compiler
+  const int h = blockIdx.y, b = blockIdx.z;
   const int hk = h / (p.H / p.Hkv);
-  const int q0 = qpair * 2 * BQ;
-
-  // K/V blocks this CTA needs (causal: only up to its last query row; Sq == Skv assumed then)
+  const int q0 = blockIdx.x * BQ;
+  // K/V blocks this CTA needs (causal: only up to its last query row; Sq == Skv then)
   int kv_len = p.Skv;
-  if (p.causal) kv_len = min(p.Skv, q0 + 2 * BQ);
+  if (p.causal) kv_len = min(p.Skv, q0 + BQ);
   const int n_kv = (kv_len + BKV - 1) / BKV;
-  // the second Q tile of the last pair may lie entirely beyond Sq (S = 8736 = 34*256 + 32): skip all of
-  // its MMAs and its softmax warpgroup instead of multiplying zero rows
-  const bool t1_active = TURNS || (q0 + BQ < p.Sq);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
-  }
-  if (warp == 1 && lane == 0) {
     mbar_init(q_full, 1);
     for (int i = 0; i < KV_SLOTS; ++i) {
-      mbar_init(&kv_full[i], 1);
-      mbar_init(&kv_empty[i], 1);
+      mbar_init(&k_full[i], 1);
+      mbar_init(&v_full[i], 1);
+      mbar_init(&k_empty[i], 8);   // one arrive per consumer warp
+      mbar_init(&v_empty[i], 8);
     }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&o_done[i], 1);
-    }
-    for (int i = 0; i < 4; ++i) mbar_init(&p_full[i], 4);  // one elected arrive per softmax warp
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
+    if (threadIdx.x == 0) {
       // ---------------------------------------------------------------- TMA producer
-      mbar_expect_tx(q_full, 2 * TILE_BYTES);
-      for (int t = 0; t < 2; ++t)
+      mbar_expect_tx(q_full, TILE_BYTES);
+      for (int half = 0; half < 2; ++half)
+        tma_load_3d(q_smem + half * HALF_BYTES, &tmQ, q_full, h * DH + half * 64, q0, b);
+      for (int j = 0; j < n_kv; ++j) {
+        const int slot = j % KV_SLOTS;
+        const uint32_t phase = (j / KV_SLOTS) & 1;
+        mbar_wait(&k_empty[slot], phase ^ 1);
+        mbar_expect_tx(&k_full[slot], TILE_BYTES);
         for (int half = 0; half < 2; ++half)
-          tma_load_3d(q_smem + t * TILE_BYTES + half * (TILE_BYTES / 2), &tmQ, q_full,
-                      h * DH + half * 64, q0 + t * BQ, b);
-      int slot = 0;
-      uint32_t phase = 0;
-      for (int j = 0; j < n_kv; ++j) {
-        for (int kv = 0; kv < 2; ++kv) {  // K_j then V_j
-          mbar_wait(&kv_empty[slot], phase ^ 1);
-          mbar_expect_tx(&kv_full[slot], TILE_BYTES);
-          uint8_t* dst = kv_smem + slot * TILE_BYTES;
-          const CUtensorMap* tm = kv == 0 ? &tmK : &tmV;
-          tma_load_3d(dst, tm, &kv_full[slot], hk * DH, j * BKV, b);
-          tma_load_3d(dst + TILE_BYTES / 2, tm, &kv_full[slot], hk * DH + 64, j * BKV, b);
-          if (++slot == KV_SLOTS) {
-            slot = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer
-    // The WHOLE warp runs this loop (waits, descriptor arithmetic) so that the address math stays on
-    // the uniform datapath; only the tcgen05.mma / tcgen05.commit instructions are predicated to one
-    // lane.  (With the loop nested under `if (lane == 0)` every descriptor went through R2UR moves and
-    // the issue thread, not the tensor pipe, paced the kernel: ncu showed it busy ~75 % of the time.)
-    constexpr uint32_t idesc_qk = make_idesc_bf16(BQ, BKV, 0);  // B = K tile, K-major
-    constexpr uint32_t idesc_pv = make_idesc_bf16(BQ, DH, 1);   // B = V tile, MN-major
-    const uint32_t q_addr = smem_u32(q_smem);
-    const uint32_t kv_addr = smem_u32(kv_smem);
-    // descriptor of byte offset 0 of each buffer; every MMA operand is "base + constant" (one uniform
-    // 64-bit add on the 14-bit address field, which cannot carry out for addresses < 256 KB)
-    const uint64_t dq_base = make_sdesc_sw128(q_addr, 16, 1024);
-    const uint64_t dk_base = make_sdesc_sw128(kv_addr, 16, 1024);
-    const uint64_t dv_base = make_sdesc_sw128(kv_addr, TILE_BYTES / 2, 1024);
-    int slot = 0;
-    uint32_t phase = 0;
-    auto issue_qk = [&](int t, int k_slot) {
-      const uint32_t d = tmem_base + uint32_t(t * 128);
-      const uint64_t qd = dq_base + uint64_t((t * TILE_BYTES) >> 4);
-      const uint64_t kd = dk_base + uint64_t((k_slot * TILE_BYTES) >> 4);
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k) {
-          const uint64_t off = uint64_t(((k >> 2) * (TILE_BYTES / 2) + (k & 3) * 32) >> 4);
-          umma_ss(d, qd + off, kd + off, idesc_qk, k != 0 ? 1u : 0u);
-        }
-      }
-      __syncwarp();
-    };
-    // O_t += P_t[:, 64*hf : 64*hf+64] · V[64*hf : 64*hf+64, :]  (4 k-steps of 16 kv rows)
-    auto issue_pv = [&](int t, int v_slot, int hf, bool first) {
-      const uint32_t d = tmem_base + 256 + uint32_t(t * 128);
-      const uint32_t pa = tmem_base + uint32_t(t * 128 + hf * 32);
-      const uint64_t vd = dv_base + uint64_t((v_slot * TILE_BYTES + hf * 8192) >> 4);
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-          umma_ts(d, pa + k * 8, vd + uint64_t((k * 2048) >> 4), idesc_pv, (first && k == 0) ? 0u : 1u);
-      }
-      __syncwarp();
-    };
-    auto commit = [&](uint64_t* bar) {
-      if (elect_one()) umma_commit(bar);
-      __syncwarp();
-    };
-    auto advance = [&]() {
-      if (++slot == KV_SLOTS) {
-        slot = 0;
-        phase ^= 1;
-      }
-    };
-    mbar_wait(q_full, 0);
-    // prologue: S_t = Q_t K_0^T for both tiles
-    mbar_wait(&kv_full[slot], phase);
-    tc_fence_after();
-    issue_qk(0, slot);
-    commit(&s_full[0]);
-    if (t1_active) {
-      issue_qk(1, slot);
-      commit(&s_full[1]);
-    }
-    commit(&kv_empty[slot]);
-    advance();
-    for (int j = 0; j < n_kv; ++j) {
-      const int v_slot = slot;
-      const uint32_t v_phase = phase;
-      advance();
-      const int k_slot = slot;  // K_{j+1} (if any)
-      const uint32_t k_phase = phase;
-      const bool more = (j + 1 < n_kv);
-      if (more) advance();
-      mbar_wait(&kv_full[v_slot], v_phase);
-      // tile 0: the first half of P·V starts while the warpgroup still exponentiates the second half
-      mbar_wait(&p_full[0], j & 1);
-      tc_fence_after();
-      issue_pv(0, v_slot, 0, j == 0);
-      mbar_wait(&p_full[1], j & 1);
-      tc_fence_after();
-      issue_pv(0, v_slot, 1, false);
-      if (more) {
-        mbar_wait(&kv_full[k_slot], k_phase);
-        tc_fence_after();
-        issue_qk(0, k_slot);
-        commit(&s_full[0]);
-      }
-      // tile 1
-      if (t1_active) {
-        mbar_wait(&p_full[2], j & 1);
-        tc_fence_after();
-        issue_pv(1, v_slot, 0, j == 0);
-        mbar_wait(&p_full[3], j & 1);
-        tc_fence_after();
-        issue_pv(1, v_slot, 1, false);
-      }
-      commit(&kv_empty[v_slot]);
-      if (more) {
-        if (t1_active) {
-          issue_qk(1, k_slot);
-          commit(&s_full[1]);
-        }
-        commit(&kv_empty[k_slot]);
-      }
-    }
-    commit(&o_done[0]);
-    commit(&o_done[1]);
-  } else {
-    // ------------------------------------------------------------------ softmax warpgroups
-    const int t = (warp - 2) >> 2;
-    const int quarter = warp & 3;
-    const int row_in_tile = quarter * 32 + lane;
-    const int q_row = q0 + t * BQ + row_in_tile;  // query index inside the sequence
-    const uint32_t lane_addr = uint32_t(quarter * 32) << 16;
-    const uint32_t s_tmem = tmem_base + lane_addr + uint32_t(t * 128);
-    const uint32_t o_tmem = tmem_base + lane_addr + 256 + uint32_t(t * 128);
-    float m = -INFINITY, l = 0.f;
-    if (t == 0 || t1_active) {
-    if (TURNS) {
-    // named barriers 1/2 = "tile 0 / tile 1 may run its exp section"; tile 0 goes first
-    if (t == 1) named_bar_arrive(1, 256);
-    }
-    for (int j = 0; j < n_kv; ++j) {
-      mbar_wait(&s_full[t], j & 1);
-      tc_fence_after();
-      uint32_t sr[128];
-      B2F_TMEM_LD_X32(s_tmem + 0, (sr + 0));
-      B2F_TMEM_LD_X32(s_tmem + 32, (sr + 32));
-      B2F_TMEM_LD_X32(s_tmem + 64, (sr + 64));
-      B2F_TMEM_LD_X32(s_tmem + 96, (sr + 96));
-      tmem_wait_ld();
-      const int kv0 = j * BKV;
-      if (BIAS) {
-        if (q_row < p.Sq) {
-          const __nv_bfloat16* brow = p.bias + (long long)h * p.bias_h_stride +
-                                      (long long)q_row * p.bias_row_stride + kv0;
-          const int n_ok = min(BKV, p.Skv - kv0);
-#pragma unroll
-          for (int c = 0; c < 128; ++c)
-            if (c < n_ok)
-              sr[c] = __float_as_uint(fmaf(__uint_as_float(sr[c]), p.bias_scale, __bfloat162float(brow[c])));
-        }
-      }
-      const bool need_mask = (kv0 + BKV > p.Skv) || (p.causal && kv0 + BKV > q0 + t * BQ);
-      if (need_mask) {
-        const int limit = p.causal ? min(p.Skv, q_row + 1) : p.Skv;
-#pragma unroll
-        for (int c = 0; c < 128; ++c)
-          if (kv0 + c >= limit) sr[c] = 0xff800000u;  // -inf
-      }
-      // row max with 3-input FMNMX3 in 4 independent chains (a single dependent chain costs ~4 clk per
-      // link and only two softmax warps share an SM sub-partition, so nothing would hide it)
-      float mx4[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i)
-        mx4[i] = fmaxf(__uint_as_float(sr[2 * i]), __uint_as_float(sr[2 * i + 1]));
-#pragma unroll
-      for (int c = 8; c < 128; c += 8)
-#pragma unroll
-        for (int i = 0; i < 4; ++i)
-          mx4[i] = fmax3(mx4[i], __uint_as_float(sr[c + 2 * i]), __uint_as_float(sr[c + 2 * i + 1]));
-      const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-      const float m_new = fmaxf(m, mx * p.scale_log2);
-      // lazy rescale: keep the stale max unless it grew by more than 2^8 (P stays < 256)
-      const bool grow = (m_new - m) > 8.0f;
-      const float m_use = grow ? m_new : m;
-      const float alpha = grow ? ex2(m - m_use) : 1.0f;
-      const float neg_m = (m_use == -INFINITY) ? 0.f : -m_use;  // fully masked row (causal tail)
-      if (j > 0 && __any_sync(0xffffffffu, grow)) {
-        // Rare path, BEFORE any P of this block is published: S_t(j) being ready proves P_t·V_{j-1}
-        // completed and P_t·V_j cannot start before the arrives below, so O_t is quiescent here.
-#pragma unroll 1
-        for (int c0 = 0; c0 < 128; c0 += 32) {
-          uint32_t o[32];
-          B2F_TMEM_LD_X32(o_tmem + c0, o);
-          tmem_wait_ld();
-#pragma unroll
-          for (int c = 0; c < 32; ++c) o[c] = __float_as_uint(__uint_as_float(o[c]) * alpha);
-          B2F_TMEM_ST_X32(o_tmem + c0, o);
-        }
-      }
-      float sum4[4] = {0.f, 0.f, 0.f, 0.f};   // two packed (FADD2) accumulator pairs
-      if (TURNS) named_bar_sync(1 + t, 256);
-#pragma unroll
-      for (int half = 0; half < 2; ++half) {
-        uint32_t pk[32];
-#pragma unroll
-        for (int c = 0; c < 32; ++c) {
-          float x0, x1;
-          ffma2(x0, x1, __uint_as_float(sr[half * 64 + 2 * c]), __uint_as_float(sr[half * 64 + 2 * c + 1]),
-                p.scale_log2, p.scale_log2, neg_m, neg_m);
-          float p0, p1;
-          if (POLY && (c % (POLY ? POLY : 1)) == (POLY ? POLY : 1) - 1) {
-            ex2_poly2(x0, x1, p0, p1);
-          } else if (ABL & 1) {
-            p0 = x0 * 1e-3f;   // ablation: no MUFU
-            p1 = x1 * 1e-3f;
-          } else {
-            p0 = ex2(x0);
-            p1 = ex2(x1);
-          }
-          const int a = (c & 1) * 2;
-          fadd2(sum4[a], sum4[a + 1], sum4[a], sum4[a + 1], p0, p1);
-          pk[c] = pack_bf16x2(p0, p1);
-        }
-        B2F_TMEM_ST_X32(s_tmem + half * 32, pk);
-        // publish this half of P (and, with the first half, the rescaled O): one arrive per warp
-        tmem_wait_st();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&p_full[t * 2 + half]);
-      }
-      if (TURNS) named_bar_arrive(1 + (t ^ 1), 256);
-      l = l * alpha + ((sum4[0] + sum4[1]) + (sum4[2] + sum4[3]));
-      m = m_use;
-    }
-    // ---------------------------------------------------------------- epilogue: O / l -> bf16
-    mbar_wait(&o_done[t], 0);
-    tc_fence_after();
-    const float inv_l = 1.0f / l;
-    const bool row_ok = q_row < p.Sq;
-    if (p.lse && row_ok) p.lse[((long long)b * p.H + h) * p.lse_stride + q_row] = m + log2f(l);
-    __nv_bfloat16* out_row =
-        p.out + ((long long)b * p.Sq + q_row) * p.ldo + (long long)h * DH;
-#pragma unroll 1
-    for (int c0 = 0; c0 < 128; c0 += 32) {
-      uint32_t o[32];
-      __syncwarp();
-      B2F_TMEM_LD_X32(o_tmem + c0, o);
-      tmem_wait_ld();
-      if (row_ok) {
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          uint4 v;
-          v.x = pack_bf16x2(__uint_as_float(o[g * 8 + 0]) * inv_l, __uint_as_float(o[g * 8 + 1]) * inv_l);
-          v.y = pack_bf16x2(__uint_as_float(o[g * 8 + 2]) * inv_l, __uint_as_float(o[g * 8 + 3]) * inv_l);
-          v.z = pack_bf16x2(__uint_as_float(o[g * 8 + 4]) * inv_l, __uint_as_float(o[g * 8 + 5]) * inv_l);
-          v.w = pack_bf16x2(__uint_as_float(o[g * 8 + 6]) * inv_l, __uint_as_float(o[g * 8 + 7]) * inv_l);
-          *reinterpret_cast<uint4*>(out_row + c0 + g * 8) = v;
-        }
-      }
-    }
-    }  // t == 0 || t1_active
-  }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
-  }
-}
-
-
-// ================================================================================================
-// CTA-PAIR kernel (cluster of 2, tcgen05 cta_group::2).  The two-tile kernel above is bound by shared-memory
-// bandwidth, not by the softmax: per KV block and Q tile an M=128 SS-MMA reads the whole Q tile (32 KB) and the
-// whole K tile (32 KB) — 128 B/clk during QK, the full smem bandwidth of an SM — plus V for P·V and the TMA
-// writes of K/V (~125 B/clk on average; every single-tile / sub-block variant kept or raised that figure, which
-// is why none was faster).  Here two CTAs own 512 query rows of a head: every MMA is M=256 (128 rows per CTA)
-// and each CTA stores only HALF of every K tile (64 of its 128 kv rows) and HALF of every V tile (64 of its 128
-// dh columns); the hardware shares the B halves between the two SMs.  Per tile and KV block an SM now moves
-// 16 KB (TMA) + 48 KB (QK: Q 32 + K/2 16) + 16 KB (P·V: V/2) = 80 KB instead of 128 KB.
-//   rows of pair pr:  tile t of CTA c = [512 pr + 256 t + 128 c, +128)
-//   TMEM per CTA (its 128 lanes of the M=256 accumulators): S0|P0, S1|P1, O0, O1 as above
-//   barriers: q_full / kv_full / p_full live on CTA 0 (the only MMA issuer; CTA 1's TMA bytes and softmax warps
-//   signal them remotely), s_full / o_done / kv_empty exist in both CTAs and receive multicast commits.
-// Non-causal, no bias (the FLUX joint attention); everything else goes to the kernels above.
-constexpr int P2_SLOTS = 8;                       // half tiles of 16 KB: K_j/2, V_j/2 alternating
-constexpr int P2_HALF = TILE_BYTES / 2;
-constexpr int P2_SMEM = 2 * TILE_BYTES + P2_SLOTS * P2_HALF + 256 + 1024;
-constexpr int P2_THREADS_NR = 128 + 8 * 32;       // light warpgroup + 8 softmax warps
-
-// NR = 0: warps 0 / 1 = TMA / MMA, warps 2.. = softmax (register budget from the launch bounds: 168 with 3 warps per
-// sub-partition).  NR > 0: warps 0-3 form a light warpgroup (TMA, MMA, TMEM allocator, idle) that gives its registers
-// up with setmaxnreg.dec and the softmax warpgroups (warps 4..) grow to NR registers.
-template <int POLY, int NR>
-static __device__ __forceinline__ void attn_pair_body(const CUtensorMap& tmQ, const CUtensorMap& tmK, const CUtensorMap& tmV,
-                                                      const AttnParams& p) {
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
-  uint8_t* q_smem = smem;                       // 2 tiles of this CTA's rows
-  uint8_t* kv_smem = smem + 2 * TILE_BYTES;     // P2_SLOTS half tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + 2 * TILE_BYTES + P2_SLOTS * P2_HALF);
-  uint64_t* q_full = bars;                      // 1   (CTA 0)
-  uint64_t* kv_full = bars + 1;                 // P2_SLOTS (CTA 0)
-  uint64_t* kv_empty = kv_full + P2_SLOTS;      // P2_SLOTS (both)
-  uint64_t* s_full = kv_empty + P2_SLOTS;       // 2 (both)
-  uint64_t* p_full = s_full + 2;                // [tile][half] = 4 (CTA 0)
-  uint64_t* o_done = p_full + 4;                // 2 (both)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(o_done + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();
-  const bool leader = crank == 0;
-  const int pr = blockIdx.x >> 1, h = blockIdx.y, b = blockIdx.z;
-  const int hk = h / (p.H / p.Hkv);
-  const int q0 = pr * 4 * BQ;                   // first row of the pair
-  const int n_kv = (p.Skv + BKV - 1) / BKV;
-  const bool t1_active = q0 + 2 * BQ < p.Sq;    // second tile of BOTH CTAs beyond Sq: skip it
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-  }
-  if (warp == 1 && lane == 0) {
-    mbar_init(q_full, 2);                       // one arrive per CTA's producer (+ both CTAs' TMA bytes)
-    for (int i = 0; i < P2_SLOTS; ++i) {
-      mbar_init(&kv_full[i], 2);
-      mbar_init(&kv_empty[i], 1);               // one multicast commit
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&s_full[i], 1);
-      mbar_init(&o_done[i], 1);
-    }
-    for (int i = 0; i < 4; ++i) mbar_init(&p_full[i], 8);   // 4 softmax warps x 2 CTAs
-    fence_mbar_init();
-  }
-  if (warp == 2) {
-    tmem_alloc_2cta(tmem_ptr, 512);
-    tmem_relinquish_2cta();
-  }
-  tc_fence_before();
-  __syncthreads();      // CTA-scope barrier for the smem word tcgen05.alloc wrote (racecheck does not model barrier.cluster)
-  cluster_sync_all();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  constexpr int SW0 = NR > 0 ? 4 : 2;   // first softmax warp
-
-  if (warp < SW0) {
-  if constexpr (NR > 0) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(80));
-  if (warp == 0) {
-    if (lane == 0) {
-      // ---------------------------------------------------------------- TMA producer (one per CTA)
-      if (leader)
-        mbar_expect_tx(q_full, 4 * TILE_BYTES);
-      else
-        mbar_arrive_cta0(q_full);
-      for (int t = 0; t < 2; ++t)
+          tma_load_3d(k_smem + slot * TILE_BYTES + half * HALF_BYTES, &tmK, &k_full[slot], hk * DH + half * 64, j * BKV, b);
+        mbar_wait(&v_empty[slot], phase ^ 1);
+        mbar_expect_tx(&v_full[slot], TILE_BYTES);
         for (int half = 0; half < 2; ++half)
-          tma_load_3d_2cta(q_smem + t * TILE_BYTES + half * (TILE_BYTES / 2), &tmQ, q_full, h * DH + half * 64,
-                           q0 + t * 2 * BQ + int(crank) * BQ, b);
-      int slot = 0;
-      uint32_t phase = 0;
-      for (int j = 0; j < n_kv; ++j) {
-        for (int kv = 0; kv < 2; ++kv) {  // K_j/2 then V_j/2
-          mbar_wait(&kv_empty[slot], phase ^ 1);
-          if (leader)
-            mbar_expect_tx(&kv_full[slot], 2 * P2_HALF);
-          else
-            mbar_arrive_cta0(&kv_full[slot]);
-          uint8_t* dst = kv_smem + slot * P2_HALF;
-          if (kv == 0) {
-            // this CTA's 64 kv rows of K_j, both 64-column dh halves (8 KB each)
-            tma_load_3d_2cta(dst, &tmK, &kv_full[slot], hk * DH, j * BKV + int(crank) * 64, b);
-            tma_load_3d_2cta(dst + P2_HALF / 2, &tmK, &kv_full[slot], hk * DH + 64, j * BKV + int(crank) * 64, b);
-          } else {
-            // this CTA's 64 dh columns of V_j, all 128 kv rows
-            tma_load_3d_2cta(dst, &tmV, &kv_full[slot], hk * DH + int(crank) * 64, j * BKV, b);
-          }
-          if (++slot == P2_SLOTS) {
-            slot = 0;
-            phase ^= 1;
-          }
-        }
+          tma_load_3d(v_smem + slot * TILE_BYTES + half * HALF_BYTES, &tmV, &v_full[slot], hk * DH + half * 64, j * BKV, b);
       }
     }
-  } else if (warp == 1) {
-    if (leader) {
-      // ---------------------------------------------------------------- MMA issuer (warp-uniform loop)
-      constexpr uint32_t idesc_qk = make_idesc_bf16(2 * BQ, BKV, 0);  // M = 256, B = K (K-major, 64 rows per CTA)
-      constexpr uint32_t idesc_pv = make_idesc_bf16(2 * BQ, DH, 1);   // M = 256, B = V (MN-major, 64 dh per CTA)
-      const uint64_t dq_base = make_sdesc_sw128(smem_u32(q_smem), 16, 1024);
-      const uint64_t dk_base = make_sdesc_sw128(smem_u32(kv_smem), 16, 1024);
-      const uint64_t dv_base = make_sdesc_sw128(smem_u32(kv_smem), P2_HALF, 1024);
-      int slot = 0;
-      uint32_t phase = 0;
-      auto issue_qk = [&](int t, int k_slot) {
-        const uint32_t d = tmem_base + uint32_t(t * 128);
-        const uint64_t qd = dq_base + uint64_t((t * TILE_BYTES) >> 4);
-        const uint64_t kd = dk_base + uint64_t((k_slot * P2_HALF) >> 4);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < DH / 16; ++k) {
-            const uint64_t qoff = uint64_t(((k >> 2) * (TILE_BYTES / 2) + (k & 3) * 32) >> 4);
-            const uint64_t koff = uint64_t(((k >> 2) * (P2_HALF / 2) + (k & 3) * 32) >> 4);
-            umma_ss_2cta(d, qd + qoff, kd + koff, idesc_qk, k != 0 ? 1u : 0u);
-          }
-        }
-        __syncwarp();
-      };
-      auto issue_pv = [&](int t, int v_slot, int hf, bool first) {
-        const uint32_t d = tmem_base + 256 + uint32_t(t * 128);
-        const uint32_t pa = tmem_base + uint32_t(t * 128 + hf * 32);
-        const uint64_t vd = dv_base + uint64_t((v_slot * P2_HALF + hf * 8192) >> 4);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            umma_ts_2cta(d, pa + k * 8, vd + uint64_t((k * 2048) >> 4), idesc_pv, (first && k == 0) ? 0u : 1u);
-        }
-        __syncwarp();
-      };
-      auto commit = [&](uint64_t* bar) {
-        if (elect_one()) umma_commit_2cta(bar);
-        __syncwarp();
-      };
-      auto advance = [&]() {
-        if (++slot == P2_SLOTS) {
-          slot = 0;
-          phase ^= 1;
-        }
-      };
-      mbar_wait(q_full, 0);
-      mbar_wait(&kv_full[slot], phase);
-      tc_fence_after();
-      issue_qk(0, slot);
-      commit(&s_full[0]);
-      if (t1_active) {
-        issue_qk(1, slot);
-        commit(&s_full[1]);
-      }
-      commit(&kv_empty[slot]);
-      advance();
-      for (int j = 0; j < n_kv; ++j) {
-        const int v_slot = slot;
-        const uint32_t v_phase = phase;
-        advance();
-        const int k_slot = slot;
-        const uint32_t k_phase = phase;
-        const bool more = (j + 1 < n_kv);
-        if (more) advance();
-        mbar_wait(&kv_full[v_slot], v_phase);
-        mbar_wait(&p_full[0], j & 1);
-        tc_fence_after();
-        issue_pv(0, v_slot, 0, j == 0);
-        mbar_wait(&p_full[1], j & 1);
-        tc_fence_after();
-        issue_pv(0, v_slot, 1, false);
-        if (more) {
-          mbar_wait(&kv_full[k_slot], k_phase);
-          tc_fence_after();
-          issue_qk(0, k_slot);
-          commit(&s_full[0]);
-        }
-        if (t1_active) {
-          mbar_wait(&p_full[2], j & 1);
-          tc_fence_after();
-          issue_pv(1, v_slot, 0, j == 0);
-          mbar_wait(&p_full[3], j & 1);
-          tc_fence_after();
-          issue_pv(1, v_slot, 1, false);
-        }
-        commit(&kv_empty[v_slot]);
-        if (more) {
-          if (t1_active) {
-            issue_qk(1, k_slot);
-            commit(&s_full[1]);
-          }
-          commit(&kv_empty[k_slot]);
-        }
-      }
-      commit(&o_done[0]);
-      commit(&o_done[1]);
-    }
-  }
-  } else {
-  if constexpr (NR > 0) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(NR));
-  {
-    // ------------------------------------------------------------------ softmax warpgroups (both CTAs)
-    const int t = (warp - SW0) >> 2;
-    const int quarter = warp & 3;
-    const int row_in_tile = quarter * 32 + lane;
-    const int q_row = q0 + t * 2 * BQ + int(crank) * BQ + row_in_tile;
-    const uint32_t lane_addr = uint32_t(quarter * 32) << 16;
-    const uint32_t s_tmem = tmem_base + lane_addr + uint32_t(t * 128);
-    const uint32_t o_tmem = tmem_base + lane_addr + 256 + uint32_t(t * 128);
-    float m = -INFINITY, l = 0.f;
-    if (t == 0 || t1_active) {
-      for (int j = 0; j < n_kv; ++j) {
-        mbar_wait(&s_full[t], j & 1);
-        tc_fence_after();
-        uint32_t sr[128];
-        const int kv0 = j * BKV;
-        float mx4[4];
-        B2F_TMEM_LD_X32(s_tmem + 0, (sr + 0));
-        B2F_TMEM_LD_X32(s_tmem + 32, (sr + 32));
-        B2F_TMEM_LD_X32(s_tmem + 64, (sr + 64));
-        B2F_TMEM_LD_X32(s_tmem + 96, (sr + 96));
-        tmem_wait_ld();
-        if (kv0 + BKV > p.Skv) {
-#pragma unroll
-          for (int c = 0; c < 128; ++c)
-            if (kv0 + c >= p.Skv) sr[c] = 0xff800000u;  // -inf
-        }
-#pragma unroll
-        for (int i = 0; i < 4; ++i) mx4[i] = fmaxf(__uint_as_float(sr[2 * i]), __uint_as_float(sr[2 * i + 1]));
-#pragma unroll
-        for (int c = 8; c < 128; c += 8)
-#pragma unroll
-          for (int i = 0; i < 4; ++i)
-            mx4[i] = fmax3(mx4[i], __uint_as_float(sr[c + 2 * i]), __uint_as_float(sr[c + 2 * i + 1]));
-        const float mx = fmaxf(fmaxf(mx4[0], mx4[1]), fmaxf(mx4[2], mx4[3]));
-        const float m_new = fmaxf(m, mx * p.scale_log2);
-        const bool grow = (m_new - m) > 8.0f;     // lazy rescale (P stays < 2^8)
-        const float m_use = grow ? m_new : m;
-        const float alpha = grow ? ex2(m - m_use) : 1.0f;
-        const float neg_m = (m_use == -INFINITY) ? 0.f : -m_use;
-        if (j > 0 && __any_sync(0xffffffffu, grow)) {
-          // S_t(j) ready proves P_t.V_{j-1} completed (same issue order as the single-CTA kernel); P_t.V_j cannot
-          // start before the arrives below (it needs all 8 warps of both CTAs), so this CTA's O_t lanes are quiescent
-#pragma unroll 1
-          for (int c0 = 0; c0 < 128; c0 += 32) {
-            uint32_t o[32];
-            B2F_TMEM_LD_X32(o_tmem + c0, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int c = 0; c < 32; ++c) o[c] = __float_as_uint(__uint_as_float(o[c]) * alpha);
-            B2F_TMEM_ST_X32(o_tmem + c0, o);
-          }
-        }
-        float sum4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          uint32_t pk[32];
-#pragma unroll
-          for (int c = 0; c < 32; ++c) {
-            float x0, x1;
-            ffma2(x0, x1, __uint_as_float(sr[half * 64 + 2 * c]), __uint_as_float(sr[half * 64 + 2 * c + 1]),
-                  p.scale_log2, p.scale_log2, neg_m, neg_m);
-            float p0, p1;
-            if (POLY && (c % (POLY ? POLY : 1)) == (POLY ? POLY : 1) - 1) {
-              ex2_poly2(x0, x1, p0, p1);
-            } else {
-              p0 = ex2(x0);
-              p1 = ex2(x1);
-            }
-            const int a = (c & 1) * 2;
-            fadd2(sum4[a], sum4[a + 1], sum4[a], sum4[a + 1], p0, p1);
-            pk[c] = pack_bf16x2(p0, p1);
-          }
-          B2F_TMEM_ST_X32(s_tmem + half * 32, pk);
-          tmem_wait_st();
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive_cta0(&p_full[t * 2 + half]);   // the issuer's barrier (remote from CTA 1)
-        }
-        l = l * alpha + ((sum4[0] + sum4[1]) + (sum4[2] + sum4[3]));
-        m = m_use;
-      }
-      mbar_wait(&o_done[t], 0);
-      tc_fence_after();
-      const float inv_l = 1.0f / l;
-      const bool row_ok = q_row < p.Sq;
-      if (p.lse && row_ok) p.lse[((long long)b * p.H + h) * p.lse_stride + q_row] = m + log2f(l);
-      __nv_bfloat16* out_row = p.out + ((long long)b * p.Sq + q_row) * p.ldo + (long long)h * DH;
-#pragma unroll 1
-      for (int c0 = 0; c0 < 128; c0 += 32) {
-        uint32_t o[32];
-        __syncwarp();
-        B2F_TMEM_LD_X32(o_tmem + c0, o);
-        tmem_wait_ld();
-        if (row_ok) {
-#pragma unroll
-          for (int g = 0; g < 4; ++g) {
-            uint4 v;
-            v.x = pack_bf16x2(__uint_as_float(o[g * 8 + 0]) * inv_l, __uint_as_float(o[g * 8 + 1]) * inv_l);
-            v.y = pack_bf16x2(__uint_as_float(o[g * 8 + 2]) * inv_l, __uint_as_float(o[g * 8 + 3]) * inv_l);
-            v.z = pack_bf16x2(__uint_as_float(o[g * 8 + 4]) * inv_l, __uint_as_float(o[g * 8 + 5]) * inv_l);
-            v.w = pack_bf16x2(__uint_as_float(o[g * 8 + 6]) * inv_l, __uint_as_float(o[g * 8 + 7]) * inv_l);
-            *reinterpret_cast<uint4*>(out_row + c0 + g * 8) = v;
-          }
-        }
-      }
-    }
-  }
+    return;
   }
 
-  tc_fence_before();
-  cluster_sync_all();   // both CTAs are done with each other's barriers / smem halves / TMEM
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2cta(tmem_base, 512);
+  // ------------------------------------------------------------------ consumer warpgroups
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
+  const int c = wg - 1;
+  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int row0 = q0 + c * 64 + w * 16 + (lane >> 2);   // this thread's rows: row0 and row0 + 8
+  const int colq = 2 * (lane & 3);                       // first of its two columns in every 8-column group
+  const uint64_t dq0 = make_sdesc_sw128(smem_u32(q_smem) + c * 8192, 16, 1024);
+  const uint64_t dk0 = make_sdesc_sw128(smem_u32(k_smem), 16, 1024);
+  const uint64_t dv0 = make_sdesc_sw128(smem_u32(v_smem), HALF_BYTES, 1024);
+  float o[64];
+#pragma unroll
+  for (int i = 0; i < 64; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // l: this thread's partial row sums
+  mbar_wait(q_full, 0);
+  for (int j = 0; j < n_kv; ++j) {
+    const int slot = j % KV_SLOTS;
+    const uint32_t phase = (j / KV_SLOTS) & 1;
+    float s[64];
+    mbar_wait(&k_full[slot], phase);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < DH / 16; ++k) {
+      const uint64_t off = uint64_t(((k >> 2) * HALF_BYTES + (k & 3) * 32) >> 4);
+      wgmma_m64n128_ss<0, 0>(s, dq0 + off, dk0 + uint64_t((slot * TILE_BYTES) >> 4) + off, k != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(s);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&k_empty[slot]);
+
+    const int kv0 = j * BKV;
+    if (BIAS) {
+#pragma unroll
+      for (int i = 0; i < 64; ++i) {
+        const int row = row0 + 8 * ((i >> 1) & 1);
+        const int col = kv0 + 8 * (i >> 2) + colq + (i & 1);
+        if (row < p.Sq && col < p.Skv)
+          s[i] = fmaf(s[i], p.bias_scale,
+                      __bfloat162float(p.bias[(long long)h * p.bias_h_stride + (long long)row * p.bias_row_stride + col]));
+      }
+    }
+    if (kv0 + BKV > p.Skv || p.causal) {
+#pragma unroll
+      for (int i = 0; i < 64; ++i) {
+        const int row = row0 + 8 * ((i >> 1) & 1);
+        const int col = kv0 + 8 * (i >> 2) + colq + (i & 1);
+        const int limit = p.causal ? min(p.Skv, row + 1) : p.Skv;
+        if (col >= limit) s[i] = -INFINITY;
+      }
+    }
+    float alpha[2], neg_m[2];
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int i = 0; i < 64; ++i)
+        if (((i >> 1) & 1) == r) mx = fmaxf(mx, s[i]);
+      mx = quad_max(mx);
+      const float m_new = fmaxf(m[r], mx * p.scale_log2);
+      alpha[r] = m[r] == -INFINITY ? 0.f : ex2(m[r] - m_new);
+      neg_m[r] = m_new == -INFINITY ? 0.f : -m_new;   // fully masked row so far
+      m[r] = m_new;
+    }
+    float sum[2] = {0.f, 0.f};
+#pragma unroll
+    for (int i = 0; i < 64; ++i) {
+      const int r = (i >> 1) & 1;
+      s[i] = ex2(fmaf(s[i], p.scale_log2, neg_m[r]));
+      sum[r] += s[i];
+    }
+#pragma unroll
+    for (int r = 0; r < 2; ++r) l[r] = l[r] * alpha[r] + sum[r];
+#pragma unroll
+    for (int i = 0; i < 64; ++i) o[i] *= alpha[(i >> 1) & 1];
+
+    uint32_t pa[BKV / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk) pack_a_frag(s, kk, pa[kk]);
+    mbar_wait(&v_full[slot], phase);
+    reg_fence(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BKV / 16; ++kk)
+      wgmma_m64n128_rs<1>(o, pa[kk], dv0 + uint64_t((slot * TILE_BYTES + kk * 2048) >> 4), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(o);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&v_empty[slot]);
+  }
+
+  // ---------------------------------------------------------------- epilogue: O / l -> bf16
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const int row = row0 + 8 * r;
+    const float lt = quad_sum(l[r]);
+    const float inv_l = 1.0f / lt;
+    if (row >= p.Sq) continue;
+    if (p.lse && (lane & 3) == 0) p.lse[((long long)b * p.H + h) * p.lse_stride + row] = m[r] + log2f(lt);
+    __nv_bfloat16* out_row = p.out + ((long long)b * p.Sq + row) * p.ldo + (long long)h * DH;
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      const int i = 4 * jj + 2 * r;
+      *reinterpret_cast<uint32_t*>(out_row + 8 * jj + colq) = pack_bf16x2(o[i] * inv_l, o[i + 1] * inv_l);
+    }
   }
 }
 
-template <int POLY>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(ATTN_THREADS, 1)
-attn_fwd_kernel_2cta(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                     const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
-  attn_pair_body<POLY, 0>(tmQ, tmK, tmV, p);
-}
-// light warpgroup + 8 softmax warps at 208 registers (3 warps per sub-partition: 80 + 2 x 208 <= 512)
-template <int POLY>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(P2_THREADS_NR, 1)
-attn_fwd_kernel_2cta_nr(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                        const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
-  attn_pair_body<POLY, 208>(tmQ, tmK, tmV, p);
-}
 }  // namespace
 
 static int attention_impl(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
@@ -759,78 +219,13 @@ static int attention_impl(const void* q, int64_t ldq, const void* k, int64_t ldk
   if ((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(k) |
        reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(out)) & 15)
     return B2F_ERR_ALIGN;
-  // kernel variant: B2F_ATTN_VARIANT selects at run time (tuning / experiments); resolved once
-  static Variant var = {nullptr, 0, 0, false};
-  if (!var.fn) {
-    const char* ev = getenv("B2F_ATTN_VARIANT");
-    const int variant = ev ? atoi(ev) : B2F_ATTN_DEFAULT_VARIANT;
-    Variant sel = {nullptr, ATTN_THREADS, ATTN_SMEM, false};
-    switch (variant) {
-      case 1: case 50: case 51: case 52: case 53: case 54: case 55: case 56: case 57: case 58: case 59:   // (50-59: what the CTA-pair kernel does not cover)
-        sel.fn = attn_fwd_kernel<4, false>; break;               // 25 % of the exponentials on the FMA pipe
-      case 2: sel.fn = attn_fwd_kernel<2, false>; break;         // 50 %
-      case 3: sel.fn = attn_fwd_kernel<0, true>; break;
-      case 4: sel.fn = attn_fwd_kernel<4, true>; break;
-      case 5: sel.fn = attn_fwd_kernel<3, false>; break;         // 33 %
-      case 6: sel.fn = attn_fwd_kernel<8, false>; break;         // 12.5 %
-      default:
-        if (!experimental_variant(variant, &sel)) sel.fn = attn_fwd_kernel<0, false>;
-        break;
-    }
-    cudaError_t e = cudaFuncSetAttribute(sel.fn, cudaFuncAttributeMaxDynamicSharedMemorySize, sel.smem);
+  static bool attr_set = false;
+  if (!attr_set) {
+    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM);
     if (e != cudaSuccess) return cuda_err(e, "attention smem attribute");
-    e = cudaFuncSetAttribute(attn_fwd_kernel<0, false, 0, true>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             ATTN_SMEM);
+    e = cudaFuncSetAttribute(attn_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM);
     if (e != cudaSuccess) return cuda_err(e, "attention smem attribute");
-    var = sel;
-  }
-  // CTA-pair kernel (B2F_ATTN_VARIANT 50 / 51 / 52): non-causal, no bias, at least one full 512-row pair
-  static const int pair_variant = [] {
-    const char* v = getenv("B2F_ATTN_VARIANT");
-    const int variant = v ? atoi(v) : B2F_ATTN_DEFAULT_VARIANT;
-    return (variant >= 50 && variant <= 59) ? variant : -1;
-  }();
-  if (pair_variant >= 0 && !causal && !bias && Sq >= 4 * BQ) {
-    static KernelFn pk = nullptr;
-    static int pk_threads = ATTN_THREADS, pk_rows = 4 * BQ, pk_smem = P2_SMEM;
-    if (!pk) {
-      switch (pair_variant) {
-        case 50: pk = attn_fwd_kernel_2cta<0>; break;
-        case 52: pk = attn_fwd_kernel_2cta<2>; break;
-        case 51: pk = attn_fwd_kernel_2cta<4>; break;
-        case 53: pk = attn_fwd_kernel_2cta_nr<4>; pk_threads = P2_THREADS_NR; break;
-        case 56: pk = attn_fwd_kernel_2cta_nr<0>; pk_threads = P2_THREADS_NR; break;
-        default: pk = attn_fwd_kernel_2cta_nr<3>; pk_threads = P2_THREADS_NR; break;   // 54
-      }
-      cudaError_t e = cudaFuncSetAttribute(pk, cudaFuncAttributeMaxDynamicSharedMemorySize, pk_smem);
-      if (e != cudaSuccess) return cuda_err(e, "attention pair smem attribute");
-    }
-    CUtensorMap tQ, tK, tV;
-    int r2 = make_tmap_3d_rows(&tQ, q, (uint64_t)H * DH, Sq, B, ldq, (uint64_t)Sq * ldq);
-    if (r2) return r2;
-    r2 = make_tmap_3d_rows(&tK, k, (uint64_t)Hkv * DH, Skv, B, ldk, (uint64_t)Skv * ldk, 64);   // 64-row K halves
-    if (r2) return r2;
-    r2 = make_tmap_3d_rows(&tV, v, (uint64_t)Hkv * DH, Skv, B, ldv, (uint64_t)Skv * ldv);
-    if (r2) return r2;
-    AttnParams pp{};
-    pp.B = B;
-    pp.H = H;
-    pp.Hkv = Hkv;
-    pp.Sq = Sq;
-    pp.Skv = Skv;
-    pp.scale_log2 = scale * 1.4426950408889634f;
-    pp.causal = 0;
-    pp.out = static_cast<__nv_bfloat16*>(out);
-    pp.ldo = ldo;
-    pp.lse = lse;
-    pp.lse_stride = lse_stride;
-    dim3 grid_p(2 * ((Sq + pk_rows - 1) / pk_rows), H, B);
-    prof_begin(KC_ATTN, stream);
-    pk<<<grid_p, pk_threads, pk_smem, stream>>>(tQ, tK, tV, pp);
-    prof_end(KC_ATTN, stream, 4.0 * B * H * (double)Sq * Skv * DH, 2.0 * DH * B * (2.0 * H * Sq + 2.0 * Hkv * Skv));
-    g_launch_count.fetch_add(1, std::memory_order_relaxed);
-    B2F_CHECK_LAUNCH("attn_fwd_kernel_2cta");
-    return B2F_OK;
+    attr_set = true;
   }
   CUtensorMap tmQ, tmK, tmV;
   int rc = make_tmap_3d_rows(&tmQ, q, (uint64_t)H * DH, Sq, B, ldq, (uint64_t)Sq * ldq);
@@ -858,18 +253,18 @@ static int attention_impl(const void* q, int64_t ldq, const void* k, int64_t ldk
     p.bias_row_stride = bias_row_stride;
     p.bias_scale = scale;
     p.scale_log2 = 1.4426950408889634f;
-    dim3 grid_b((Sq + 2 * BQ - 1) / (2 * BQ), H, B);
+    dim3 grid_b((Sq + BQ - 1) / BQ, H, B);
     prof_begin(KC_ATTN, stream);
-    attn_fwd_kernel<0, false, 0, true><<<grid_b, ATTN_THREADS, ATTN_SMEM, stream>>>(tmQ, tmK, tmV, p);
+    attn_fwd_kernel<true><<<grid_b, ATTN_THREADS, ATTN_SMEM, stream>>>(tmQ, tmK, tmV, p);
     prof_end(KC_ATTN, stream, (causal ? 2.0 : 4.0) * B * H * (double)Sq * Skv * DH,
              2.0 * DH * B * (2.0 * H * Sq + 2.0 * Hkv * Skv) + 2.0 * H * (double)Sq * Skv);
     g_launch_count.fetch_add(1, std::memory_order_relaxed);
     B2F_CHECK_LAUNCH("attn_fwd_kernel<bias>");
     return B2F_OK;
   }
-  dim3 grid(var.single_tile ? (Sq + BQ - 1) / BQ : (Sq + 2 * BQ - 1) / (2 * BQ), H, B);
+  dim3 grid((Sq + BQ - 1) / BQ, H, B);
   prof_begin(KC_ATTN, stream);
-  var.fn<<<grid, var.threads, var.smem, stream>>>(tmQ, tmK, tmV, p);
+  attn_fwd_kernel<false><<<grid, ATTN_THREADS, ATTN_SMEM, stream>>>(tmQ, tmK, tmV, p);
   prof_end(KC_ATTN, stream, (causal ? 2.0 : 4.0) * B * H * (double)Sq * Skv * DH,
            2.0 * DH * B * (2.0 * H * Sq + 2.0 * Hkv * Skv));
   g_launch_count.fetch_add(1, std::memory_order_relaxed);

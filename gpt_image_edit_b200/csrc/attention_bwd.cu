@@ -1,23 +1,23 @@
-// Backward of the fused softmax attention (head_dim 128, non-causal, H == Hkv: the FLUX joint attention) for sm_100a.
+// Backward of the fused softmax attention (head_dim 128, non-causal, H == Hkv: the FLUX joint attention) for sm_90a.
 //
 // Given Q, K, V, dO, the forward's base-2 log-sum-exp rows lse2[b,h,q] and delta[b,h,q] = rowsum(dO * O):
 //   P  = exp2(scale_log2 * Q K^T - lse2)          (the normalised probabilities, recomputed, never stored)
 //   dP = dO V^T;   dS = P * (dP - delta)
 //   dV = P^T dO;   dK = scale * dS^T Q;   dQ = scale * dS K
 // Two launches of one kernel template, both free of atomics (deterministic):
-//   MODE 0 (dK, dV): a CTA owns 128 K/V rows of one (batch, head) and streams Q / dO tiles;  everything is
-//                    held TRANSPOSED (rows = kv, columns = q) so that P^T and dS^T land in TMEM as the A operands
-//                    of the two accumulating MMAs;
-//   MODE 1 (dQ):     a CTA owns 128 query rows and streams K / V tiles.
-// Per 128 x 128 block:   S~  = X0 . Y0^T   (SS)      X = stationary tiles, Y = streamed tiles
-//                        dP~ = X1 . Y1^T   (SS)      MODE 0: X = (K, V), Y = (Q, dO);  MODE 1: X = (Q, dO), Y = (K, V)
-//                        P~, dS~ -> bf16 over S~ / dP~ in TMEM (tcgen05.st), one thread per row
-//                        G1 += P~ . Y1     (TS, MODE 0 only: dV)     Y tiles re-read as MN-major B operands
-//                        G0 += dS~ . Y0    (TS: dK or dQ)
-// TMEM (512 columns): S~ | P~ [0,128)   dP~ | dS~ [128,256)   G0 [256,384)   G1 [384,512).
-//   warp 0 (1 lane)  TMA producer: X tiles once, (Y0, Y1, lse2, delta) through a 2-stage ring
-//   warp 1           tcgen05.mma issuer (warp-uniform loop, one elected lane issues)
-//   warps 2..5       one thread per row of the block: tcgen05.ld S~ and dP~, exp2, tcgen05.st P~ and dS~
+//   MODE 0 (dK, dV): a CTA owns 128 K/V rows of one (batch, head) and streams Q / dO blocks; everything is held
+//                    TRANSPOSED (rows = kv, columns = q) so that P^T and dS^T are the register A operands of the two
+//                    accumulating MMAs;
+//   MODE 1 (dQ):     a CTA owns 128 query rows and streams K / V blocks.
+// X = the stationary tiles, Y = the streamed 64-row blocks; MODE 0: X = (K, V), Y = (Q, dO);  MODE 1: X = (Q, dO),
+// Y = (K, V).  Per block and consumer warpgroup (64 stationary rows):
+//                        S~  = X0 . Y0^T   (wgmma, smem x smem, 64 x 64 in registers)
+//                        dP~ = X1 . Y1^T
+//                        P~, dS~ -> bf16 register fragments
+//                        G1 += P~ . Y1     (MODE 0 only: dV)     Y blocks re-read as MN-major B operands
+//                        G0 += dS~ . Y0    (dK or dQ)
+//   warpgroup 0 (1 lane)   TMA producer: X tiles once, (Y0, Y1, lse2, delta) through a 2-stage ring
+//   warpgroups 1, 2        consumers, 64 stationary rows each; G0 / G1 accumulate in registers
 //
 // Replaces the autograd of F.scaled_dot_product_attention / flash_attn backward reached by
 // accelerator.backward(loss) in the reference (train_denoiser.py:1172) for every FLUX block.
@@ -34,10 +34,13 @@ using namespace attn;
 
 namespace {
 
-constexpr int BWD_THREADS = 192;
+constexpr int BWD_THREADS = 384;
 constexpr int BWD_STAGES = 2;
-constexpr int BWD_VEC_BYTES = 128 * 4;   // one 128-entry fp32 row of lse2 / delta
-constexpr int BWD_SMEM = (2 + 2 * BWD_STAGES) * TILE_BYTES + BWD_STAGES * 2 * BWD_VEC_BYTES + 256 + 1024;
+constexpr int BS = 64;                          // streamed rows per block
+constexpr int Y_BYTES = BS * DH * 2;            // 16 KB: two [64][64] swizzled halves
+constexpr int Y_HALF = Y_BYTES / 2;
+constexpr int BWD_VEC_FLOATS = 2 * BS;          // lse2[64], delta[64] of one stage
+constexpr int BWD_SMEM = 2 * TILE_BYTES + BWD_STAGES * 2 * Y_BYTES + BWD_STAGES * BWD_VEC_FLOATS * 4 + 256 + 1024;
 
 struct AttnBwdParams {
   int B, H, S, S_pad;
@@ -51,266 +54,181 @@ struct AttnBwdParams {
 
 template <int MODE>
 __global__ void __launch_bounds__(BWD_THREADS, 1)
-attn_bwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                const __grid_constant__ CUtensorMap tmV, const __grid_constant__ CUtensorMap tmdO,
+attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_constant__ CUtensorMap tmX1,
+                const __grid_constant__ CUtensorMap tmY0, const __grid_constant__ CUtensorMap tmY1,
                 const AttnBwdParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* x_smem = smem;                                  // X0, X1
   uint8_t* y_smem = smem + 2 * TILE_BYTES;                 // per stage: Y0, Y1
-  float* vec_smem = reinterpret_cast<float*>(smem + (2 + 2 * BWD_STAGES) * TILE_BYTES);   // per stage: lse2[128], delta[128]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (2 + 2 * BWD_STAGES) * TILE_BYTES + BWD_STAGES * 2 * BWD_VEC_BYTES);
+  float* vec_smem = reinterpret_cast<float*>(y_smem + BWD_STAGES * 2 * Y_BYTES);   // per stage: lse2[64], delta[64]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(vec_smem + BWD_STAGES * BWD_VEC_FLOATS);
   uint64_t* x_full = bars;                   // 1
   uint64_t* y_full = bars + 1;               // BWD_STAGES
   uint64_t* y_empty = y_full + BWD_STAGES;   // BWD_STAGES
-  uint64_t* s_full = y_empty + BWD_STAGES;   // 1
-  uint64_t* p_ready = s_full + 1;            // 1 (4 arrives)
-  uint64_t* acc_done = p_ready + 1;          // 1
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_done + 1);
 
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const int blk = blockIdx.x, h = blockIdx.y, b = blockIdx.z;
-  const int row0 = blk * 128;                    // first stationary row (kv in MODE 0, q in MODE 1)
-  const int n_it = (p.S + 127) / 128;            // streamed blocks
-  const CUtensorMap* tmX0 = MODE == 0 ? &tmK : &tmQ;
-  const CUtensorMap* tmX1 = MODE == 0 ? &tmV : &tmdO;
-  const CUtensorMap* tmY0 = MODE == 0 ? &tmQ : &tmK;
-  const CUtensorMap* tmY1 = MODE == 0 ? &tmdO : &tmV;
+  const int wg = __shfl_sync(0xffffffffu, int(threadIdx.x >> 7), 0);   // warp-uniform for the compiler
+  const int h = blockIdx.y, b = blockIdx.z;
+  const int row0_cta = blockIdx.x * 128;         // first stationary row (kv in MODE 0, q in MODE 1)
+  const int n_it = (p.S + BS - 1) / BS;          // streamed blocks
 
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(&tmQ);
-    tma_prefetch_desc(&tmK);
-    tma_prefetch_desc(&tmV);
-    tma_prefetch_desc(&tmdO);
-  }
-  if (warp == 1 && lane == 0) {
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmX0);
+    tma_prefetch_desc(&tmX1);
+    tma_prefetch_desc(&tmY0);
+    tma_prefetch_desc(&tmY1);
     mbar_init(x_full, 1);
     for (int i = 0; i < BWD_STAGES; ++i) {
       mbar_init(&y_full[i], 1);
-      // a stage is free when its MMAs have completed (one tcgen05.commit) AND the four row warps have finished reading
-      // the lse2 / delta vectors staged with it (MODE 0; they arrive in MODE 1 as well to keep one protocol)
-      mbar_init(&y_empty[i], 5);
+      mbar_init(&y_empty[i], 8);   // one arrive per consumer warp: its MMAs and its reads of lse2 / delta are done
     }
-    mbar_init(s_full, 1);
-    mbar_init(p_ready, 4);
-    mbar_init(acc_done, 1);
     fence_mbar_init();
   }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr, 512);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
+    if (threadIdx.x == 0) {
       // ---------------------------------------------------------------- TMA producer
       mbar_expect_tx(x_full, 2 * TILE_BYTES);
       for (int half = 0; half < 2; ++half) {
-        tma_load_3d(x_smem + half * (TILE_BYTES / 2), tmX0, x_full, h * DH + half * 64, row0, b);
-        tma_load_3d(x_smem + TILE_BYTES + half * (TILE_BYTES / 2), tmX1, x_full, h * DH + half * 64, row0, b);
+        tma_load_3d(x_smem + half * HALF_BYTES, &tmX0, x_full, h * DH + half * 64, row0_cta, b);
+        tma_load_3d(x_smem + TILE_BYTES + half * HALF_BYTES, &tmX1, x_full, h * DH + half * 64, row0_cta, b);
       }
-      int stage = 0;
-      uint32_t phase = 0;
       const float* lse_row = p.lse + ((long long)b * p.H + h) * p.S_pad;
       const float* dl_row = p.delta + ((long long)b * p.H + h) * p.S_pad;
       for (int i = 0; i < n_it; ++i) {
-        mbar_wait(&y_empty[stage], phase ^ 1);
-        uint8_t* y0 = y_smem + stage * 2 * TILE_BYTES;
-        uint8_t* y1 = y0 + TILE_BYTES;
-        mbar_expect_tx(&y_full[stage], 2 * TILE_BYTES + (MODE == 0 ? 2 * BWD_VEC_BYTES : 0));
+        const int stage = i % BWD_STAGES;
+        mbar_wait(&y_empty[stage], ((i / BWD_STAGES) & 1) ^ 1);
+        uint8_t* y0 = y_smem + stage * 2 * Y_BYTES;
+        uint8_t* y1 = y0 + Y_BYTES;
+        mbar_expect_tx(&y_full[stage], 2 * Y_BYTES + (MODE == 0 ? BWD_VEC_FLOATS * 4 : 0));
         for (int half = 0; half < 2; ++half) {
-          tma_load_3d(y0 + half * (TILE_BYTES / 2), tmY0, &y_full[stage], h * DH + half * 64, i * 128, b);
-          tma_load_3d(y1 + half * (TILE_BYTES / 2), tmY1, &y_full[stage], h * DH + half * 64, i * 128, b);
+          tma_load_3d(y0 + half * Y_HALF, &tmY0, &y_full[stage], h * DH + half * 64, i * BS, b);
+          tma_load_3d(y1 + half * Y_HALF, &tmY1, &y_full[stage], h * DH + half * 64, i * BS, b);
         }
         if (MODE == 0) {
-          // the streamed index is the query index: its lse2 / delta rows ride along with the tiles
-          bulk_load_1d(vec_smem + stage * 256, lse_row + i * 128, BWD_VEC_BYTES, &y_full[stage]);
-          bulk_load_1d(vec_smem + stage * 256 + 128, dl_row + i * 128, BWD_VEC_BYTES, &y_full[stage]);
-        }
-        if (++stage == BWD_STAGES) {
-          stage = 0;
-          phase ^= 1;
+          // the streamed index is the query index: its lse2 / delta rows ride along with the blocks
+          bulk_load_1d(vec_smem + stage * BWD_VEC_FLOATS, lse_row + i * BS, BS * 4, &y_full[stage]);
+          bulk_load_1d(vec_smem + stage * BWD_VEC_FLOATS + BS, dl_row + i * BS, BS * 4, &y_full[stage]);
         }
       }
     }
-  } else if (warp == 1) {
-    // ---------------------------------------------------------------- MMA issuer (warp-uniform loop)
-    constexpr uint32_t idesc_ss = make_idesc_bf16(128, 128, 0);   // both operands K-major over head_dim
-    constexpr uint32_t idesc_ts = make_idesc_bf16(128, DH, 1);    // A from TMEM, B = streamed tile MN-major
-    const uint64_t dx_base = make_sdesc_sw128(smem_u32(x_smem), 16, 1024);
-    const uint64_t dyk_base = make_sdesc_sw128(smem_u32(y_smem), 16, 1024);               // K-major view
-    const uint64_t dym_base = make_sdesc_sw128(smem_u32(y_smem), TILE_BYTES / 2, 1024);   // MN-major view
-    const uint32_t t_s = tmem_base, t_dp = tmem_base + 128, t_g0 = tmem_base + 256, t_g1 = tmem_base + 384;
-    int stage = 0;
-    uint32_t phase = 0;
-    mbar_wait(x_full, 0);
-    for (int i = 0; i < n_it; ++i) {
-      mbar_wait(&y_full[stage], phase);
-      tc_fence_after();
-      const uint32_t y_off = uint32_t(stage * 2 * TILE_BYTES);
-      if (elect_one()) {
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k) {
-          const uint64_t off = uint64_t(((k >> 2) * (TILE_BYTES / 2) + (k & 3) * 32) >> 4);
-          umma_ss(t_s, dx_base + off, dyk_base + uint64_t(y_off >> 4) + off, idesc_ss, k != 0 ? 1u : 0u);
-        }
-#pragma unroll
-        for (int k = 0; k < DH / 16; ++k) {
-          const uint64_t off = uint64_t(((k >> 2) * (TILE_BYTES / 2) + (k & 3) * 32) >> 4);
-          umma_ss(t_dp, dx_base + uint64_t(TILE_BYTES >> 4) + off, dyk_base + uint64_t((y_off + TILE_BYTES) >> 4) + off,
-                  idesc_ss, k != 0 ? 1u : 0u);
-        }
-        umma_commit(s_full);
-      }
-      __syncwarp();
-      mbar_wait(p_ready, i & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        if (MODE == 0) {
-          // dV += P~ . dO      (A = P~ bf16 in the S region, B = Y1 as [N = dh, K = q rows])
-#pragma unroll
-          for (int k = 0; k < 8; ++k)
-            umma_ts(t_g1, t_s + k * 8, dym_base + uint64_t((y_off + TILE_BYTES + k * 2048) >> 4), idesc_ts,
-                    (i | k) != 0 ? 1u : 0u);
-        }
-        // dK / dQ += dS~ . Y0
-#pragma unroll
-        for (int k = 0; k < 8; ++k)
-          umma_ts(t_g0, t_dp + k * 8, dym_base + uint64_t((y_off + k * 2048) >> 4), idesc_ts, (i | k) != 0 ? 1u : 0u);
-        umma_commit(&y_empty[stage]);
-        if (i == n_it - 1) umma_commit(acc_done);
-      }
-      __syncwarp();
-      if (++stage == BWD_STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
-    }
-  } else {
-    // ---------------------------------------------------------------- one thread per stationary row
-    const int quarter = warp & 3;
-    const int row_in = quarter * 32 + lane;
-    const int row = row0 + row_in;
-    const bool row_ok = row < p.S;
-    const uint32_t lane_addr = uint32_t(quarter * 32) << 16;
-    const uint32_t t_s = tmem_base + lane_addr, t_dp = t_s + 128;
-    float my_lse = __int_as_float(0x7f800000), my_delta = 0.f;
-    if (MODE == 1 && row_ok) {
-      my_lse = p.lse[((long long)b * p.H + h) * p.S_pad + row];
-      my_delta = p.delta[((long long)b * p.H + h) * p.S_pad + row];
-    }
-    int stage = 0;
-    uint32_t phase = 0;
-    for (int i = 0; i < n_it; ++i) {
-      mbar_wait(&y_full[stage], phase);      // makes the staged lse2 / delta rows visible to this thread
-      mbar_wait(s_full, i & 1);
-      tc_fence_after();
-      const float* lse_s = vec_smem + stage * 256;
-      const float* dl_s = lse_s + 128;
-      const int col0 = i * 128;
-      // A warp reads TMEM at ~40 B/clk and its loads do not overlap each other (scripts/debug/ldtm_bw.cu): the two
-      // 32-column loads of chunk c + 1 are issued before the (MUFU-bound) arithmetic of chunk c, two register sets.
-      uint32_t sr[2][32], dr[2][32];
-      B2F_TMEM_LD_X32(t_s, sr[0]);
-      B2F_TMEM_LD_X32(t_dp, dr[0]);
-#pragma unroll
-      for (int ch = 0; ch < 4; ++ch) {
-        const int c0 = ch * 32;
-        uint32_t* sc = sr[ch & 1];
-        uint32_t* dc = dr[ch & 1];
-        tmem_wait_ld();
-        if (ch < 3) {
-          B2F_TMEM_LD_X32(t_s + c0 + 32, sr[(ch + 1) & 1]);
-          B2F_TMEM_LD_X32(t_dp + c0 + 32, dr[(ch + 1) & 1]);
-        }
-        B2F_TIE16(sc);       // after the loads of the next chunk: the arithmetic below cannot be scheduled above them
-        B2F_TIE16(sc + 16);
-        B2F_TIE16(dc);
-        B2F_TIE16(dc + 16);
-        uint32_t pk[16], dk[16];
-#pragma unroll
-        for (int j = 0; j < 32; j += 2) {
-          float l0, l1, d0, d1;
-          if (MODE == 0) {
-            l0 = lse_s[c0 + j];
-            l1 = lse_s[c0 + j + 1];
-            d0 = dl_s[c0 + j];
-            d1 = dl_s[c0 + j + 1];
-          } else {
-            l0 = l1 = my_lse;
-            d0 = d1 = my_delta;
-          }
-          float p0 = ex2(fmaf(__uint_as_float(sc[j]), p.scale_log2, -l0));
-          float p1 = ex2(fmaf(__uint_as_float(sc[j + 1]), p.scale_log2, -l1));
-          if (MODE == 0) {
-            if (!row_ok) p0 = p1 = 0.f;                       // K/V rows beyond the sequence (zero-filled tiles)
-          } else {
-            if (col0 + c0 + j >= p.S) p0 = 0.f;               // K/V columns beyond the sequence
-            if (col0 + c0 + j + 1 >= p.S) p1 = 0.f;
-          }
-          const float s0 = p0 * (__uint_as_float(dc[j]) - d0);
-          const float s1 = p1 * (__uint_as_float(dc[j + 1]) - d1);
-          pk[j >> 1] = pack_bf16x2(p0, p1);
-          dk[j >> 1] = pack_bf16x2(s0, s1);
-        }
-        // bf16 pairs over the fp32 columns already consumed: columns [c0/2, c0/2 + 16) end at or before c0 + 32, the first
-        // column of the chunk in flight
-        if (MODE == 0) B2F_TMEM_ST_X16(t_s + (c0 >> 1), pk);
-        B2F_TMEM_ST_X16(t_dp + (c0 >> 1), dk);
-      }
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(&y_empty[stage]);     // this warp's generic-proxy reads of the stage's smem are done
-        mbar_arrive(p_ready);
-      }
-      if (++stage == BWD_STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
-    }
-    // ---------------------------------------------------------------- epilogue: accumulators -> bf16 -> global
-    mbar_wait(acc_done, 0);
-    tc_fence_after();
-#pragma unroll 1
-    for (int g = 0; g < (MODE == 0 ? 2 : 1); ++g) {
-      __nv_bfloat16* base = g == 0 ? p.g0 : p.g1;
-      const long long ld = g == 0 ? p.ld0 : p.ld1;
-      const float mul = g == 0 ? p.scale : 1.0f;
-      __nv_bfloat16* out_row = base + ((long long)b * p.S + row) * ld + (long long)h * DH;
-      const uint32_t t_g = tmem_base + lane_addr + 256 + uint32_t(g * 128);
-#pragma unroll 1
-      for (int c0 = 0; c0 < 128; c0 += 32) {
-        uint32_t o[32];
-        __syncwarp();
-        B2F_TMEM_LD_X32(t_g + c0, o);
-        tmem_wait_ld();
-        if (row_ok) {
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            uint4 v;
-            v.x = pack_bf16x2(__uint_as_float(o[q * 8 + 0]) * mul, __uint_as_float(o[q * 8 + 1]) * mul);
-            v.y = pack_bf16x2(__uint_as_float(o[q * 8 + 2]) * mul, __uint_as_float(o[q * 8 + 3]) * mul);
-            v.z = pack_bf16x2(__uint_as_float(o[q * 8 + 4]) * mul, __uint_as_float(o[q * 8 + 5]) * mul);
-            v.w = pack_bf16x2(__uint_as_float(o[q * 8 + 6]) * mul, __uint_as_float(o[q * 8 + 7]) * mul);
-            *reinterpret_cast<uint4*>(out_row + c0 + q * 8) = v;
-          }
-        }
-      }
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512);
+  // ------------------------------------------------------------------ consumer warpgroups
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
+  const int c = wg - 1;
+  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
+  const int row0 = row0_cta + c * 64 + w * 16 + (lane >> 2);   // this thread's stationary rows: row0, row0 + 8
+  const int colq = 2 * (lane & 3);
+  const uint64_t dx0 = make_sdesc_sw128(smem_u32(x_smem) + c * 8192, 16, 1024);
+  const uint64_t dx1 = dx0 + uint64_t(TILE_BYTES >> 4);
+  const uint64_t dyk = make_sdesc_sw128(smem_u32(y_smem), 16, 1024);        // K-major view of a Y block
+  const uint64_t dym = make_sdesc_sw128(smem_u32(y_smem), Y_HALF, 1024);    // MN-major view
+  float my_lse[2] = {0.f, 0.f}, my_delta[2] = {0.f, 0.f};
+  if (MODE == 1) {
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      // rows beyond S read the padding (lse = +inf, delta = 0): P = 0 there
+      my_lse[r] = p.lse[((long long)b * p.H + h) * p.S_pad + row0 + 8 * r];
+      my_delta[r] = p.delta[((long long)b * p.H + h) * p.S_pad + row0 + 8 * r];
+    }
+  }
+  float g0[64], g1[64];   // g1 (dV) is used in MODE 0 only; the compiler drops it from MODE 1
+#pragma unroll
+  for (int i = 0; i < 64; ++i) g0[i] = g1[i] = 0.f;
+  mbar_wait(x_full, 0);
+  for (int it = 0; it < n_it; ++it) {
+    const int stage = it % BWD_STAGES;
+    mbar_wait(&y_full[stage], (it / BWD_STAGES) & 1);
+    const uint64_t y0_off = uint64_t((stage * 2 * Y_BYTES) >> 4), y1_off = uint64_t((stage * 2 * Y_BYTES + Y_BYTES) >> 4);
+    float st[32], dpt[32];
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < DH / 16; ++k) {
+      const uint32_t xo = (k >> 2) * HALF_BYTES + (k & 3) * 32, yo = (k >> 2) * Y_HALF + (k & 3) * 32;
+      wgmma_m64n64_ss<0, 0>(st, dx0 + uint64_t(xo >> 4), dyk + y0_off + uint64_t(yo >> 4), k != 0 ? 1u : 0u);
+    }
+#pragma unroll
+    for (int k = 0; k < DH / 16; ++k) {
+      const uint32_t xo = (k >> 2) * HALF_BYTES + (k & 3) * 32, yo = (k >> 2) * Y_HALF + (k & 3) * 32;
+      wgmma_m64n64_ss<0, 0>(dpt, dx1 + uint64_t(xo >> 4), dyk + y1_off + uint64_t(yo >> 4), k != 0 ? 1u : 0u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(st);
+    reg_fence(dpt);
+    const float* lse_s = vec_smem + stage * BWD_VEC_FLOATS;
+    const float* dl_s = lse_s + BS;
+#pragma unroll
+    for (int i = 0; i < 32; ++i) {
+      const int r = (i >> 1) & 1;
+      const int lc = 8 * (i >> 2) + colq + (i & 1);   // streamed index inside the block
+      float l, d;
+      if (MODE == 0) {
+        l = lse_s[lc];
+        d = dl_s[lc];
+      } else {
+        l = my_lse[r];
+        d = my_delta[r];
+      }
+      float pv = ex2(fmaf(st[i], p.scale_log2, -l));
+      if (MODE == 0) {
+        if (row0 + 8 * r >= p.S) pv = 0.f;            // K/V rows beyond the sequence (zero-filled tiles)
+      } else {
+        if (it * BS + lc >= p.S) pv = 0.f;            // K/V columns beyond the sequence
+      }
+      st[i] = pv;
+      dpt[i] = pv * (dpt[i] - d);
+    }
+    uint32_t pf[BS / 16][4], df[BS / 16][4];
+#pragma unroll
+    for (int kk = 0; kk < BS / 16; ++kk) {
+      pack_a_frag(st, kk, pf[kk]);
+      pack_a_frag(dpt, kk, df[kk]);
+    }
+    reg_fence(g0);
+    if (MODE == 0) reg_fence(g1);
+    wgmma_fence();
+    if (MODE == 0) {
+      // dV += P~ . dO      (B = Y1 as [K = q rows, N = dh], MN-major)
+#pragma unroll
+      for (int kk = 0; kk < BS / 16; ++kk)
+        wgmma_m64n128_rs<1>(g1, pf[kk], dym + y1_off + uint64_t((kk * 2048) >> 4), 1u);
+    }
+    // dK / dQ += dS~ . Y0
+#pragma unroll
+    for (int kk = 0; kk < BS / 16; ++kk)
+      wgmma_m64n128_rs<1>(g0, df[kk], dym + y0_off + uint64_t((kk * 2048) >> 4), 1u);
+    wgmma_commit();
+    wgmma_wait<0>();
+    reg_fence(g0);
+    if (MODE == 0) reg_fence(g1);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&y_empty[stage]);
+  }
+
+  // ---------------------------------------------------------------- epilogue: accumulators -> bf16 -> global
+#pragma unroll
+  for (int g = 0; g < (MODE == 0 ? 2 : 1); ++g) {
+    __nv_bfloat16* base = g == 0 ? p.g0 : p.g1;
+    const long long ld = g == 0 ? p.ld0 : p.ld1;
+    const float mul = g == 0 ? p.scale : 1.0f;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      const int row = row0 + 8 * r;
+      if (row >= p.S) continue;
+      __nv_bfloat16* out_row = base + ((long long)b * p.S + row) * ld + (long long)h * DH;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        const int i = 4 * jj + 2 * r;
+        const float v0 = g == 0 ? g0[i] : g1[i];
+        const float v1 = g == 0 ? g0[i + 1] : g1[i + 1];
+        *reinterpret_cast<uint32_t*>(out_row + 8 * jj + colq) = pack_bf16x2(v0 * mul, v1 * mul);
+      }
+    }
   }
 }
 
@@ -339,15 +257,18 @@ int attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const 
     if (e != cudaSuccess) return cuda_err(e, "attention bwd smem attribute");
     attr_set = true;
   }
-  CUtensorMap tQ, tK, tV, tO;
-  int rc = make_tmap_3d_rows(&tQ, q, (uint64_t)H * DH, S, B, ldq, (uint64_t)S * ldq);
-  if (rc) return rc;
-  rc = make_tmap_3d_rows(&tK, k, (uint64_t)H * DH, S, B, ldk, (uint64_t)S * ldk);
-  if (rc) return rc;
-  rc = make_tmap_3d_rows(&tV, v, (uint64_t)H * DH, S, B, ldv, (uint64_t)S * ldv);
-  if (rc) return rc;
-  rc = make_tmap_3d_rows(&tO, dout, (uint64_t)H * DH, S, B, lddo, (uint64_t)S * lddo);
-  if (rc) return rc;
+  // every operand as a stationary tile (128-row boxes) and as a streamed block (64-row boxes)
+  CUtensorMap tQ, tK, tV, tO, sQ, sK, sV, sO;
+  const void* src[4] = {q, k, v, dout};
+  const int64_t lds[4] = {ldq, ldk, ldv, lddo};
+  CUtensorMap* tiles[4] = {&tQ, &tK, &tV, &tO};
+  CUtensorMap* blocks[4] = {&sQ, &sK, &sV, &sO};
+  for (int i = 0; i < 4; ++i) {
+    int rc = make_tmap_3d_rows(tiles[i], src[i], (uint64_t)H * DH, S, B, lds[i], (uint64_t)S * lds[i]);
+    if (rc) return rc;
+    rc = make_tmap_3d_rows(blocks[i], src[i], (uint64_t)H * DH, S, B, lds[i], (uint64_t)S * lds[i], BS);
+    if (rc) return rc;
+  }
   AttnBwdParams p{};
   p.B = B;
   p.H = H;
@@ -364,7 +285,7 @@ int attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const 
   p.g1 = static_cast<__nv_bfloat16*>(dv);
   p.ld1 = lddv;
   prof_begin(KC_ATTN, stream);
-  attn_bwd_kernel<0><<<grid, BWD_THREADS, BWD_SMEM, stream>>>(tQ, tK, tV, tO, p);
+  attn_bwd_kernel<0><<<grid, BWD_THREADS, BWD_SMEM, stream>>>(tK, tV, sQ, sO, p);
   prof_end(KC_ATTN, stream, 4.0 * unit, 2.0 * DH * B * H * 6.0 * S);
   g_launch_count.fetch_add(1, std::memory_order_relaxed);
   B2F_CHECK_LAUNCH("attn_bwd_kernel<dKdV>");
@@ -372,7 +293,7 @@ int attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const 
   p.ld0 = lddq;
   p.g1 = nullptr;
   prof_begin(KC_ATTN, stream);
-  attn_bwd_kernel<1><<<grid, BWD_THREADS, BWD_SMEM, stream>>>(tQ, tK, tV, tO, p);
+  attn_bwd_kernel<1><<<grid, BWD_THREADS, BWD_SMEM, stream>>>(tQ, tO, sK, sV, p);
   prof_end(KC_ATTN, stream, 3.0 * unit, 2.0 * DH * B * H * 5.0 * S);
   g_launch_count.fetch_add(1, std::memory_order_relaxed);
   B2F_CHECK_LAUNCH("attn_bwd_kernel<dQ>");

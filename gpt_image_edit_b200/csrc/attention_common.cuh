@@ -1,5 +1,5 @@
-// Shared definitions of the attention kernels (attention.cu: production kernels and host dispatch;
-// attention_experiments.cu: alternative structures kept for the record, selected by B2F_ATTN_VARIANT).
+// Shared definitions of the attention kernels (attention.cu: forward kernel and host dispatch; attention_bwd.cu:
+// backward kernels).
 #pragma once
 #include "host_common.h"
 #include "ptx.cuh"
@@ -8,12 +8,13 @@ namespace b2f {
 namespace attn {
 
 constexpr int DH = 128;
-constexpr int BQ = 128;   // rows per query tile
+constexpr int BQ = 128;   // query rows per CTA (64 per consumer warpgroup)
 constexpr int BKV = 128;  // rows per K/V block
-constexpr int KV_SLOTS = 4;
-constexpr int TILE_BYTES = 128 * DH * 2;  // 32 KB
-constexpr int ATTN_THREADS = 320;
-constexpr int ATTN_SMEM = (2 + KV_SLOTS) * TILE_BYTES + 256 + 1024;
+constexpr int KV_SLOTS = 2;
+constexpr int TILE_BYTES = 128 * DH * 2;  // 32 KB: [128 rows][128 dh] as two [128][64] swizzled halves
+constexpr int HALF_BYTES = TILE_BYTES / 2;
+constexpr int ATTN_THREADS = 384;         // producer warpgroup + 2 consumer warpgroups
+constexpr int ATTN_SMEM = (1 + 2 * KV_SLOTS) * TILE_BYTES + 256 + 1024;
 
 struct AttnParams {
   int B, H, Hkv, Sq, Skv;
@@ -37,46 +38,25 @@ static __device__ __forceinline__ float ex2(float x) {
   return y;
 }
 
-// 2^x on the FMA/ALU pipes (no MUFU): round-to-nearest split x = n + f, f in [-0.5, 0.5], degree-3
-// minimax polynomial for 2^f (max rel. error 1.0e-4, far below the bf16 rounding of P), exponent
-// add through the integer pipe.  Used for a fraction of the exponentials so the SFU (16 ex2/clk/SM)
-// stops being co-critical with the tensor pipe.
-static __device__ __forceinline__ float ex2_poly(float x) {
-  x = fmaxf(x, -125.0f);
-  const float t = x + 12582912.0f;            // 1.5 * 2^23: low mantissa bits of t hold n
-  const float f = x - (t - 12582912.0f);
-  float r = fmaf(0.05592203512787819f, f, 0.24264007806777954f);
-  r = fmaf(r, f, 0.6931210160255432f);
-  r = fmaf(r, f, 0.9999244809150696f);
-  return __int_as_float(__float_as_int(r) + (__float_as_int(t) << 23));
+// Row reductions over the four lanes of a quad (the threads sharing an accumulator row of a wgmma result).
+static __device__ __forceinline__ float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+static __device__ __forceinline__ float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// Packed pair version (FFMA2 / FADD2): 2^x0, 2^x1 without MUFU in 11 issue slots.
-static __device__ __forceinline__ void ex2_poly2(float x0, float x1, float& r0, float& r1) {
-  x0 = fmaxf(x0, -125.0f);
-  x1 = fmaxf(x1, -125.0f);
-  float t0, t1, n0, n1, f0, f1;
-  fadd2(t0, t1, x0, x1, 12582912.0f, 12582912.0f);
-  fadd2(n0, n1, t0, t1, -12582912.0f, -12582912.0f);
-  fadd2(f0, f1, x0, x1, -n0, -n1);
-  ffma2(r0, r1, f0, f1, 0.05592203512787819f, 0.05592203512787819f, 0.24264007806777954f, 0.24264007806777954f);
-  ffma2(r0, r1, r0, r1, f0, f1, 0.6931210160255432f, 0.6931210160255432f);
-  ffma2(r0, r1, r0, r1, f0, f1, 0.9999244809150696f, 0.9999244809150696f);
-  r0 = __int_as_float(__float_as_int(r0) + (__float_as_int(t0) << 23));
-  r1 = __int_as_float(__float_as_int(r1) + (__float_as_int(t1) << 23));
+// One 16-column k-chunk of an m64nXk16 accumulator (fp32, layout of ptx.cuh) packed to bf16 as the register A operand
+// of the next wgmma: chunk kk covers accumulator elements [8 kk, 8 kk + 8).
+template <int R>
+static __device__ __forceinline__ void pack_a_frag(const float (&s)[R], int kk, uint32_t (&a)[4]) {
+  a[0] = pack_bf16x2(s[8 * kk + 0], s[8 * kk + 1]);
+  a[1] = pack_bf16x2(s[8 * kk + 2], s[8 * kk + 3]);
+  a[2] = pack_bf16x2(s[8 * kk + 4], s[8 * kk + 5]);
+  a[3] = pack_bf16x2(s[8 * kk + 6], s[8 * kk + 7]);
 }
-
-typedef void (*KernelFn)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const AttnParams);
-
-// launch shape of a kernel variant
-struct Variant {
-  KernelFn fn;
-  int threads, smem;
-  bool single_tile;   // one 128-row Q tile per CTA (grid.x = ceil(Sq / 128)) instead of two
-};
-
-// attention_experiments.cu: fills `out` for variants 10-12, 30-32, 40-42, 60-62; false for anything else
-bool experimental_variant(int variant, Variant* out);
 
 }  // namespace attn
 }  // namespace b2f

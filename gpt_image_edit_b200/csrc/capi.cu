@@ -117,7 +117,7 @@ const char* b2f_strerror(int code) {
     case B2F_ERR_CUDA: return "CUDA error (see stderr)";
     case B2F_ERR_UNSUPPORTED: return "unsupported shape or mode";
     case B2F_ERR_ALIGN: return "pointer or pitch not 16-byte aligned";
-    case B2F_ERR_NODEVICE: return "no sm_100 device";
+    case B2F_ERR_NODEVICE: return "no sm_90 device";
     case B2F_ERR_WORKSPACE: return "workspace too small";
     default: return "unknown error";
   }

@@ -1,4 +1,4 @@
-// 3x3 convolution as an implicit GEMM on tcgen05 (sm_100a), NHWC bf16, fp32 accumulation in TMEM.
+// 3x3 convolution as an implicit GEMM on wgmma (sm_90a), NHWC bf16, fp32 accumulation in registers.
 //
 //   out[n, y, x, co] = bias[co] + sum_{ky,kx,ci} in[n, y*s + ky - p, x*s + kx - p, ci] * w[co, ky, kx, ci]
 //
@@ -8,16 +8,15 @@
 // padding come from TMA's out-of-bounds zero fill, no im2col buffer and no halo staging code.
 // The stride-2 downsample (diffusers Downsample2D: pad right/bottom by 1, stride 2, no other padding)
 // uses a second tensor map whose traversal stride is 2 in x and y.
-// Weights are OHWI ([Cout, 3, 3, Cin] = K-major [Cout, 9*Cin]).  Warp roles, smem ring, TMEM
-// double buffering and the epilogue structure are those of gemm.cu.
+// Weights are OHWI ([Cout, 3, 3, Cin] = K-major [Cout, 9*Cin]).  Warp roles, smem ring and the staged
+// epilogue are those of gemm.cu (gemm_sm90.cuh).
 //
 // Replaces cuDNN conv as reached by diffusers AutoencoderKL (ResnetBlock2D conv1/conv2, Downsample2D,
 // Upsample2D conv, conv_in/conv_out; SURVEY.md A.4; reference call sites
 // univa/utils/flux_pipeline.py:600-613, 1127-1129).
 #include <atomic>
 
-#include "host_common.h"
-#include "ptx.cuh"
+#include "gemm_sm90.cuh"
 
 namespace b2f {
 
@@ -25,11 +24,9 @@ extern std::atomic<uint64_t> g_launch_count;
 
 namespace {
 
-constexpr int TILE_H = 8, TILE_W = 16;
-constexpr int BLOCK_M = TILE_H * TILE_W;  // 128
-constexpr int BLOCK_K = 64;
-constexpr int UMMA_K = 16;
-constexpr int CONV_THREADS = 192;
+using namespace sm90;
+
+constexpr int TILE_H = 8, TILE_W = 16;   // TILE_H * TILE_W = BLOCK_M
 
 struct ConvParams {
   int N, Ho, Wo, Cin, Cout, stride;
@@ -42,252 +39,143 @@ struct ConvParams {
   int tiles_y, tiles_x, num_m_blocks, num_n_blocks;
 };
 
-template <int BN>
-struct ConvCfg {
-  static constexpr int STAGES = BN == 256 ? 4 : 6;
-  static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
-  static constexpr int B_BYTES = BN * BLOCK_K * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
-  static constexpr int TMEM_COLS = 2 * BN;
-};
-
-template <int BN>
-__global__ void __launch_bounds__(CONV_THREADS, 1)
+__global__ void __launch_bounds__(THREADS, 1)
 conv3x3_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant__ CUtensorMap tmW,
                const ConvParams p) {
-  using Cfg = ConvCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tmem_full = empty_bar + Cfg::STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  if (warp == 0 && lane == 0) {
+  const Smem s = carve(smem_raw);
+  const int wg = threadIdx.x >> 7;
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmIn);
     tma_prefetch_desc(&tmW);
   }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < Cfg::STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 4);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
+  init_barriers(s);
 
-  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
   const int cchunks = p.Cin / BLOCK_K;
   const int num_kb = 9 * cchunks;
   const int tiles_per_img = p.tiles_y * p.tiles_x;
+  // n-block fastest: neighbouring CTAs share the same input patch rows through L2
+  const int t = blockIdx.x;
+  const int n_blk = t % p.num_n_blocks;
+  const int m = t / p.num_n_blocks;
+  const int n_img = m / tiles_per_img;
+  const int r = m - n_img * tiles_per_img;
+  const int y0 = (r / p.tiles_x) * TILE_H;
+  const int x0 = (r % p.tiles_x) * TILE_W;
 
-  // n-block fastest: the CTAs of one wave share the same input patch rows through L2
-  auto decode = [&](int t, int& n_img, int& y0, int& x0, int& n_blk) {
-    n_blk = t % p.num_n_blocks;
-    const int m = t / p.num_n_blocks;
-    n_img = m / tiles_per_img;
-    const int r = m - n_img * tiles_per_img;
-    y0 = (r / p.tiles_x) * TILE_H;
-    x0 = (r % p.tiles_x) * TILE_W;
-  };
-
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       const int pad = p.stride == 1 ? 1 : 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        int n_img, y0, x0, n_blk;
-        decode(t, n_img, y0, x0, n_blk);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          const int tap = kb / cchunks;
-          const int c0 = (kb - tap * cchunks) * BLOCK_K;
-          const int ky = tap / 3, kx = tap - ky * 3;
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sb = sa + Cfg::A_BYTES;
-          mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-          tma_load_4d(sa, &tmIn, &full_bar[stage], c0, x0 * p.stride + kx - pad,
-                      y0 * p.stride + ky - pad, n_img);
-          tma_load_2d(sb, &tmW, &full_bar[stage], tap * p.Cin + c0, n_blk * BN);
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc_bf16(BLOCK_M, BN, 0);
-    const uint64_t d_base = make_sdesc_sw128(smem_u32(smem), 16, 1024);
-    int stage = 0;
-    uint32_t phase = 0;
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      mbar_wait(&tmem_empty[as], aphase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + uint32_t(as * BN);
       for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint64_t da = d_base + uint64_t((stage * Cfg::STAGE_BYTES) >> 4);
-        const uint64_t db = da + uint64_t(Cfg::A_BYTES >> 4);
-        if (elect_one()) {
-#pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-            umma_ss(d_tmem, da + uint64_t((k * UMMA_K * 2) >> 4), db + uint64_t((k * UMMA_K * 2) >> 4), idesc,
-                    (kb | k) != 0 ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (kb == num_kb - 1) umma_commit(&tmem_full[as]);
-        }
-        __syncwarp();
-        if (++stage == Cfg::STAGES) {
+        const int tap = kb / cchunks;
+        const int c0 = (kb - tap * cchunks) * BLOCK_K;
+        const int ky = tap / 3, kx = tap - ky * 3;
+        mbar_wait(&s.empty[stage], phase ^ 1);
+        uint8_t* sa = s.ring + stage * STAGE_BYTES;
+        uint8_t* sb = sa + A_BYTES;
+        mbar_expect_tx(&s.full[stage], STAGE_BYTES);
+        tma_load_4d(sa, &tmIn, &s.full[stage], c0, x0 * p.stride + kx - pad, y0 * p.stride + ky - pad, n_img);
+        tma_load_2d(sb, &tmW, &s.full[stage], tap * p.Cin + c0, n_blk * BLOCK_N);
+        if (++stage == STAGES) {
           stage = 0;
           phase ^= 1;
         }
       }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
     }
-  } else {
-    const int q = warp & 3;
-    const int row_in_tile = q * 32 + lane;
-    const int yl = row_in_tile / TILE_W, xl = row_in_tile % TILE_W;
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      int n_img, y0, x0, n_blk;
-      decode(t, n_img, y0, x0, n_blk);
-      mbar_wait(&tmem_full[as], aphase);
-      tc_fence_after();
-      const int y = y0 + yl, x = x0 + xl;
-      const bool row_ok = (y < p.Ho) && (x < p.Wo);
-      const long long pix = ((long long)n_img * p.Ho + y) * p.Wo + x;
-      __nv_bfloat16* out_row = p.out + pix * p.Cout;
-      const __nv_bfloat16* res_row = p.resid ? p.resid + pix * p.Cout : nullptr;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t acc[32];
-        const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + uint32_t(as * BN + c0);
-        __syncwarp();
-        B2F_TMEM_LD_X32(taddr, acc);
-        tmem_wait_ld();
-        if (c0 + 32 == BN) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[as]);
-        }
-        const int n0 = n_blk * BN + c0;
-        if (!row_ok || n0 >= p.Cout) continue;
-#pragma unroll
-        for (int g = 0; g < 4; ++g) {
-          const int n = n0 + g * 8;
-          if (n >= p.Cout) break;
-          float v[8];
-#pragma unroll
-          for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(acc[g * 8 + j]);
-          if (p.bias) {
-            const uint4 bq = __ldg(reinterpret_cast<const uint4*>(p.bias + n));
-            const uint32_t bw[4] = {bq.x, bq.y, bq.z, bq.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float2 b2 = unpack_bf16x2(bw[j]);
-              v[2 * j] += b2.x;
-              v[2 * j + 1] += b2.y;
-            }
-          }
-          if (p.out_nchw == 2) {
-            uint8_t* o8 = reinterpret_cast<uint8_t*>(p.out) + (((long long)n_img * p.Ho + y) * p.Wo + x) * p.Cout;
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int co = n + j;
-              if (co < p.Cout) {
-                const float img = bf16r(v[j]);                                   // the bf16 image the decoder returns
-                const float u = fminf(fmaxf(img / 2.0f + 0.5f, 0.0f), 1.0f);     // denormalise + clamp in fp32
-                o8[co] = (uint8_t)rintf(u * 255.0f);                             // numpy round (half to even)
-              }
-            }
-            continue;
-          }
-          if (p.out_nchw) {
-            // small heads (Cout <= 32): planar output, one scalar per (pixel, channel)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const int co = n + j;
-              if (co < p.Cout)
-                p.out[(((long long)n_img * p.Cout + co) * p.Ho + y) * p.Wo + x] =
-                    __float2bfloat16_rn(v[j]);
-            }
-            continue;
-          }
-          if (res_row) {
-            const uint4 rq = *reinterpret_cast<const uint4*>(res_row + n);
-            const uint32_t rw[4] = {rq.x, rq.y, rq.z, rq.w};
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const float2 r2 = unpack_bf16x2(rw[j]);
-              v[2 * j] = r2.x + bf16r(v[2 * j]);
-              v[2 * j + 1] = r2.y + bf16r(v[2 * j + 1]);
-            }
-          }
-          uint4 o;
-          o.x = pack_bf16x2(v[0], v[1]);
-          o.y = pack_bf16x2(v[2], v[3]);
-          o.z = pack_bf16x2(v[4], v[5]);
-          o.w = pack_bf16x2(v[6], v[7]);
-          *reinterpret_cast<uint4*>(out_row + n) = o;
-        }
-      }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
-    }
+    return;
   }
+  float acc[64];
+  mainloop<0, 0>(s, num_kb, wg - 1, acc);
+  stage_accumulators(s, wg - 1, acc);
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
+  const int e = threadIdx.x - 128;
+  const int row_in_tile = e & (BLOCK_M - 1), half = e >> 7;
+  const int yl = row_in_tile / TILE_W, xl = row_in_tile % TILE_W;
+  const int y = y0 + yl, x = x0 + xl;
+  if (y >= p.Ho || x >= p.Wo) return;
+  const long long pix = ((long long)n_img * p.Ho + y) * p.Wo + x;
+  __nv_bfloat16* out_row = p.out + pix * p.Cout;
+  const __nv_bfloat16* res_row = p.resid ? p.resid + pix * p.Cout : nullptr;
+  const float* crow = s.cbuf + row_in_tile * CROW;
+#pragma unroll 1
+  for (int c0 = half * (BLOCK_N / 2); c0 < (half + 1) * (BLOCK_N / 2); c0 += 32) {
+    const int n0 = n_blk * BLOCK_N + c0;
+    if (n0 >= p.Cout) break;
+    uint32_t acc32[32];
+    load_chunk(crow, c0, acc32);
+#pragma unroll
+    for (int g = 0; g < 4; ++g) {
+      const int n = n0 + g * 8;
+      if (n >= p.Cout) break;
+      float v[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(acc32[g * 8 + j]);
+      if (p.bias) {
+        const uint4 bq = __ldg(reinterpret_cast<const uint4*>(p.bias + n));
+        const uint32_t bw[4] = {bq.x, bq.y, bq.z, bq.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 b2 = unpack_bf16x2(bw[j]);
+          v[2 * j] += b2.x;
+          v[2 * j + 1] += b2.y;
+        }
+      }
+      if (p.out_nchw == 2) {
+        uint8_t* o8 = reinterpret_cast<uint8_t*>(p.out) + pix * p.Cout;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int co = n + j;
+          if (co < p.Cout) {
+            const float img = bf16r(v[j]);                                   // the bf16 image the decoder returns
+            const float u = fminf(fmaxf(img / 2.0f + 0.5f, 0.0f), 1.0f);     // denormalise + clamp in fp32
+            o8[co] = (uint8_t)rintf(u * 255.0f);                             // numpy round (half to even)
+          }
+        }
+        continue;
+      }
+      if (p.out_nchw) {
+        // small heads (Cout <= 32): planar output, one scalar per (pixel, channel)
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int co = n + j;
+          if (co < p.Cout)
+            p.out[(((long long)n_img * p.Cout + co) * p.Ho + y) * p.Wo + x] = __float2bfloat16_rn(v[j]);
+        }
+        continue;
+      }
+      if (res_row) {
+        const uint4 rq = *reinterpret_cast<const uint4*>(res_row + n);
+        const uint32_t rw[4] = {rq.x, rq.y, rq.z, rq.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const float2 r2 = unpack_bf16x2(rw[j]);
+          v[2 * j] = r2.x + bf16r(v[2 * j]);
+          v[2 * j + 1] = r2.y + bf16r(v[2 * j + 1]);
+        }
+      }
+      uint4 o;
+      o.x = pack_bf16x2(v[0], v[1]);
+      o.y = pack_bf16x2(v[2], v[3]);
+      o.z = pack_bf16x2(v[4], v[5]);
+      o.w = pack_bf16x2(v[6], v[7]);
+      *reinterpret_cast<uint4*>(out_row + n) = o;
+    }
   }
 }
 
-template <int BN>
 int launch_conv(const CUtensorMap& tmIn, const CUtensorMap& tmW, ConvParams p, cudaStream_t stream) {
-  using Cfg = ConvCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel<BN>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) return cuda_err(e, "conv smem attribute");
     attr_set = true;
   }
-  p.num_n_blocks = (p.Cout + BN - 1) / BN;
+  p.num_n_blocks = (p.Cout + BLOCK_N - 1) / BLOCK_N;
   const int num_tiles = p.num_m_blocks * p.num_n_blocks;
-  const int grid = num_tiles < device_info().num_sms ? num_tiles : device_info().num_sms;
   prof_begin(KC_CONV, stream);
-  conv3x3_kernel<BN><<<grid, CONV_THREADS, Cfg::SMEM_BYTES, stream>>>(tmIn, tmW, p);
+  conv3x3_kernel<<<num_tiles, THREADS, SMEM_BYTES, stream>>>(tmIn, tmW, p);
   const double pix = (double)p.N * p.Ho * p.Wo;
   prof_end(KC_CONV, stream, 2.0 * pix * 9.0 * p.Cin * p.Cout,
            2.0 * (pix * p.stride * p.stride * p.Cin + pix * p.Cout + 9.0 * p.Cin * p.Cout));
@@ -325,15 +213,14 @@ int conv3x3(const void* in, const void* w, const void* bias, void* out, const vo
   p.tiles_y = (p.Ho + TILE_H - 1) / TILE_H;
   p.tiles_x = (p.Wo + TILE_W - 1) / TILE_W;
   p.num_m_blocks = N * p.tiles_y * p.tiles_x;
-  const bool use256 = (Cout % 256 == 0) && (long long)p.num_m_blocks * (Cout / 256) >= device_info().num_sms;
   CUtensorMap tmIn, tmW;
   int rc = make_tmap_4d_bf16(&tmIn, in, N, Hin, Win, Cin, TILE_H, TILE_W, BLOCK_K, stride);
   if (rc) return rc;
   // weights padded by the caller to a multiple of 8 rows when Cout is tiny; OOB rows read as zero
   rc = make_tmap_2d_bf16(&tmW, w, (uint64_t)Cout, (uint64_t)9 * Cin, (uint64_t)9 * Cin,
-                         use256 ? 256 : 128, BLOCK_K);
+                         BLOCK_N, BLOCK_K);
   if (rc) return rc;
-  return use256 ? launch_conv<256>(tmIn, tmW, p, stream) : launch_conv<128>(tmIn, tmW, p, stream);
+  return launch_conv(tmIn, tmW, p, stream);
 }
 
 }  // namespace b2f

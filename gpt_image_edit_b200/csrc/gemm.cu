@@ -1,24 +1,18 @@
-// Persistent warp-specialised bf16 GEMM for sm_100a:  out[M,N] = epi(A[M,K] · W[N,K]^T + bias).
+// Warp-specialised bf16 GEMM for sm_90a:  out[M,N] = epi(A[M,K] · W[N,K]^T + bias).
 //
-//   warp 0 (1 lane)  TMA producer      cp.async.bulk.tensor → 128B-swizzled smem ring
-//   warp 1 (1 lane)  MMA issuer        tcgen05.mma cta_group::1 kind::f16, M=128, N=BN, K=16
-//   warps 2..5       epilogue          tcgen05.ld (32 lanes x 32 cols) → bias/act/gate/resid → global
+//   warpgroup 0 (1 lane)  TMA producer      cp.async.bulk.tensor → 128B-swizzled smem ring
+//   warpgroups 1, 2       wgmma consumers   m64n128k16, 64 rows of the 128 x 128 tile each, fp32 in registers
+//   epilogue              accumulators staged in smem → bias/act/gate/resid → global, one row per thread
 //
-// Accumulators live in TMEM (2 stages x BN fp32 columns) so the epilogue of tile i overlaps the
-// main loop of tile i+1.  Both operands are K-major ([rows, K] row-major), which is what
-// nn.Linear stores (SURVEY.md A.6) — no transposes anywhere.
+// Both operands of the forward GEMM are K-major ([rows, K] row-major), which is what nn.Linear stores
+// (SURVEY.md A.6) — no transposes anywhere.  The building blocks are shared with conv.cu (gemm_sm90.cuh).
 //
 // Replaces: torch.nn.functional.linear → cuBLASLt (diffusers FluxTransformer2DModel linears,
 // reference call site univa/utils/flux_pipeline.py:1067; SURVEY.md §2b row 1).
 #include <atomic>
 #include <cstdlib>
 
-#ifndef B2F_GEMM_2CTA_DEFAULT
-#define B2F_GEMM_2CTA_DEFAULT 1
-#endif
-
-#include "host_common.h"
-#include "ptx.cuh"
+#include "gemm_sm90.cuh"
 
 namespace b2f {
 
@@ -26,11 +20,7 @@ extern std::atomic<uint64_t> g_launch_count;
 
 namespace {
 
-constexpr int BLOCK_M = 128;
-constexpr int BLOCK_K = 64;  // 64 bf16 = 128 B = one swizzle row
-constexpr int UMMA_K = 16;
-constexpr int GEMM_THREADS = 320;   // TMA producer warp, MMA warp, 8 epilogue warps (two per TMEM lane quarter)
-constexpr int EPI_WARPS = 8;
+using namespace sm90;
 
 struct GemmParams {
   int batch, M, N, K;  // M rows per batch item
@@ -65,20 +55,8 @@ struct GemmParams {
 //   MODE 1  dgrad:    out[M,N] = A[M,K] . Wt[K,N]            A K-major, B MN-major: dX = dY . W with W as stored [out,in]
 //   MODE 2  wgrad:    out[M,N] = sum_b At[b,K,M]^T . Bt[b,K,N]   both MN-major (tokens are the rows of both), fp32 output
 // An MN-major 64(k) x 64(mn) box is one 128B-swizzled 8 KB TMA box; a tile of `mn` columns is mn/64 boxes 8 KB apart
-// (descriptor LBO = 8192, SBO = 1024, 16 k-rows = 2048 bytes per UMMA k-step) — the layout the attention kernel
-// uses for V.
-constexpr int MN_BOX_BYTES = 64 * 64 * 2;
-
-template <int BN>
-struct GemmCfg {
-  static constexpr int STAGES = BN == 256 ? 4 : 6;
-  static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;
-  static constexpr int B_BYTES = BN * BLOCK_K * 2;
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int BAR_BYTES = 256;
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + BAR_BYTES + 1024;
-  static constexpr int TMEM_COLS = 2 * BN;
-};
+// (descriptor LBO = 8192, SBO = 1024, 16 k-rows = 2048 bytes per wgmma k-step) — the layout the attention kernels
+// use for V.
 
 __device__ __forceinline__ void tile_coords(const GemmParams& p, int t, int& m_blk, int& n_blk) {
   // Panels of `panel_n` n-blocks; inside a panel n runs fastest so that the W panel stays in L2
@@ -226,26 +204,20 @@ __device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const int ep
   }
 }
 
-
-// One 128-column head of a fused QKV projection for one token, straight from the accumulators:
+// One 128-column head of a fused QKV projection for one token, straight from the staged accumulators:
 //   x = bf16(acc + bias);  y = bf16(x * rsqrt(mean(x^2) + eps));  z = bf16(y * w);
 //   out = bf16(z * cos + rot(z) * sin)        (diffusers RMSNorm + apply_rotary_emb, SURVEY.md A.2)
-// — the same rounding chain as rmsnorm_rope_kernel, but without the extra HBM round trip.  The head is pulled from TMEM
-// in four 32-column chunks; x is kept as 64 packed bf16 pairs (not 128 floats) and every rounding is the packed
-// cvt.rn.bf16x2 (the scalar conversion is an XU-pipe instruction: 8 clocks per warp).
-// `release` is called once the last TMEM read of this head has completed.
-template <typename Release>
-__device__ __forceinline__ void epilogue_head_norm_rope(const GemmParams& p, uint32_t taddr, int n_head0, long long row,
-                                                        __nv_bfloat16* out_row, bool is_k, bool active, Release release) {
+// — the same rounding chain as rmsnorm_rope_kernel, but without the extra HBM round trip.  Every rounding is the packed
+// cvt.rn.bf16x2.
+__device__ __forceinline__ void epilogue_head_norm_rope(const GemmParams& p, const float* crow, int n_head0,
+                                                        long long row, __nv_bfloat16* out_row, bool is_k) {
   const __nv_bfloat16* w = is_k ? p.nw_k : p.nw_q;
-  // pass 1: sum of squares of x = bf16(acc + bias) over the head (nothing kept: the head is re-read from TMEM in pass 2,
-  // which costs less than holding 128 values in registers at 8 epilogue warps per CTA)
+  // pass 1: sum of squares of x = bf16(acc + bias) over the head
   float ss = 0.f;
 #pragma unroll 1
   for (int cc = 0; cc < 4; ++cc) {
     uint32_t acc[32];
-    B2F_TMEM_LD_X32(taddr + cc * 32, acc);
-    tmem_wait_ld();
+    load_chunk(crow, cc * 32, acc);
 #pragma unroll
     for (int g = 0; g < 4; ++g) {
       const int c = cc * 32 + g * 8;
@@ -268,11 +240,7 @@ __device__ __forceinline__ void epilogue_head_norm_rope(const GemmParams& p, uin
 #pragma unroll 1
   for (int cc = 0; cc < 4; ++cc) {
     uint32_t acc[32];
-    __syncwarp();
-    B2F_TMEM_LD_X32(taddr + cc * 32, acc);
-    tmem_wait_ld();
-    if (cc == 3) release();
-    if (!active) continue;
+    load_chunk(crow, cc * 32, acc);
 #pragma unroll
     for (int g = 0; g < 4; ++g) {
       const int c = cc * 32 + g * 8;
@@ -311,44 +279,18 @@ __device__ __forceinline__ __nv_bfloat16* out_row_ptr(const GemmParams& p, int b
   return p.out + bidx * p.out_bs + row * p.ldc;
 }
 
-// Epilogue of one output tile for the calling warp: its 32 rows (TMEM lane quarter q) x its half of the BN columns
-// (`half` = 0 / 1: two warps share a lane quarter).  TMEM -> registers -> fused math -> global.
-// `arrive_cta0`: the CTA-pair kernel hands the accumulator stage back on CTA 0's barrier.
-template <int BN>
-__device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tmem_base, int as, int q, int half, int lane,
-                                              int n_blk, bool row_ok, long long row, __nv_bfloat16* out_row,
-                                              const __nv_bfloat16* res_row, const __nv_bfloat16* gate_row,
-                                              uint64_t* tmem_empty_bar, bool arrive_cta0,
-                                              __nv_bfloat16* out_row2 = nullptr) {
-  auto release = [&]() {
-    // all TMEM reads of this warp's part of the accumulator stage are complete: hand it back to the MMA warp
-    tc_fence_before();
-    __syncwarp();
-    if (lane == 0) {
-      if (arrive_cta0)
-        mbar_arrive_cta0(tmem_empty_bar);
-      else
-        mbar_arrive(tmem_empty_bar);
-    }
-  };
-  constexpr int HALF = BN / 2;             // columns per warp: 128 (one head), 96 or 64
-  const uint32_t lane_base = tmem_base + (uint32_t(q * 32) << 16) + uint32_t(as * BN + half * HALF);
+// Epilogue of one output row for the calling thread: its `half` (0 / 1) of the tile's 128 columns, read from the
+// staged accumulators.  A fused QKV head is the whole tile: the half-0 thread of the row runs it.
+__device__ __forceinline__ void epilogue_row(const GemmParams& p, const float* crow, int half, int n_blk, bool row_ok,
+                                             long long row, __nv_bfloat16* out_row, const __nv_bfloat16* res_row,
+                                             const __nv_bfloat16* gate_row, __nv_bfloat16* out_row2) {
+  if (!row_ok) return;
   if (p.epi == B2F_EPI_QKV_NORM_ROPE) {
-    if (BN != 256) {
-      // 128-wide tiles (small problems): the head belongs to the half-0 warps, the others only release
-      if (half == 1) {
-        __syncwarp();
-        release();
-        return;
-      }
-    }
-    const int h0 = BN == 256 ? half * 128 : 0;
-    const uint32_t taddr = tmem_base + (uint32_t(q * 32) << 16) + uint32_t(as * BN + h0);
-    const int n_head0 = n_blk * BN + h0;
+    if (half == 1) return;
+    const int n_head0 = n_blk * BLOCK_N;
     const int which = n_head0 / p.d_model;  // 0 = Q, 1 = K, 2 = V, >= 3: second output block
-    __syncwarp();
     if (which < 2 && n_head0 < p.N) {
-      epilogue_head_norm_rope(p, taddr, n_head0, row, out_row, which == 1, row_ok, release);
+      epilogue_head_norm_rope(p, crow, n_head0, row, out_row, which == 1);
       return;
     }
     const bool second = p.split_n > 0 && n_head0 >= p.split_n;
@@ -356,565 +298,117 @@ __device__ __forceinline__ void epilogue_tile(const GemmParams& p, uint32_t tmem
     const int epi = second ? p.epi2 : B2F_EPI_BIAS;
 #pragma unroll 1
     for (int cc = 0; cc < 4; ++cc) {
+      if (n_head0 + cc * 32 >= p.N) break;
       uint32_t acc[32];
-      __syncwarp();
-      B2F_TMEM_LD_X32(taddr + cc * 32, acc);
-      tmem_wait_ld();
-      if (cc == 3) release();
-      if (!row_ok || n_head0 + cc * 32 >= p.N) continue;
+      load_chunk(crow, cc * 32, acc);
       epilogue_chunk(p, epi, acc, n_head0 + cc * 32, orow, res_row, gate_row);
     }
     return;
   }
 #pragma unroll 1
-  for (int c0 = 0; c0 < HALF; c0 += 32) {
+  for (int c0 = 0; c0 < BLOCK_N / 2; c0 += 32) {
+    const int n0 = n_blk * BLOCK_N + half * (BLOCK_N / 2) + c0;
+    if (n0 >= p.N) break;
     uint32_t acc[32];
-    __syncwarp();  // tcgen05.ld is .sync.aligned: reconverge after the predicated stores
-    B2F_TMEM_LD_X32(lane_base + c0, acc);
-    tmem_wait_ld();
-    if (c0 + 32 >= HALF) release();
-    const int n0 = n_blk * BN + half * HALF + c0;
-    if (!row_ok || n0 >= p.N) continue;
+    load_chunk(crow, half * (BLOCK_N / 2) + c0, acc);
     epilogue_chunk(p, p.epi, acc, n0, out_row, res_row, gate_row);
   }
 }
 
-template <int BN, int MODE = 0>
-__global__ void __launch_bounds__(GEMM_THREADS, 1)
+template <int MODE>
+__global__ void __launch_bounds__(THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmParams p) {
-  using Cfg = GemmCfg<BN>;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tmem_full = empty_bar + Cfg::STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-
-  if (warp == 0 && lane == 0) {
+  const Smem s = carve(smem_raw);
+  const int wg = threadIdx.x >> 7;
+  if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
   }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < Cfg::STAGES; ++i) {
-      mbar_init(&full_bar[i], 1);
-      mbar_init(&empty_bar[i], 1);
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], EPI_WARPS);
-    }
-    fence_mbar_init();
-  }
-  if (warp == 2) {
-    tmem_alloc(tmem_ptr, Cfg::TMEM_COLS);
-    tmem_relinquish();
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
+  init_barriers(s);
 
-  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
+  int m_blk, n_blk;
+  tile_coords(p, blockIdx.x, m_blk, n_blk);
   const int num_kb = MODE == 2 ? p.kbatch * p.kb_per_batch : (p.K + BLOCK_K - 1) / BLOCK_K;
+  const int bb = m_blk / p.m_blocks_per_batch;
+  const int mb = m_blk - bb * p.m_blocks_per_batch;
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (wg == 0) {
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        int m_blk, n_blk;
-        tile_coords(p, t, m_blk, n_blk);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sb = sa + Cfg::A_BYTES;
-          mbar_expect_tx(&full_bar[stage], Cfg::STAGE_BYTES);
-          const int bb = m_blk / p.m_blocks_per_batch;
-          const int mb = m_blk - bb * p.m_blocks_per_batch;
-          if (MODE == 2) {
-            const int kbb = kb / p.kb_per_batch;
-            const int kr = (kb - kbb * p.kb_per_batch) * BLOCK_K;
-#pragma unroll
-            for (int i = 0; i < BLOCK_M / 64; ++i)
-              tma_load_3d(sa + i * MN_BOX_BYTES, &tmA, &full_bar[stage], m_blk * BLOCK_M + 64 * i, kr, kbb);
-#pragma unroll
-            for (int i = 0; i < BN / 64; ++i)
-              tma_load_3d(sb + i * MN_BOX_BYTES, &tmB, &full_bar[stage], n_blk * BN + 64 * i, kr, kbb);
-          } else {
-            tma_load_3d(sa, &tmA, &full_bar[stage], kb * BLOCK_K, mb * BLOCK_M, bb);
-            if (MODE == 1) {
-#pragma unroll
-              for (int i = 0; i < BN / 64; ++i)
-                tma_load_2d(sb + i * MN_BOX_BYTES, &tmB, &full_bar[stage], n_blk * BN + 64 * i, kb * BLOCK_K);
-            } else {
-              tma_load_2d(sb, &tmB, &full_bar[stage], kb * BLOCK_K, n_blk * BN);
-            }
-          }
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // whole warp runs the loop (uniform-datapath address math); one elected lane issues the MMAs
-    constexpr uint32_t idesc = make_idesc_bf16(BLOCK_M, BN, MODE >= 1, MODE == 2);
-    // K-major operands advance 32 bytes per UMMA k-step inside the swizzle row; MN-major ones 16 rows = 2048 bytes
-    constexpr int A_KSTEP = MODE == 2 ? 2048 : UMMA_K * 2;
-    constexpr int B_KSTEP = MODE >= 1 ? 2048 : UMMA_K * 2;
-    const uint64_t da_base = make_sdesc_sw128(smem_u32(smem), MODE == 2 ? MN_BOX_BYTES : 16, 1024);
-    const uint64_t db_base = make_sdesc_sw128(smem_u32(smem) + Cfg::A_BYTES, MODE >= 1 ? MN_BOX_BYTES : 16, 1024);
-    int stage = 0;
-    uint32_t phase = 0;
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      mbar_wait(&tmem_empty[as], aphase ^ 1);
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + uint32_t(as * BN);
       for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        tc_fence_after();
-        const uint64_t da = da_base + uint64_t((stage * Cfg::STAGE_BYTES) >> 4);
-        const uint64_t db = db_base + uint64_t((stage * Cfg::STAGE_BYTES) >> 4);
-        if (elect_one()) {
+        mbar_wait(&s.empty[stage], phase ^ 1);
+        uint8_t* sa = s.ring + stage * STAGE_BYTES;
+        uint8_t* sb = sa + A_BYTES;
+        mbar_expect_tx(&s.full[stage], STAGE_BYTES);
+        if (MODE == 2) {
+          const int kbb = kb / p.kb_per_batch;
+          const int kr = (kb - kbb * p.kb_per_batch) * BLOCK_K;
 #pragma unroll
-          for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-            umma_ss(d_tmem, da + uint64_t((k * A_KSTEP) >> 4), db + uint64_t((k * B_KSTEP) >> 4), idesc,
-                    (kb | k) != 0 ? 1u : 0u);
-          umma_commit(&empty_bar[stage]);
-          if (kb == num_kb - 1) umma_commit(&tmem_full[as]);
+          for (int i = 0; i < BLOCK_M / 64; ++i)
+            tma_load_3d(sa + i * MN_BOX_BYTES, &tmA, &s.full[stage], m_blk * BLOCK_M + 64 * i, kr, kbb);
+#pragma unroll
+          for (int i = 0; i < BLOCK_N / 64; ++i)
+            tma_load_3d(sb + i * MN_BOX_BYTES, &tmB, &s.full[stage], n_blk * BLOCK_N + 64 * i, kr, kbb);
+        } else {
+          tma_load_3d(sa, &tmA, &s.full[stage], kb * BLOCK_K, mb * BLOCK_M, bb);
+          if (MODE == 1) {
+#pragma unroll
+            for (int i = 0; i < BLOCK_N / 64; ++i)
+              tma_load_2d(sb + i * MN_BOX_BYTES, &tmB, &s.full[stage], n_blk * BLOCK_N + 64 * i, kb * BLOCK_K);
+          } else {
+            tma_load_2d(sb, &tmB, &s.full[stage], kb * BLOCK_K, n_blk * BLOCK_N);
+          }
         }
-        __syncwarp();
-        if (++stage == Cfg::STAGES) {
+        if (++stage == STAGES) {
           stage = 0;
           phase ^= 1;
         }
       }
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
     }
-  } else {
-    // ------------------------------------------------------------------ epilogue warps
-    const int q = warp & 3;  // TMEM lane quarter this warp may touch
-    const int half = (warp - 2) >> 2;   // which half of the tile's columns
-    const int row_in_tile = q * 32 + lane;
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      int m_blk, n_blk;
-      tile_coords(p, t, m_blk, n_blk);
-      mbar_wait(&tmem_full[as], aphase);
-      tc_fence_after();
-      const int bidx = m_blk / p.m_blocks_per_batch;
-      const long long row = (long long)(m_blk - bidx * p.m_blocks_per_batch) * BLOCK_M + row_in_tile;
-      const bool row_ok = row < p.M;
-      const __nv_bfloat16* gate_row = p.gate ? p.gate + (long long)bidx * p.gate_ld : nullptr;
-      __nv_bfloat16* out_row = out_row_ptr(p, bidx, row);
-      const __nv_bfloat16* res_row = p.resid ? p.resid + bidx * p.resid_bs + row * p.ldr : nullptr;
-      __nv_bfloat16* out_row2 = p.out2 ? p.out2 + bidx * p.out2_bs + row * p.ldc2 - p.split_n : nullptr;
-      epilogue_tile<BN>(p, tmem_base, as, q, half, lane, n_blk, row_ok, row, out_row, res_row, gate_row, &tmem_empty[as],
-                        false, out_row2);
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
-    }
+    return;
   }
+  float acc[64];
+  mainloop<MODE == 2, MODE >= 1>(s, num_kb, wg - 1, acc);
+  stage_accumulators(s, wg - 1, acc);
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, Cfg::TMEM_COLS);
-  }
+  const int e = threadIdx.x - 128;
+  const int row_in_tile = e & (BLOCK_M - 1), half = e >> 7;
+  const long long row = (long long)mb * BLOCK_M + row_in_tile;
+  const bool row_ok = row < p.M;
+  const __nv_bfloat16* gate_row = p.gate ? p.gate + (long long)bb * p.gate_ld : nullptr;
+  __nv_bfloat16* out_row = out_row_ptr(p, bb, row);
+  const __nv_bfloat16* res_row = p.resid ? p.resid + bb * p.resid_bs + row * p.ldr : nullptr;
+  __nv_bfloat16* out_row2 = p.out2 ? p.out2 + bb * p.out2_bs + row * p.ldc2 - p.split_n : nullptr;
+  epilogue_row(p, s.cbuf + row_in_tile * CROW, half, n_blk, row_ok, row, out_row, res_row, gate_row, out_row2);
 }
 
-template <int BN, int MODE = 0>
+template <int MODE>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN>;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<BN, MODE>,
-                                         cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         Cfg::SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
     if (e != cudaSuccess) return cuda_err(e, "gemm smem attribute");
     attr_set = true;
   }
   p.m_blocks_per_batch = (p.M + BLOCK_M - 1) / BLOCK_M;
   p.num_m_blocks = p.batch * p.m_blocks_per_batch;
-  p.num_n_blocks = (p.N + BN - 1) / BN;
-  p.panel_n = BN == 256 ? 16 : 32;
+  p.num_n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
+  p.panel_n = 16;
   const int num_tiles = p.num_m_blocks * p.num_n_blocks;
-  const int grid = num_tiles < device_info().num_sms ? num_tiles : device_info().num_sms;
   const double kk = MODE == 2 ? (double)p.kbatch * p.K : (double)p.K;
   prof_begin(KC_GEMM, stream);
-  gemm_bf16_kernel<BN, MODE><<<grid, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
+  gemm_bf16_kernel<MODE><<<num_tiles, THREADS, SMEM_BYTES, stream>>>(tmA, tmB, p);
   {
     char tag_[96];
-    snprintf(tag_, sizeof tag_, "gemm1cta%d m%d %dx%dx%d b%d e%d", BN, MODE, p.M, p.N, (int)kk, p.batch, p.epi);
+    snprintf(tag_, sizeof tag_, "gemm m%d %dx%dx%d b%d e%d", MODE, p.M, p.N, (int)kk, p.batch, p.epi);
     prof_end_tagged(KC_GEMM, stream, 2.0 * p.batch * (double)p.M * p.N * kk,
                     2.0 * ((double)p.batch * p.M * kk + (double)p.N * kk + (double)p.batch * p.M * p.N), tag_);
   }
   g_launch_count.fetch_add(1, std::memory_order_relaxed);
   B2F_CHECK_LAUNCH("gemm_bf16_kernel");
-  return B2F_OK;
-}
-
-
-// ================================================================================================
-// CTA-pair variant (cta_group::2): one 256 x 256 output tile per pair of SMs.
-//   CTA r of the pair loads A rows [m0 + 128 r, +128) and W rows [n0 + 128 r, +128) into ITS smem;
-//   CTA 0's MMA lane issues tcgen05.mma.cta_group::2 (M = 256, N = 256): each SM's tensor core
-//   multiplies its own 128 A rows with BOTH halves of W (its own + the peer's smem) into its own
-//   TMEM (128 lanes x 256 columns).  Per SM and k-step that is 32 KB of TMA traffic instead of the
-//   48 KB of the 1-CTA 128x256 tile — a third less L2->SM bandwidth and energy per FLOP.
-//   Barriers: TMA bytes of both CTAs are counted on CTA 0's `full` barrier; tcgen05.commit
-//   multicasts "stage free" / "accumulator ready" to both CTAs; both CTAs' epilogue warps arrive on
-//   CTA 0's `tmem_empty`.
-template <int BN_>
-struct Gemm2CfgT {
-  static constexpr int BN = BN_;       // 256, or 192: the narrower tile exists for shapes whose 256-wide tiling leaves the last
-                                       // wave mostly empty (M = 8192, N = 3072: 384 tiles = 5.19 waves of 74 pairs -> 6.92 at 192)
-  static constexpr int STAGES = 6;
-  static constexpr int A_BYTES = BLOCK_M * BLOCK_K * 2;       // 128 rows of A per CTA
-  static constexpr int B_BYTES = (BN / 2) * BLOCK_K * 2;      // 128 rows of W per CTA
-  static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;       // 32 KB
-  static constexpr int SMEM_BYTES = STAGES * STAGE_BYTES + 256 + 1024;
-  static constexpr int TMEM_COLS = 512;   // two accumulator stages of BN fp32 columns (power-of-two allocation)
-};
-using Gemm2Cfg = Gemm2CfgT<256>;
-
-// CL = CTAs per cluster: 2 = one CTA pair; 4 = two CTA pairs side by side in N (a 256 x 512 super tile) that
-// SHARE their A rows: each CTA fetches a 64-row slice of its 128 A rows and TMA-multicasts it to the CTA of the
-// same half in the other pair, so a k-step costs 24 KB of L2->SM traffic per CTA instead of 32 KB (the pair
-// kernel runs at the L2->SM bandwidth cap: ncu shows ~11.6 TB/s of xbar2l1tex reads at 75 % tensor activity).
-// A stage may be overwritten only when BOTH pairs have consumed it, so every CTA's `empty` barrier takes one
-// multicast commit from each pair leader.
-template <int CL, int MODE = 0, int BNP = 256>
-__device__ __forceinline__ void gemm_pair_body(const CUtensorMap* tmA, const CUtensorMap* tmB, const GemmParams& p) {
-  static_assert(CL == 2 || MODE == 0, "the 4-CTA cluster variant exists for the forward layout only");
-  static_assert(BNP == 256 || (CL == 2 && MODE == 0), "the 192-wide tile exists for the plain forward pair kernel only");
-  using Cfg = Gemm2CfgT<BNP>;
-  constexpr int PAIRS = CL / 2;
-  constexpr int BN = Cfg::BN;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + Cfg::STAGES * Cfg::STAGE_BYTES);
-  uint64_t* empty_bar = full_bar + Cfg::STAGES;
-  uint64_t* tmem_full = empty_bar + Cfg::STAGES;
-  uint64_t* tmem_empty = tmem_full + 2;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
-  const uint32_t crank = cluster_ctarank();
-  const uint32_t rank = crank & 1;        // half of the pair tile this CTA owns
-  const int pc = int(crank >> 1);         // pair inside the cluster
-  const bool leader = rank == 0;
-  const int pair = blockIdx.x / CL;       // work unit index: one (super) tile per cluster
-  const int num_pairs = gridDim.x / CL;
-
-  if (warp == 0 && lane == 0) {
-    tma_prefetch_desc(tmA);
-    tma_prefetch_desc(tmB);
-  }
-  if (warp == 1 && lane == 0) {
-    for (int i = 0; i < Cfg::STAGES; ++i) {
-      mbar_init(&full_bar[i], 2);   // one arrive per CTA's producer (+ both CTAs' TMA bytes)
-      mbar_init(&empty_bar[i], PAIRS);  // one multicast commit per pair leader
-    }
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&tmem_full[i], 1);
-      mbar_init(&tmem_empty[i], 2 * EPI_WARPS);  // 8 epilogue warps x 2 CTAs
-    }
-    fence_mbar_init();
-  }
-  if (warp == 2) {
-    tmem_alloc_2cta(tmem_ptr, Cfg::TMEM_COLS);
-    tmem_relinquish_2cta();
-  }
-  tc_fence_before();
-  cluster_sync_all();  // peer barriers are initialised before any remote arrive / multicast
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  // p.m_blocks_per_batch / num_m_blocks are in units of 256-row pair tiles here
-  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
-  const int num_kb = MODE == 2 ? p.kbatch * p.kb_per_batch : (p.K + BLOCK_K - 1) / BLOCK_K;
-
-  if (warp == 0) {
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int t = pair; t < num_tiles; t += num_pairs) {
-        int m_blk, n_blk;
-        tile_coords(p, t, m_blk, n_blk);
-        n_blk = n_blk * PAIRS + pc;
-        const int bb = m_blk / p.m_blocks_per_batch;
-        const int mb = m_blk - bb * p.m_blocks_per_batch;
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + stage * Cfg::STAGE_BYTES;
-          uint8_t* sb = sa + Cfg::A_BYTES;
-          if (leader)
-            mbar_expect_tx(&full_bar[stage], 2 * Cfg::STAGE_BYTES);
-          else
-            mbar_arrive_cta0(&full_bar[stage]);
-          if (MODE == 2) {
-            // wgrad: this CTA's 128 output rows (columns of dY) and 128 output columns (columns of X), 64 tokens
-            const int kbb = kb / p.kb_per_batch;
-            const int kr = (kb - kbb * p.kb_per_batch) * BLOCK_K;
-#pragma unroll
-            for (int i = 0; i < 2; ++i) {
-              tma_load_3d_2cta(sa + i * MN_BOX_BYTES, tmA, &full_bar[stage], m_blk * 256 + int(rank) * BLOCK_M + 64 * i, kr, kbb);
-              tma_load_3d_2cta(sb + i * MN_BOX_BYTES, tmB, &full_bar[stage], n_blk * BN + int(rank) * (BN / 2) + 64 * i, kr, kbb);
-            }
-          } else if (CL == 2) {
-            tma_load_3d_2cta(sa, tmA, &full_bar[stage], kb * BLOCK_K, mb * 256 + int(rank) * BLOCK_M, bb);
-          } else {
-            // 64-row slice `pc` of this half's A rows, to the same smem offset of both CTAs holding this half
-            tma_load_3d_2cta_mc(sa + pc * (Cfg::A_BYTES / 2), tmA, &full_bar[stage], kb * BLOCK_K,
-                                mb * 256 + int(rank) * BLOCK_M + pc * (BLOCK_M / 2), bb,
-                                uint16_t((1u << rank) | (1u << (2 + rank))));
-          }
-          if (MODE == 1) {
-            // dgrad: this CTA's 128 output columns of W^T (= columns of W as stored), 64 contraction rows
-#pragma unroll
-            for (int i = 0; i < 2; ++i)
-              tma_load_2d_2cta(sb + i * MN_BOX_BYTES, tmB, &full_bar[stage], n_blk * BN + int(rank) * (BN / 2) + 64 * i,
-                               kb * BLOCK_K);
-          } else if (MODE == 0) {
-            tma_load_2d_2cta(sb, tmB, &full_bar[stage], kb * BLOCK_K, n_blk * BN + int(rank) * (BN / 2));
-          }
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    if (leader) {
-      constexpr uint32_t idesc = make_idesc_bf16(256, BN, MODE >= 1, MODE == 2);
-      constexpr int A_KSTEP = MODE == 2 ? 2048 : UMMA_K * 2;
-      constexpr int B_KSTEP = MODE >= 1 ? 2048 : UMMA_K * 2;
-      const uint64_t da_base = make_sdesc_sw128(smem_u32(smem), MODE == 2 ? MN_BOX_BYTES : 16, 1024);
-      const uint64_t db_base = make_sdesc_sw128(smem_u32(smem) + Cfg::A_BYTES, MODE >= 1 ? MN_BOX_BYTES : 16, 1024);
-      int stage = 0;
-      uint32_t phase = 0;
-      int as = 0;
-      uint32_t aphase = 0;
-      for (int t = pair; t < num_tiles; t += num_pairs) {
-        mbar_wait(&tmem_empty[as], aphase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + uint32_t(as * BN);
-        for (int kb = 0; kb < num_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint64_t da = da_base + uint64_t((stage * Cfg::STAGE_BYTES) >> 4);
-          const uint64_t db = db_base + uint64_t((stage * Cfg::STAGE_BYTES) >> 4);
-          if (elect_one()) {
-#pragma unroll
-            for (int k = 0; k < BLOCK_K / UMMA_K; ++k)
-              umma_ss_2cta(d_tmem, da + uint64_t((k * A_KSTEP) >> 4), db + uint64_t((k * B_KSTEP) >> 4),
-                           idesc, (kb | k) != 0 ? 1u : 0u);
-            umma_commit_mc(&empty_bar[stage], uint16_t((1u << CL) - 1));
-            if (kb == num_kb - 1) umma_commit_mc(&tmem_full[as], uint16_t(3u << (2 * pc)));
-          }
-          __syncwarp();
-          if (++stage == Cfg::STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        if (++as == 2) {
-          as = 0;
-          aphase ^= 1;
-        }
-      }
-    }
-  } else {
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int row_in_tile = int(rank) * BLOCK_M + q * 32 + lane;  // row inside the 256-row pair tile
-    int as = 0;
-    uint32_t aphase = 0;
-    for (int t = pair; t < num_tiles; t += num_pairs) {
-      int m_blk, n_blk;
-      tile_coords(p, t, m_blk, n_blk);
-      n_blk = n_blk * PAIRS + pc;
-      mbar_wait(&tmem_full[as], aphase);
-      tc_fence_after();
-      const int bidx = m_blk / p.m_blocks_per_batch;
-      const long long row = (long long)(m_blk - bidx * p.m_blocks_per_batch) * 256 + row_in_tile;
-      const bool row_ok = row < p.M;
-      const __nv_bfloat16* gate_row = p.gate ? p.gate + (long long)bidx * p.gate_ld : nullptr;
-      __nv_bfloat16* out_row = out_row_ptr(p, bidx, row);
-      const __nv_bfloat16* res_row = p.resid ? p.resid + bidx * p.resid_bs + row * p.ldr : nullptr;
-      __nv_bfloat16* out_row2 = p.out2 ? p.out2 + bidx * p.out2_bs + row * p.ldc2 - p.split_n : nullptr;
-      epilogue_tile<BN>(p, tmem_base, as, q, half, lane, n_blk, row_ok, row, out_row, res_row, gate_row, &tmem_empty[as],
-                        true, out_row2);
-      if (++as == 2) {
-        as = 0;
-        aphase ^= 1;
-      }
-    }
-  }
-
-  tc_fence_before();
-  cluster_sync_all();  // both CTAs are done with each other's smem / barriers / TMEM
-  if (warp == 2) {
-    tc_fence_after();
-    tmem_dealloc_2cta(tmem_base, Cfg::TMEM_COLS);
-  }
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_2cta_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                      const GemmParams p) {
-  gemm_pair_body<2>(&tmA, &tmB, p);
-}
-
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_2cta_n192_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                           const GemmParams p) {
-  gemm_pair_body<2, 0, 192>(&tmA, &tmB, p);
-}
-
-// dgrad / wgrad operand layouts of the CTA-pair kernel (MODE 1 / 2, see GemmParams)
-template <int MODE>
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_grad_2cta_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                      const GemmParams p) {
-  gemm_pair_body<2, MODE>(&tmA, &tmB, p);
-}
-
-__global__ void __cluster_dims__(4, 1, 1) __launch_bounds__(GEMM_THREADS, 1)
-gemm_bf16_4cta_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                      const GemmParams p) {
-  gemm_pair_body<4>(&tmA, &tmB, p);
-}
-
-static int pair_kernel_attrs_once() {
-  static int rc = -1;
-  if (rc >= 0) return rc;
-  cudaError_t e = cudaFuncSetAttribute(gemm_bf16_2cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                       Gemm2Cfg::SMEM_BYTES);
-  if (e != cudaSuccess) return cuda_err(e, "gemm 2cta smem attribute");
-  e = cudaFuncSetAttribute(gemm_bf16_4cta_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Gemm2Cfg::SMEM_BYTES);
-  if (e != cudaSuccess) return cuda_err(e, "gemm 4cta smem attribute");
-  e = cudaFuncSetAttribute(gemm_bf16_2cta_n192_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, Gemm2CfgT<192>::SMEM_BYTES);
-  if (e != cudaSuccess) return cuda_err(e, "gemm 2cta n192 smem attribute");
-  e = cudaFuncSetAttribute(gemm_grad_2cta_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, Gemm2Cfg::SMEM_BYTES);
-  if (e != cudaSuccess) return cuda_err(e, "gemm dgrad 2cta smem attribute");
-  e = cudaFuncSetAttribute(gemm_grad_2cta_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, Gemm2Cfg::SMEM_BYTES);
-  if (e != cudaSuccess) return cuda_err(e, "gemm wgrad 2cta smem attribute");
-  rc = B2F_OK;
-  return rc;
-}
-
-template <int MODE = 0>
-int launch_gemm_2cta(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg;
-  if (int rc = pair_kernel_attrs_once()) return rc;
-  p.m_blocks_per_batch = (p.M + 255) / 256;
-  p.num_m_blocks = p.batch * p.m_blocks_per_batch;
-  p.num_n_blocks = (p.N + Cfg::BN - 1) / Cfg::BN;
-  p.panel_n = 16;
-  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
-  const int max_pairs = device_info().num_sms / 2;
-  const int pairs = num_tiles < max_pairs ? num_tiles : max_pairs;
-  const double kk = MODE == 2 ? (double)p.kbatch * p.K : (double)p.K;
-  prof_begin(KC_GEMM, stream);
-  if constexpr (MODE == 0)
-    gemm_bf16_2cta_kernel<<<2 * pairs, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
-  else
-    gemm_grad_2cta_kernel<MODE><<<2 * pairs, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
-  {
-    char tag_[96];
-    snprintf(tag_, sizeof tag_, "gemm2cta256 m%d %dx%dx%d b%d e%d", MODE, p.M, p.N, (int)kk, p.batch, p.epi);
-    prof_end_tagged(KC_GEMM, stream, 2.0 * p.batch * (double)p.M * p.N * kk,
-                    2.0 * ((double)p.batch * p.M * kk + (double)p.N * kk + (double)p.batch * p.M * p.N), tag_);
-  }
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("gemm_bf16_2cta_kernel");
-  return B2F_OK;
-}
-
-int launch_gemm_2cta_n192(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream) {
-  using Cfg = Gemm2CfgT<192>;
-  if (int rc = pair_kernel_attrs_once()) return rc;
-  p.m_blocks_per_batch = (p.M + 255) / 256;
-  p.num_m_blocks = p.batch * p.m_blocks_per_batch;
-  p.num_n_blocks = (p.N + Cfg::BN - 1) / Cfg::BN;
-  p.panel_n = 16;
-  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
-  const int max_pairs = device_info().num_sms / 2;
-  const int pairs = num_tiles < max_pairs ? num_tiles : max_pairs;
-  prof_begin(KC_GEMM, stream);
-  gemm_bf16_2cta_n192_kernel<<<2 * pairs, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
-  {
-    char tag_[96];
-    snprintf(tag_, sizeof tag_, "gemm2cta192 m0 %dx%dx%d b%d e%d", p.M, p.N, p.K, p.batch, p.epi);
-    prof_end_tagged(KC_GEMM, stream, 2.0 * p.batch * (double)p.M * p.N * p.K,
-                    2.0 * ((double)p.batch * p.M * p.K + (double)p.N * p.K + (double)p.batch * p.M * p.N), tag_);
-  }
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("gemm_bf16_2cta_n192_kernel");
-  return B2F_OK;
-}
-
-// co-resident 4-CTA clusters of the quad kernel (a GPC holds floor(SMs_in_GPC / 4) of them), queried once
-static int max_quad_clusters() {
-  static int n = -1;
-  if (n >= 0) return n;
-  if (pair_kernel_attrs_once() != B2F_OK) return 0;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(4 * 64, 1, 1);
-  cfg.blockDim = dim3(GEMM_THREADS, 1, 1);
-  cfg.dynamicSmemBytes = Gemm2Cfg::SMEM_BYTES;
-  cudaLaunchAttribute attr;
-  attr.id = cudaLaunchAttributeClusterDimension;
-  attr.val.clusterDim.x = 4;
-  attr.val.clusterDim.y = 1;
-  attr.val.clusterDim.z = 1;
-  cfg.attrs = &attr;
-  cfg.numAttrs = 1;
-  int c = 0;
-  if (cudaOccupancyMaxActiveClusters(&c, gemm_bf16_4cta_kernel, &cfg) != cudaSuccess || c <= 0) {
-    cudaGetLastError();
-    c = 0;
-  }
-  n = c;
-  return n;
-}
-
-int launch_gemm_4cta(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream) {
-  using Cfg = Gemm2Cfg;
-  p.m_blocks_per_batch = (p.M + 255) / 256;
-  p.num_m_blocks = p.batch * p.m_blocks_per_batch;
-  p.num_n_blocks = (p.N + 2 * Cfg::BN - 1) / (2 * Cfg::BN);   // 512-column super tiles
-  p.panel_n = 8;
-  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
-  const int max_clusters = max_quad_clusters();
-  const int clusters = num_tiles < max_clusters ? num_tiles : max_clusters;
-  prof_begin(KC_GEMM, stream);
-  gemm_bf16_4cta_kernel<<<4 * clusters, GEMM_THREADS, Cfg::SMEM_BYTES, stream>>>(tmA, tmB, p);
-  prof_end(KC_GEMM, stream, 2.0 * p.batch * (double)p.M * p.N * p.K,
-           2.0 * ((double)p.batch * p.M * p.K + (double)p.N * p.K + (double)p.batch * p.M * p.N));
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("gemm_bf16_4cta_kernel");
   return B2F_OK;
 }
 
@@ -991,38 +485,13 @@ static int gemm_bf16_impl(const void* A, int64_t lda, int64_t a_bs, const void* 
     }
   }
 
-  const long long num_m = (long long)batch * ((M + BLOCK_M - 1) / BLOCK_M);
-  const bool use256 = num_m * ((N + 255) / 256) >= device_info().num_sms && N >= 256;
   CUtensorMap tmA, tmB;
-  // CTA-pair kernel for the large projections (>= one full wave of 256x256 pair tiles)
-  static const int mode_2cta = [] { const char* v = getenv("B2F_GEMM_2CTA"); return v ? atoi(v) : B2F_GEMM_2CTA_DEFAULT; }();
-  const long long pair_tiles = (long long)batch * ((M + 255) / 256) * ((N + 255) / 256);
-  if (mode_2cta && N >= 256 && pair_tiles >= device_info().num_sms / 2) {
-    // mode 2: 4-CTA clusters (two pairs sharing A by TMA multicast) when there is at least a wave of super tiles
-    const bool quad = mode_2cta == 2 && N >= 512 && max_quad_clusters() > 0 &&
-                      (long long)batch * ((M + 255) / 256) * ((N + 511) / 512) >= max_quad_clusters();
-    int rc2 = make_tmap_3d_rows(&tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)batch, (uint64_t)lda,
-                                batch > 1 ? (uint64_t)a_bs : (uint64_t)M * lda, quad ? 64 : 128);
-    if (rc2 != B2F_OK) return rc2;
-    // tile width: 192 instead of 256 when that packs the waves better (cost ~ waves x tile width); plain epilogues only
-    static const int allow_n192 = [] { const char* v = getenv("B2F_GEMM_N192"); return v ? atoi(v) : 1; }();
-    const long long m_tiles = (long long)batch * ((M + 255) / 256), n_pairs = device_info().num_sms / 2;
-    const long long waves256 = (m_tiles * ((N + 255) / 256) + n_pairs - 1) / n_pairs;
-    const long long waves192 = (m_tiles * ((N + 191) / 192) + n_pairs - 1) / n_pairs;
-    const bool n192 = allow_n192 && !quad && epilogue != B2F_EPI_QKV_NORM_ROPE && (N % 192) == 0 &&
-                      waves192 * 192 * 100 < waves256 * 256 * 95;
-    rc2 = make_tmap_2d_bf16(&tmB, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, n192 ? 96 : 128, BLOCK_K);
-    if (rc2 != B2F_OK) return rc2;
-    if (n192) return launch_gemm_2cta_n192(tmA, tmB, p, stream);
-    return quad ? launch_gemm_4cta(tmA, tmB, p, stream) : launch_gemm_2cta<0>(tmA, tmB, p, stream);
-  }
   int rc = make_tmap_3d_rows(&tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)batch, (uint64_t)lda,
                              batch > 1 ? (uint64_t)a_bs : (uint64_t)M * lda);
   if (rc != B2F_OK) return rc;
-  rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, use256 ? 256 : 128,
-                         BLOCK_K);
+  rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, BLOCK_N, BLOCK_K);
   if (rc != B2F_OK) return rc;
-  return use256 ? launch_gemm<256>(tmA, tmB, p, stream) : launch_gemm<128>(tmA, tmB, p, stream);
+  return launch_gemm<0>(tmA, tmB, p, stream);
 }
 
 int gemm_bf16(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
@@ -1063,17 +532,12 @@ int gemm_dgrad(const void* dY, int64_t ldy, int64_t dy_bs, const void* W, int64_
   p.ldr = ld_aux;
   p.resid_bs = aux_bs;
   CUtensorMap tmA, tmB;
-  const long long pair_tiles = (long long)batch * ((M + 255) / 256) * ((N + 255) / 256);
-  const bool pair = N >= 256 && pair_tiles >= device_info().num_sms / 2;
   int rc = make_tmap_3d_rows(&tmA, dY, (uint64_t)K, (uint64_t)M, (uint64_t)batch, (uint64_t)ldy,
                              batch > 1 ? (uint64_t)dy_bs : (uint64_t)M * ldy);
   if (rc != B2F_OK) return rc;
   rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)K, (uint64_t)N, (uint64_t)ldw, 64, 64);   // 64 (k) x 64 (n) boxes
   if (rc != B2F_OK) return rc;
-  if (pair) return launch_gemm_2cta<1>(tmA, tmB, p, stream);
-  const long long num_m = (long long)batch * ((M + BLOCK_M - 1) / BLOCK_M);
-  const bool use256 = num_m * ((N + 255) / 256) >= device_info().num_sms && N >= 256;
-  return use256 ? launch_gemm<256, 1>(tmA, tmB, p, stream) : launch_gemm<128, 1>(tmA, tmB, p, stream);
+  return launch_gemm<1>(tmA, tmB, p, stream);
 }
 
 // dW[M, N] (+)= sum_b dY[b, :, M]^T . X[b, :, N]  (fp32 output, contraction over the `rows` tokens of every batch
@@ -1104,11 +568,7 @@ int gemm_wgrad(const void* dY, int64_t ldy, int64_t dy_bs, const void* X, int64_
   rc = make_tmap_3d_rows(&tmB, X, (uint64_t)N, (uint64_t)rows, (uint64_t)batch, (uint64_t)ldx,
                          batch > 1 ? (uint64_t)x_bs : (uint64_t)rows * ldx, 64);
   if (rc != B2F_OK) return rc;
-  const long long pair_tiles = (long long)((M + 255) / 256) * ((N + 255) / 256);
-  if (N >= 256 && pair_tiles >= device_info().num_sms / 2) return launch_gemm_2cta<2>(tmA, tmB, p, stream);
-  const long long num_m = (M + BLOCK_M - 1) / BLOCK_M;
-  const bool use256 = num_m * ((N + 255) / 256) >= device_info().num_sms && N >= 256;
-  return use256 ? launch_gemm<256, 2>(tmA, tmB, p, stream) : launch_gemm<128, 2>(tmA, tmB, p, stream);
+  return launch_gemm<2>(tmA, tmB, p, stream);
 }
 
 int gemm_qkv_norm_rope(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,

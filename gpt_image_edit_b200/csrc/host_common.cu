@@ -28,7 +28,7 @@ const DeviceInfo& device_info() {
     cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
     cudaDeviceGetAttribute(&info.num_sms, cudaDevAttrMultiProcessorCount, dev);
     cudaDeviceGetAttribute(&info.max_smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
-    info.ok = (major == 10) && info.num_sms > 0;
+    info.ok = (major == 9) && info.num_sms > 0;
   });
   return info;
 }

@@ -1,10 +1,10 @@
 // FLUX VAE (diffusers AutoencoderKL, SURVEY.md A.4) encode / decode composed from libb2f kernels.
 // Activations are NHWC bf16 inside; the ABI takes and returns the NCHW tensors the reference passes
 // (univa/utils/flux_pipeline.py:600-613 encode -> latent_dist, :1127-1129 decode).
-//   3x3 convs            tcgen05 implicit GEMM (conv.cu), residual add fused into conv2's epilogue
-//   1x1 shortcut convs   plain tcgen05 GEMM over [pixels, C]
+//   3x3 convs            wgmma implicit GEMM (conv.cu), residual add fused into conv2's epilogue
+//   1x1 shortcut convs   plain wgmma GEMM over [pixels, C]
 //   GroupNorm+SiLU       two HBM-bound passes (vae_kernels.cu)
-//   mid-block attention  single head, dh = C: QK^T and PV as tcgen05 GEMMs around a row softmax
+//   mid-block attention  single head, dh = C: QK^T and PV as wgmma GEMMs around a row softmax
 #include <map>
 #include <string>
 #include <vector>

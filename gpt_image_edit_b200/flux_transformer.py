@@ -2,7 +2,7 @@
 (`model.denoise_tower.denoiser`, a diffusers `FluxTransformer2DModel`; reference
 univa/serve/cli.py:64-68, univa/models/modeling_univa_denoise_tower.py:21) — same call signature,
 config attributes and state-dict key names, but the forward is a single C-ABI call into libb2f
-(`b2f_flux_forward`, hand-written sm_100a kernels).  Nothing here computes the model in torch.
+(`b2f_flux_forward`, hand-written sm_90a kernels).  Nothing here computes the model in torch.
 
 Storage: projections that the engine runs as one GEMM (q/k/v, the single block's q/k/v/proj_mlp,
 every AdaLN linear) are STORED row-concatenated; `state_dict()` / `load_state_dict()` expose and

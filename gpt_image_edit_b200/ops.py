@@ -32,7 +32,7 @@ def _as3(t: torch.Tensor) -> torch.Tensor:
 
 
 def linear(x, weight, bias=None, *, epilogue: int = EPI_BIAS, out=None, resid=None, gate=None) -> torch.Tensor:
-    """out = epilogue(x @ weight^T + bias) via b2f_gemm_bf16 (tcgen05).
+    """out = epilogue(x @ weight^T + bias) via b2f_gemm_bf16 (wgmma).
 
     x: [M,K] or [B,M,K] (any batch/row pitch); weight [N,K]; gate [B,N] for EPI_GATE_RESID."""
     _req(x, "x")

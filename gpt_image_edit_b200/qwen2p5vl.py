@@ -3,7 +3,7 @@ compute behind `UnivaQwen2p5VLForConditionalGeneration.forward(output_type="deno
 (reference univa/models/qwen2p5vl/modeling_univa_qwen2p5vl.py:325-530; arithmetic from
 transformers' Qwen2_5_VL modules, SURVEY.md Appendix B).
 
-Every matmul is `b2f_gemm_bf16` (tcgen05), every attention is `b2f_attention_fwd` (causal GQA for
+Every matmul is `b2f_gemm_bf16` (wgmma), every attention is `b2f_attention_fwd` (causal GQA for
 the decoder; windowed / full bidirectional for the ViT, head_dim 80 zero-padded to 128 in the weight
 layout so no activation is ever re-laid-out), norms / RoPE / SwiGLU / gathers are the HBM-bound
 kernels of csrc/llm_kernels.cu.  Python here only sequences C-ABI calls and does integer position
@@ -461,7 +461,7 @@ class B200Qwen2p5VL(torch.nn.Module):
         return ops.rmsnorm(x, W["model.norm"], eps=tc.rms_norm_eps)
 
     def lm_logits(self, hidden):
-        """lm_head on [n, hidden] -> [n, vocab] bf16 (tcgen05 GEMM; vocab rows stream once from HBM)."""
+        """lm_head on [n, hidden] -> [n, vocab] bf16 (wgmma GEMM; vocab rows stream once from HBM)."""
         return ops.linear(hidden.reshape(-1, self.tc.hidden_size), self.W["lm_head"])
 
     @torch.no_grad()

@@ -13,8 +13,8 @@ Replaces `pipe.text_encoder_2` (transformers `T5EncoderModel`) and `pipe.text_en
                     hidden state at argmax(input_ids) (config eos_token_id == 2 legacy rule, which
                     is what FLUX.1's text_encoder/config.json carries)
 
-Every matmul is the tcgen05 GEMM (`b2f_gemm_bf16`, residual adds and quick-GELU fused into the
-epilogue), attention is the FA-style tcgen05 kernel with head_dim 64 zero-padded to the 128-wide
+Every matmul is the wgmma GEMM (`b2f_gemm_bf16`, residual adds and quick-GELU fused into the
+epilogue), attention is the FA-style wgmma kernel with head_dim 64 zero-padded to the 128-wide
 head slot in the WEIGHT layout (so no activation is ever re-laid out) — `b2f_attention_bias_fwd`
 for T5, causal `b2f_attention_fwd` for CLIP; norms / gated-GELU / embeddings are the HBM-bound
 kernels in csrc/llm_kernels.cu.  There is no CPU path.

@@ -4,7 +4,7 @@ What the reference assembles from accelerate + DeepSpeed ZeRO-2 + torch.autograd
 
   FluxTrainGraph       forward with per-block checkpoints / backward with per-block recompute of the FLUX denoiser
                        (`b2f_flux_train_forward` / `b2f_flux_train_backward`) plus MLP2's forward / backward
-                       (two tcgen05 GEMMs each way), gradients in fp32
+                       (two wgmma GEMMs each way), gradients in fp32
   trainable_params()   the reference's trainable set (train_denoiser.py:71-119, 519-548) mapped onto this repo's
                        fused weight storage
   ShardedAdamW         ZeRO-2: gradients live in per-block buckets; each bucket is reduce-scattered (NCCL, fp32)
@@ -470,6 +470,30 @@ def compute_loss_weighting_for_sd3(weighting_scheme, sigmas):
     return torch.ones_like(sigmas)
 
 
+def optimizer_state_bytes(n_params: int, world: int) -> int:
+    """Device bytes ShardedAdamW allocates per rank for `n_params` trainable parameters: the full fp32 gradient buffer and
+    bf16 flat copy, plus this rank's 1/world slice of the reduced fp32 gradient (world > 1), fp32 master weights and the
+    two Adam moments."""
+    n = int(n_params)
+    return 4 * n + 2 * n + (4 * n // world if world > 1 else 0) + 12 * n // world
+
+
+def check_optimizer_fits(n_params: int, world: int, device: torch.device) -> None:
+    """Refuses, before allocating, a ZeRO-2 optimizer whose per-rank state exceeds the device memory still free (the model
+    weights are resident by then), and names the smallest world size whose state would fit."""
+    if device.type != "cuda":
+        return
+    free, _ = torch.cuda.mem_get_info(device)
+    need = optimizer_state_bytes(n_params, world)
+    if need <= free:
+        return
+    fits = [w for w in (2, 4, 8, 16, 32, 64) if w > world and optimizer_state_bytes(n_params, w) <= free]
+    hint = f"at least {fits[0]} ranks" if fits else "more ranks or fewer trainable parameters"
+    raise _lib.B2FError(f"ZeRO-2 state for {n_params / 1e9:.2f} B trainable parameters needs {need / 2**30:.1f} GiB per rank "
+                        f"at world size {world}, {free / 2**30:.1f} GiB of device memory is free: use {hint} "
+                        "(activation memory comes on top)")
+
+
 class Stage2Trainer:
     """`train_denoiser.py`'s loop body (:829-1181) on this engine: VAE-encode target and context, flow-matching noising,
     Qwen2.5-VL prefill (frozen) -> MLP2 -> FLUX with block checkpoints, loss, backward, ZeRO-2 AdamW step.
@@ -494,6 +518,7 @@ class Stage2Trainer:
         if tc.gradient_checkpointing:
             den.enable_gradient_checkpointing()               # always on in this engine: the backward recomputes each block
         world = dist.get_world_size(group) if (dist.is_available() and dist.is_initialized()) else 1
+        check_optimizer_fits(sum(p.storage.numel() for p in params), world, params[0].storage.device)
         comm = torch.cuda.Stream() if (overlap_comm and world > 1) else None
         self.opt = ShardedAdamW(params, lr=tc.learning_rate, betas=(tc.adam_beta1, tc.adam_beta2), eps=tc.adam_epsilon,
                                 weight_decay=tc.adam_weight_decay, max_grad_norm=tc.max_grad_norm, group=group, comm_stream=comm)

@@ -1,7 +1,7 @@
 """Drop-in for the object the reference uses as `pipe.vae` / `vae` (diffusers `AutoencoderKL` with
 the FLUX config; reference univa/utils/flux_pipeline.py:255-258, 609-611, 1128-1129;
 train_denoiser.py:428, 887-898).  encode/decode are single C-ABI calls into libb2f
-(`b2f_vae_encode` / `b2f_vae_decode`: tcgen05 implicit-GEMM convs, fused GroupNorm+SiLU passes).
+(`b2f_vae_encode` / `b2f_vae_decode`: wgmma implicit-GEMM convs, fused GroupNorm+SiLU passes).
 
 Weights are stored in the layout the kernels consume (OHWI conv weights, fused mid-attention qkv,
 padded biases); `state_dict()` / `load_state_dict()` speak the diffusers layout and key names.

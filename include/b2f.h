@@ -1,4 +1,4 @@
-/* b2f.h — C ABI of the B200-native FLUX-Kontext denoising engine (libb2f.so).
+/* b2f.h — C ABI of the H100-native FLUX-Kontext denoising engine (libb2f.so).
  *
  * The reference (wyhlovecpp/GPT-Image-Edit) has no FFI: its hot path sits behind Python object
  * protocols whose arithmetic lives in diffusers 0.32.2 / torch (SURVEY.md §8b).  Every entry
@@ -27,7 +27,7 @@ extern "C" {
 #define B2F_ERR_CUDA (-2)        /* CUDA runtime/driver error (message on stderr) */
 #define B2F_ERR_UNSUPPORTED (-3) /* shape or mode not implemented */
 #define B2F_ERR_ALIGN (-4)       /* pointer or pitch not 16-byte aligned */
-#define B2F_ERR_NODEVICE (-5)    /* no sm_100 device visible */
+#define B2F_ERR_NODEVICE (-5)    /* no sm_90 device visible */
 #define B2F_ERR_WORKSPACE (-6)   /* workspace too small */
 
 typedef void* b2f_stream_t; /* cudaStream_t */
@@ -52,7 +52,7 @@ int b2f_prof_collect(int kernel_class, double* ms, int64_t* launches, double* fl
 int b2f_prof_shapes(char* buf, int cap);
 
 /* ------------------------------------------------------------------------------------------
- * Linear layer: out[M,N] = epilogue(A[M,K] · W[N,K]^T + bias[N]).  tcgen05.mma, TMA, TMEM.
+ * Linear layer: out[M,N] = epilogue(A[M,K] · W[N,K]^T + bias[N]).  wgmma (fp32 accumulators in registers), TMA, mbarrier pipeline.
  * Replaces torch.nn.functional.linear → cuBLASLt as reached by diffusers' nn.Linear modules
  * (FluxTransformer2DModel: x_embedder, context_embedder, to_q/k/v, to_out, ff.net.*, proj_mlp,
  * proj_out, norm*.linear — SURVEY.md Appendix A.1/A.6; call site univa/utils/flux_pipeline.py:1067).
@@ -151,7 +151,7 @@ int b2f_silu(const void* x, void* y, int64_t n, b2f_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Fused softmax attention, head_dim 128:  O = softmax(Q K^T * scale [+ causal mask]) V.
- * tcgen05 QK^T and PV with S/P/O in TMEM, K/V streamed by TMA, online softmax (FA-style).
+ * wgmma QK^T and PV with S/P/O in registers, K/V streamed by TMA, online softmax (FA-style).
  * Replaces F.scaled_dot_product_attention in diffusers' FluxAttnProcessor2_0 (joint [txt;img]
  * attention of FluxTransformerBlock / FluxSingleTransformerBlock, SURVEY.md A.2; reference call
  * site univa/utils/flux_pipeline.py:1067) and flash_attn reached through
@@ -281,7 +281,7 @@ int b2f_move_rows(const void* src, int64_t ld_src, void* dst, int64_t ld_dst, co
                   int64_t n, int D, int scatter, b2f_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
- * 3x3 convolution, NHWC bf16, tcgen05 implicit GEMM (A tiles are shifted 4-D TMA boxes of the
+ * 3x3 convolution, NHWC bf16, wgmma implicit GEMM (A tiles are shifted 4-D TMA boxes of the
  * input; padding = TMA zero fill).  Replaces cuDNN conv as reached by diffusers AutoencoderKL
  * (SURVEY.md A.4).  in [N,Hin,Win,Cin] (Cin % 64 == 0), w OHWI [Cout,3,3,Cin], bias [>=8] bf16 or
  * NULL, out [N,Ho,Wo,Cout] (NHWC) or, with out_nchw, [N,Cout,Ho,Wo].  stride 1: padding 1.
@@ -315,13 +315,13 @@ int b2f_transpose_bf16(const void* in, int64_t ld_in, void* out, int64_t ld_out,
  * Activations and activation gradients are bf16, weight gradients and token reductions fp32.
  */
 /* Backward-data GEMM of nn.Linear: dX[batch, M, N] = epi(dY[batch, M, K] · W[K, N]) with W as stored ([out = K, in = N],
- * read as an MN-major tcgen05 operand: no transposed copy).  epilogue: B2F_EPI_BIAS (store), B2F_EPI_DGELU /
+ * read as an MN-major wgmma operand: no transposed copy).  epilogue: B2F_EPI_BIAS (store), B2F_EPI_DGELU /
  * B2F_EPI_DSILU (times act'(aux), aux = saved pre-activation [batch, M, N]), B2F_EPI_RESID (dX = aux + result). */
 int b2f_gemm_dgrad(const void* dY, int64_t ldy, int64_t dy_batch_stride, const void* W, int64_t ldw, void* dX,
                    int64_t ldx, int64_t dx_batch_stride, int batch, int M, int N, int K, int epilogue, const void* aux,
                    int64_t ld_aux, int64_t aux_batch_stride, b2f_stream_t stream);
 /* Backward-weight GEMM: dW[M, N] (+)= sum_b dY[b, :rows, :M]^T · X[b, :rows, :N], fp32 output (pitch ldw floats); both
- * operands are token-major activations read as MN-major tcgen05 operands. */
+ * operands are token-major activations read as MN-major wgmma operands. */
 int b2f_gemm_wgrad(const void* dY, int64_t ldy, int64_t dy_batch_stride, const void* X, int64_t ldx,
                    int64_t x_batch_stride, float* dW, int64_t ldw, int batch, int rows, int M, int N, int accumulate,
                    b2f_stream_t stream);
@@ -335,7 +335,7 @@ int b2f_attention_fwd_lse(const void* q, int64_t ldq, const void* k, int64_t ldk
 int b2f_attn_delta(const void* o, int64_t ldo, const void* dout, int64_t lddo, float* delta, float* lse, int B, int H,
                    int S, int S_pad, b2f_stream_t stream);
 /* Attention backward (non-causal, H == Hkv, head_dim 128): dq, dk, dv from q, k, v, dout, lse2 and delta.  Two
- * tcgen05 kernels (dK/dV with the scores held transposed in TMEM; dQ), no atomics: bit-reproducible.  All tensors
+ * wgmma kernels (dK/dV with the scores held transposed in registers; dQ), no atomics: bit-reproducible.  All tensors
  * token-major [B, S, H*128] views.  S_pad: pitch of the lse / delta rows, a multiple of 128. */
 int b2f_attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
                       const void* dout, int64_t lddo, const float* lse, const float* delta, int64_t S_pad, void* dq,

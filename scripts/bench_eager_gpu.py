@@ -1,5 +1,5 @@
 """Whole-path GPU comparator (context, NOT the reference arm): one C1024 MMDiT forward of the bf16 oracle on the same
-B200 — the reference's op sequence through the libraries it would use on a GPU (cuBLAS nn.Linear, cuDNN / flash SDPA,
+GPU — the reference's op sequence through the libraries it would use on a GPU (cuBLAS nn.Linear, cuDNN / flash SDPA,
 ATen norm and elementwise chains) — next to this engine's `b2f_flux_forward` on identical weights and inputs.
 
     python scripts/bench_eager_gpu.py [--height 1024 --width 1024 --steps 5]     -> gpurun_out/eager_gpu_step.json

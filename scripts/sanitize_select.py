@@ -1,5 +1,5 @@
 """Node ids of the toy-shape GPU tests scripts/sanitize.sh runs under compute-sanitizer: every kernel family that
-hand-rolls mbarrier / TMEM / cluster protocols, at shapes small enough for a 10-100x slowdown."""
+hand-rolls mbarrier / wgmma pipelines, at shapes small enough for a 10-100x slowdown."""
 import subprocess
 import sys
 

@@ -1,4 +1,4 @@
-"""GPU parity: b2f_gemm_bf16 (tcgen05) against a torch fp32 reference of the same op.
+"""GPU parity: b2f_gemm_bf16 (wgmma) against a torch fp32 reference of the same op.
 
 Tolerance: inputs are bf16, accumulation fp32, one bf16 rounding on the output, so the result must
 match round_bf16(fp32 reference) to within 1 bf16 ulp of the largest magnitude in the row-block

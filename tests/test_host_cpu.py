@@ -16,7 +16,7 @@ def test_library_loads_and_exports_every_declared_symbol():
         assert hasattr(_lib.lib, name), f"libb2f.so does not export {name}"
     assert set(declared) == set(_lib._SIGNATURES), "ctypes signatures out of sync with include/b2f.h"
     assert _lib.lib.b2f_version() >= 1
-    assert _lib.lib.b2f_strerror(-5).decode() == "no sm_100 device"
+    assert _lib.lib.b2f_strerror(-5).decode() == "no sm_90 device"
 
 
 def test_no_cpu_fallback_paths():

@@ -5,7 +5,7 @@ autograd over diffusers' modules).
 Every gradient the engine produces — the reference's trainable set (train_denoiser.py:71-119) plus MLP2 — is compared
 with the fp32 oracle's autograd on identical bf16-rounded weights; the torch-bf16 autograd of the same oracle is
 compared with the fp32 one as well, and the engine's error must stay within 2x torch-bf16's + 1e-2 (the rule
-DESIGN.md section 3 uses for composed models).
+used for composed models).
 """
 from types import SimpleNamespace
 

@@ -192,7 +192,7 @@ def main(conf):
     from univa.training.synthetic_data import SyntheticEditDataset, collate
 
     if not torch.cuda.is_available():
-        raise SystemExit("train_denoiser.py runs on B200s through libb2f; there is no CPU path")
+        raise SystemExit("train_denoiser.py runs on H100s through libb2f; there is no CPU path")
     tc, dc, mc = conf.training_config, conf.dataset_config, conf.model_config
     world, rank, local_rank = D.env_world()
     device = torch.device("cuda", local_rank)

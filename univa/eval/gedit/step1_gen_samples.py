@@ -75,7 +75,7 @@ def run_model_and_return_samples(args: EvalConfig, state: dict, prompt_text: str
 
 def main(args: EvalConfig):
     if not torch.cuda.is_available():
-        raise SystemExit("the sampling driver runs on B200s through libb2f; there is no CPU path")
+        raise SystemExit("the sampling driver runs on H100s through libb2f; there is no CPU path")
     world, rank, local_rank = D.env_world()
     device = torch.device("cuda", local_rank)
     torch.cuda.set_device(device)

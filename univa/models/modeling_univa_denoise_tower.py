@@ -3,7 +3,7 @@
 
   .denoiser            B200FluxTransformer2DModel  (handed to the pipeline, reference cli.py:64-68)
   .denoise_projector   Linear(in, 3*out) · SiLU · Linear(3*out, out)   ("mlp2x_gelu" — the activation IS
-                       SiLU in the reference, :33-43), run as two tcgen05 GEMMs with the SiLU fused
+                       SiLU in the reference, :33-43), run as two wgmma GEMMs with the SiLU fused
   .forward(...)        training-time glue (:49-110): concat [vlm embeds, prefix T5 embeds], zero txt_ids,
                        call the denoiser, return sample
 State-dict keys: `denoiser.*` and `denoise_projector.{0,2}.{weight,bias}` as in the reference checkpoint

@@ -255,7 +255,7 @@ def reply_text(token_ids, processor=None):
 
 def main(args):
     if not torch.cuda.is_available():
-        raise SystemExit("univa.serve.cli runs on a B200 through libb2f; there is no CPU path")
+        raise SystemExit("univa.serve.cli runs on an H100 through libb2f; there is no CPU path")
     device = torch.device("cuda")
     model, task_head, processor = load_main_model_and_processor(args.model_path, device, args.synthetic, args.small)
     pipe, tokenizers, text_encoders = load_pipe(model.denoise_tower.denoiser, args.flux_path, device, args.synthetic, args.small)
