@@ -29,11 +29,11 @@ def _randn(*shape, g, scale=1.0):
 @pytest.mark.parametrize("B,M,N,K", [
     (1, 128, 128, 64),        # one tile, one k-block
     (1, 200, 136, 72),        # ragged everything
-    (2, 300, 256, 512),       # batched rows, 1-CTA 128-wide kernel
-    (1, 2336, 3072, 3072),    # to_out dgrad at 512^2 (pair kernel)
-    (1, 2336, 3072, 9216),    # QKV dgrad (pair kernel, long K)
-    (2, 1024, 1024, 4096),    # pair kernel with batch
-    (1, 4736, 512, 256),      # 1-CTA 256-wide kernel
+    (2, 300, 256, 512),       # batched rows with a ragged last m-block; 8 k-blocks: two turns of the 4-stage ring
+    (1, 2336, 3072, 3072),    # to_out dgrad at 512^2: 24 n-blocks (a panel of 16 and one of 8), 48 k-blocks
+    (1, 2336, 3072, 9216),    # QKV dgrad: long K (144 k-blocks)
+    (2, 1024, 1024, 4096),    # batch 2 with whole m-blocks, 8 n-blocks in one partial panel
+    (1, 4736, 512, 256),      # 37 m-blocks, narrow N, exactly one turn of the ring
 ])
 def test_gemm_dgrad(B, M, N, K):
     from gpt_image_edit_b200 import train_ops as T
@@ -71,12 +71,12 @@ def test_gemm_dgrad_pitched_views_and_epilogues():
 
 
 @pytest.mark.parametrize("B,rows,M,N", [
-    (1, 64, 128, 128),
-    (1, 100, 136, 200),       # ragged: token tail inside a 64-row box, M/N tails
-    (3, 150, 256, 384),       # contraction over three batch items with a ragged tail each
-    (1, 2336, 3072, 3072),    # to_out wgrad at 512^2 (pair kernel)
-    (2, 1000, 1024, 4608),    # pair kernel, batch 2
-    (1, 288, 12288, 3584),    # MLP2 first linear
+    (1, 64, 128, 128),        # one tile, one 64-token k-block
+    (1, 100, 136, 200),       # ragged: token tail inside the second 64-row k-block, M/N tails
+    (3, 150, 256, 384),       # contraction over three batch items with a ragged third k-block each
+    (1, 2336, 3072, 3072),    # to_out wgrad at 512^2: 37 k-blocks (the ring wraps), 24 n-blocks in two panels
+    (2, 1000, 1024, 4608),    # batch 2, 16 k-blocks per item with a tail; 36 n-blocks: two full panels and 4
+    (1, 288, 12288, 3584),    # MLP2 first linear: 96 m-blocks
 ])
 def test_gemm_wgrad(B, rows, M, N):
     from gpt_image_edit_b200 import train_ops as T
@@ -121,7 +121,7 @@ def _attn_ref(q, k, v, do):
     (1, 128, 1),     # one block
     (1, 256, 2),
     (2, 200, 2),     # ragged tail
-    (1, 1000, 3),    # pair forward kernel (>= 512 rows), ragged
+    (1, 1000, 3),    # 8 query tiles / K/V blocks (slot reuse), ragged tail of 104 rows
     (1, 2336, 2),    # S of the 512^2 training config
 ])
 def test_attention_lse_and_backward(B, S, H):
