@@ -59,6 +59,8 @@ _SIGNATURES = {
     "b2f_rmsnorm_rope": (_i32, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, C.c_float, _vp]),
     "b2f_euler_step": (_i32, [_vp, _i64, _vp, _i64, _i64, _i32, C.c_float, _vp]),
     "b2f_silu": (_i32, [_vp, _vp, _i64, _vp]),
+    "b2f_temb_sinusoid": (_i32, [_vp, _vp, _i32, _vp]),
+    "b2f_temb_combine": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp]),
     "b2f_rope_tables": (_i32, [_vp, _i32, C.POINTER(_i32), C.c_double, _vp, _vp, _vp]),
     "b2f_rmsnorm": (_i32, [_vp, _i64, _vp, _vp, _i64, _i64, _i32, C.c_float, _vp]),
     "b2f_rope_half": (_i32, [_vp, _i64, _i32, _i32, _vp, _vp, _i32, _i64, _i32, _vp]),

@@ -25,6 +25,9 @@ int rmsnorm_rope(void* q, void* k, int64_t ld, int64_t batch_stride, const void*
 int euler_step(void* x, int64_t ldx, const void* v, int64_t ldv, int64_t rows, int cols, float dt,
                cudaStream_t stream);
 int silu(const void* x, void* y, int64_t n, cudaStream_t stream);
+int temb_sinusoid(const float* t, void* out, int rows, cudaStream_t stream);
+int temb_combine(const void* t, const void* g, const void* txt, void* temb, void* silu_temb, int64_t n,
+                 cudaStream_t stream);
 void prof_set(bool on);
 int rmsnorm(const void* x, int64_t ldx, const void* w, void* y, int64_t ldy, int64_t rows, int D,
             float eps, cudaStream_t stream);
@@ -243,6 +246,13 @@ int b2f_move_rows(const void* src, int64_t ld_src, void* dst, int64_t ld_dst, co
 
 int b2f_silu(const void* x, void* y, int64_t n, b2f_stream_t stream) {
   return b2f::silu(x, y, n, static_cast<cudaStream_t>(stream));
+}
+int b2f_temb_sinusoid(const float* t, void* out, int rows, b2f_stream_t stream) {
+  return b2f::temb_sinusoid(t, out, rows, static_cast<cudaStream_t>(stream));
+}
+int b2f_temb_combine(const void* t, const void* g, const void* txt, void* temb, void* silu_temb, int64_t n,
+                     b2f_stream_t stream) {
+  return b2f::temb_combine(t, g, txt, temb, silu_temb, n, static_cast<cudaStream_t>(stream));
 }
 
 int b2f_attention_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,

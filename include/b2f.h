@@ -149,6 +149,15 @@ int b2f_rope_tables(const float* ids, int S, const int* axes_dim, double theta, 
  * linear (SURVEY.md A.1). */
 int b2f_silu(const void* x, void* y, int64_t n, b2f_stream_t stream);
 
+/* The two row kernels of b2f_flux_temb, exposed on their own so they can be checked element by element.
+ * Timestep projection (Timesteps(256, flip_sin_to_cos=True, shift 0)): t fp32 DEVICE [rows] ->
+ * out bf16 [rows, 256] = [cos(t f) | sin(t f)], f_j = exp(-ln(10000) j / 128), fp32 math.
+ * Combine: temb = bf16(bf16(t + g) + txt) (g may be null: bf16(t + txt)), silu_temb = bf16(silu(temb)),
+ * all bf16 contiguous of n elements (n % 8 == 0). */
+int b2f_temb_sinusoid(const float* t, void* out, int rows, b2f_stream_t stream);
+int b2f_temb_combine(const void* t, const void* g, const void* txt, void* temb, void* silu_temb, int64_t n,
+                     b2f_stream_t stream);
+
 /* ------------------------------------------------------------------------------------------
  * Fused softmax attention, head_dim 128:  O = softmax(Q K^T * scale [+ causal mask]) V.
  * wgmma QK^T and PV with S/P/O in registers, K/V streamed by TMA, online softmax (FA-style).
