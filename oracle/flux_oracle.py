@@ -167,7 +167,8 @@ def apply_rotary_emb(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor) -> t
     cos, sin = cos[None, None], sin[None, None]
     xr, xi = x.reshape(*x.shape[:-1], -1, 2).unbind(-1)
     x_rot = torch.stack([-xi, xr], dim=-1).flatten(3)
-    return (x.float() * cos + x_rot.float() * sin).to(x.dtype)
+    ct = torch.promote_types(x.dtype, torch.float32)          # fp32 for 16-bit inputs, fp64 stays fp64
+    return (x.to(ct) * cos + x_rot.to(ct) * sin).to(x.dtype)
 
 
 def rms_norm(x: torch.Tensor, weight: torch.Tensor, eps: float = 1e-6) -> torch.Tensor:
@@ -229,9 +230,16 @@ def double_block(sd, i, cfg, x, c, temb, cos, sin, attn_mask=None):
     """`FluxTransformerBlock.forward` (A.1)."""
     p = f"transformer_blocks.{i}."
     e = _lin(sd, p + "norm1.linear", F.silu(temb))
+    ec = _lin(sd, p + "norm1_context.linear", F.silu(temb))
+    return double_block_mod(sd, i, cfg, x, c, e, ec, cos, sin, attn_mask)
+
+
+def double_block_mod(sd, i, cfg, x, c, e, ec, cos, sin, attn_mask=None):
+    """`double_block` after its two AdaLN linears: e / ec [B, 6d] are the image / text modulation rows
+    (shift, scale, gate of the attention, then of the MLP)."""
+    p = f"transformer_blocks.{i}."
     shift_msa, scale_msa, gate_msa, shift_mlp, scale_mlp, gate_mlp = e.chunk(6, dim=1)
     xn = layer_norm(x) * (1 + scale_msa[:, None]) + shift_msa[:, None]
-    ec = _lin(sd, p + "norm1_context.linear", F.silu(temb))
     c_shift_msa, c_scale_msa, c_gate_msa, c_shift_mlp, c_scale_mlp, c_gate_mlp = ec.chunk(6, dim=1)
     cn = layer_norm(c) * (1 + c_scale_msa[:, None]) + c_shift_msa[:, None]
 
@@ -251,8 +259,13 @@ def double_block(sd, i, cfg, x, c, temb, cos, sin, attn_mask=None):
 
 def single_block(sd, i, cfg, h, temb, cos, sin, attn_mask=None):
     """`FluxSingleTransformerBlock.forward` (A.1)."""
+    e = _lin(sd, f"single_transformer_blocks.{i}.norm.linear", F.silu(temb))
+    return single_block_mod(sd, i, cfg, h, e, cos, sin, attn_mask)
+
+
+def single_block_mod(sd, i, cfg, h, e, cos, sin, attn_mask=None):
+    """`single_block` after its AdaLN linear: e [B, 3d] is the modulation row (shift, scale, gate)."""
     p = f"single_transformer_blocks.{i}."
-    e = _lin(sd, p + "norm.linear", F.silu(temb))
     shift, scale, gate = e.chunk(3, dim=1)
     hn = layer_norm(h) * (1 + scale[:, None]) + shift[:, None]
     m = F.gelu(_lin(sd, p + "proj_mlp", hn), approximate="tanh")
