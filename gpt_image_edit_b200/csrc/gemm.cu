@@ -1,14 +1,23 @@
-// Warp-specialised bf16 GEMM for sm_90a:  out[M,N] = epi(A[M,K] · W[N,K]^T + bias).
+// Persistent, warp-specialised bf16 GEMM for sm_90a with ping-pong consumers:  out[M,N] = epi(A[M,K] · W[N,K]^T + bias).
 //
-//   warpgroup 0 (1 lane)  TMA producer      cp.async.bulk.tensor → 128B-swizzled smem ring
-//   warpgroups 1, 2       wgmma consumers   m64n128k16, 64 rows of the 128 x 128 tile each, fp32 in registers
-//   epilogue              accumulators staged in smem → bias/act/gate/resid → global, one row per thread
+//   grid                  min(tiles, SMs) CTAs; CTA b takes the 128 x 128 tiles b, b + grid, ... in panel order
+//   warpgroup 0 (1 lane)  TMA producer      cp.async.bulk.tensor → 128B-swizzled smem ring of STAGES stages, streamed
+//                                           across tile boundaries (setmaxnreg.dec to 40 registers)
+//   warpgroups 1, 2       wgmma consumers   each owns whole tiles, alternating (the CTA's tiles 0, 2, ... / 1, 3, ...):
+//                                           two m64n128k16 per k16 step, 128 fp32 accumulators per thread
+//                                           (setmaxnreg.inc to 232); named barriers make them take turns on the main
+//                                           loop, so one runs its MMAs while the other runs its epilogue
+//   epilogue              x = bf16(acc + bias) from registers → the consumer's own bf16 staging tile →
+//                         act/gate/resid → global with 16-byte accesses, 16 threads per row; a fused QKV head runs one
+//                         thread per row; the fp32 wgrad output goes straight from registers
 //
+// Every output element sees the same k16 accumulation order as a one-tile-per-CTA kernel with the same k-blocks.
 // Both operands of the forward GEMM are K-major ([rows, K] row-major), which is what nn.Linear stores
-// (SURVEY.md A.6) — no transposes anywhere.  The building blocks are shared with conv.cu (gemm_sm90.cuh).
+// (SURVEY.md A.6) — no transposes anywhere.  The tile shape and ring layout are shared with conv.cu (gemm_sm90.cuh).
 //
 // Replaces: torch.nn.functional.linear → cuBLASLt (diffusers FluxTransformer2DModel linears,
 // reference call site univa/utils/flux_pipeline.py:1067; SURVEY.md §2b row 1).
+#include <algorithm>
 #include <atomic>
 #include <cstdlib>
 
@@ -90,306 +99,419 @@ __device__ __forceinline__ float dsilu_f(float x) {
   return s * (1.0f + x * (1.0f - s));
 }
 
-// Epilogue for 32 accumulator columns of one output row: bias / activation / gate / residual with the
-// bf16 rounding points of the torch-eager chain, then 16-byte stores.
-__device__ __forceinline__ void epilogue_chunk(const GemmParams& p, const int epi, const uint32_t (&acc)[32], int n0,
-                                               __nv_bfloat16* out_row, const __nv_bfloat16* res_row,
-                                               const __nv_bfloat16* gate_row) {
+// Epilogue of one 8-column group of one output row from x = bf16(acc + bias) (bf16(acc) without a bias):
+// activation / gate / residual with the bf16 rounding points of the torch-eager chain, then one 16-byte store.
+// Every chain starts by rounding acc + bias to bf16, which the staging tile already did; rounding x again is exact.
+// rq: the 8 residual (GATE_RESID / RESID) or saved pre-activation (DGELU / DSILU) values, gq: the 8 gate values.
+__device__ __forceinline__ void epilogue_group(const int epi, float (&v)[8], const uint4 rq, const uint4 gq,
+                                               __nv_bfloat16* out) {
+  if (epi == B2F_EPI_GELU_TANH) {
 #pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    const int n = n0 + g * 8;
-    if (n >= p.N) break;
-    float v[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) v[j] = __uint_as_float(acc[g * 8 + j]);
-    if (p.bias) {
-      const uint4 bq = __ldg(reinterpret_cast<const uint4*>(p.bias + n));
-      const uint32_t bw[4] = {bq.x, bq.y, bq.z, bq.w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 b2 = unpack_bf16x2(bw[j]);
-        v[2 * j] += b2.x;
-        v[2 * j + 1] += b2.y;
-      }
+    for (int j = 0; j < 8; j += 2) {
+      bf16r2(v[j], v[j + 1]);            // packed rounding (the scalar conversion runs on the slow XU pipe)
+      v[j] = gelu_tanh_f(v[j]);
+      v[j + 1] = gelu_tanh_f(v[j + 1]);
     }
-    if (epi == B2F_EPI_GELU_TANH) {
+  } else if (epi == B2F_EPI_GELU_ERF) {
 #pragma unroll
-      for (int j = 0; j < 8; j += 2) {
-        bf16r2(v[j], v[j + 1]);            // packed rounding (the scalar conversion runs on the slow XU pipe)
-        v[j] = gelu_tanh_f(v[j]);
-        v[j + 1] = gelu_tanh_f(v[j + 1]);
-      }
-    } else if (epi == B2F_EPI_GELU_ERF) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float x = bf16r(v[j]);
-        v[j] = 0.5f * x * (1.0f + erff(x * 0.70710678118654752f));
-      }
-    } else if (epi == B2F_EPI_SILU) {
-#pragma unroll
-      for (int j = 0; j < 8; j += 2) {
-        bf16r2(v[j], v[j + 1]);
-        v[j] = silu_f(v[j]);
-        v[j + 1] = silu_f(v[j + 1]);
-      }
-    } else if (epi == B2F_EPI_QUICK_GELU) {
-      // transformers QuickGELUActivation in bf16 eager: x * sigmoid(1.702 * x), each op rounded
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float x = bf16r(v[j]);
-        const float t = bf16r(1.702f * x);
-        v[j] = x * bf16r(1.0f / (1.0f + __expf(-t)));
-      }
-    } else if (epi == B2F_EPI_GATE_RESID) {
-      const uint4 gq = __ldg(reinterpret_cast<const uint4*>(gate_row + n));
-      const uint4 rq = *reinterpret_cast<const uint4*>(res_row + n);
-      const uint32_t gw[4] = {gq.x, gq.y, gq.z, gq.w};
-      const uint32_t rw[4] = {rq.x, rq.y, rq.z, rq.w};
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 g2 = unpack_bf16x2(gw[j]);
-        const float2 r2 = unpack_bf16x2(rw[j]);
-        float y0 = v[2 * j], y1 = v[2 * j + 1];
-        bf16r2(y0, y1);
-        y0 *= g2.x;
-        y1 *= g2.y;
-        bf16r2(y0, y1);
-        v[2 * j] = r2.x + y0;
-        v[2 * j + 1] = r2.y + y1;
-      }
+    for (int j = 0; j < 8; ++j) {
+      const float x = bf16r(v[j]);
+      v[j] = 0.5f * x * (1.0f + erff(x * 0.70710678118654752f));
     }
-    else if (epi == B2F_EPI_DGELU || epi == B2F_EPI_DSILU) {
-      // backward of the activation fused into the dgrad GEMM: out = bf16(acc) * act'(u), u = the saved
-      // pre-activation (read through the resid pointer)
-      const uint4 uq = *reinterpret_cast<const uint4*>(res_row + n);
-      const uint32_t uw[4] = {uq.x, uq.y, uq.z, uq.w};
+  } else if (epi == B2F_EPI_SILU) {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 u2 = unpack_bf16x2(uw[j]);
-        const float d0 = epi == B2F_EPI_DGELU ? dgelu_tanh_f(u2.x) : dsilu_f(u2.x);
-        const float d1 = epi == B2F_EPI_DGELU ? dgelu_tanh_f(u2.y) : dsilu_f(u2.y);
-        v[2 * j] = bf16r(v[2 * j]) * d0;
-        v[2 * j + 1] = bf16r(v[2 * j + 1]) * d1;
-      }
-    } else if (epi == B2F_EPI_F32 || epi == B2F_EPI_F32_ACC) {
-      float* o = reinterpret_cast<float*>(out_row) + n;
-      float4 a0 = make_float4(v[0], v[1], v[2], v[3]), a1 = make_float4(v[4], v[5], v[6], v[7]);
-      if (epi == B2F_EPI_F32_ACC) {
-        const float4 p0 = *reinterpret_cast<const float4*>(o), p1 = *reinterpret_cast<const float4*>(o + 4);
-        a0.x += p0.x; a0.y += p0.y; a0.z += p0.z; a0.w += p0.w;
-        a1.x += p1.x; a1.y += p1.y; a1.z += p1.z; a1.w += p1.w;
-      }
-      *reinterpret_cast<float4*>(o) = a0;
-      *reinterpret_cast<float4*>(o + 4) = a1;
-      continue;
+    for (int j = 0; j < 8; j += 2) {
+      bf16r2(v[j], v[j + 1]);
+      v[j] = silu_f(v[j]);
+      v[j + 1] = silu_f(v[j + 1]);
     }
-    else if (epi == B2F_EPI_RESID) {
-      const uint4 rq = *reinterpret_cast<const uint4*>(res_row + n);
-      const uint32_t rw[4] = {rq.x, rq.y, rq.z, rq.w};
+  } else if (epi == B2F_EPI_QUICK_GELU) {
+    // transformers QuickGELUActivation in bf16 eager: x * sigmoid(1.702 * x), each op rounded
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const float2 r2 = unpack_bf16x2(rw[j]);
-        float y0 = v[2 * j], y1 = v[2 * j + 1];
-        bf16r2(y0, y1);
-        v[2 * j] = r2.x + y0;
-        v[2 * j + 1] = r2.y + y1;
-      }
+    for (int j = 0; j < 8; ++j) {
+      const float x = bf16r(v[j]);
+      const float t = bf16r(1.702f * x);
+      v[j] = x * bf16r(1.0f / (1.0f + __expf(-t)));
     }
-    uint4 o;
-    o.x = pack_bf16x2(v[0], v[1]);
-    o.y = pack_bf16x2(v[2], v[3]);
-    o.z = pack_bf16x2(v[4], v[5]);
-    o.w = pack_bf16x2(v[6], v[7]);
-    *reinterpret_cast<uint4*>(out_row + n) = o;
+  } else if (epi == B2F_EPI_GATE_RESID) {
+    const uint32_t gw[4] = {gq.x, gq.y, gq.z, gq.w};
+    const uint32_t rw[4] = {rq.x, rq.y, rq.z, rq.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 g2 = unpack_bf16x2(gw[j]);
+      const float2 r2 = unpack_bf16x2(rw[j]);
+      float y0 = v[2 * j], y1 = v[2 * j + 1];
+      bf16r2(y0, y1);
+      y0 *= g2.x;
+      y1 *= g2.y;
+      bf16r2(y0, y1);
+      v[2 * j] = r2.x + y0;
+      v[2 * j + 1] = r2.y + y1;
+    }
+  } else if (epi == B2F_EPI_DGELU || epi == B2F_EPI_DSILU) {
+    // backward of the activation fused into the dgrad GEMM: out = bf16(acc) * act'(u), u = the saved
+    // pre-activation (read through the resid pointer)
+    const uint32_t uw[4] = {rq.x, rq.y, rq.z, rq.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 u2 = unpack_bf16x2(uw[j]);
+      const float d0 = epi == B2F_EPI_DGELU ? dgelu_tanh_f(u2.x) : dsilu_f(u2.x);
+      const float d1 = epi == B2F_EPI_DGELU ? dgelu_tanh_f(u2.y) : dsilu_f(u2.y);
+      v[2 * j] = bf16r(v[2 * j]) * d0;
+      v[2 * j + 1] = bf16r(v[2 * j + 1]) * d1;
+    }
+  } else if (epi == B2F_EPI_RESID) {
+    const uint32_t rw[4] = {rq.x, rq.y, rq.z, rq.w};
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float2 r2 = unpack_bf16x2(rw[j]);
+      float y0 = v[2 * j], y1 = v[2 * j + 1];
+      bf16r2(y0, y1);
+      v[2 * j] = r2.x + y0;
+      v[2 * j + 1] = r2.y + y1;
+    }
+  }
+  uint4 o;
+  o.x = pack_bf16x2(v[0], v[1]);
+  o.y = pack_bf16x2(v[2], v[3]);
+  o.z = pack_bf16x2(v[4], v[5]);
+  o.w = pack_bf16x2(v[6], v[7]);
+  *reinterpret_cast<uint4*>(out) = o;
+}
+
+__device__ __forceinline__ void unpack_bf16x8(const uint4 q, float (&v)[8]) {
+  const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    const float2 f = unpack_bf16x2(w[j]);
+    v[2 * j] = f.x;
+    v[2 * j + 1] = f.y;
   }
 }
 
-// One 128-column head of a fused QKV projection for one token, straight from the staged accumulators:
-//   x = bf16(acc + bias);  y = bf16(x * rsqrt(mean(x^2) + eps));  z = bf16(y * w);
+// One 128-column head of a fused QKV projection for one token, from its row of the staged tile x = bf16(acc + bias):
+//   y = bf16(x * rsqrt(mean(x^2) + eps));  z = bf16(y * w);
 //   out = bf16(z * cos + rot(z) * sin)        (diffusers RMSNorm + apply_rotary_emb, SURVEY.md A.2)
-// — the same rounding chain as rmsnorm_rope_kernel, but without the extra HBM round trip.  Every rounding is the packed
-// cvt.rn.bf16x2.
-__device__ __forceinline__ void epilogue_head_norm_rope(const GemmParams& p, const float* crow, int n_head0,
+// — the same rounding chain as rmsnorm_rope_kernel, but without the extra HBM round trip.  The sum of squares runs over
+// the columns in order, one thread per row.  Every rounding is the packed cvt.rn.bf16x2.
+__device__ __forceinline__ void epilogue_head_norm_rope(const GemmParams& p, const uint8_t* srow, int n_head0,
                                                         long long row, __nv_bfloat16* out_row, bool is_k) {
   const __nv_bfloat16* w = is_k ? p.nw_k : p.nw_q;
-  // pass 1: sum of squares of x = bf16(acc + bias) over the head
   float ss = 0.f;
-#pragma unroll 1
-  for (int cc = 0; cc < 4; ++cc) {
-    uint32_t acc[32];
-    load_chunk(crow, cc * 32, acc);
+#pragma unroll 4
+  for (int g = 0; g < BLOCK_N / 8; ++g) {
+    float x[8];
+    unpack_bf16x8(*reinterpret_cast<const uint4*>(srow + g * 16), x);
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const int c = cc * 32 + g * 8;
-      const uint4 bq = p.bias ? __ldg(reinterpret_cast<const uint4*>(p.bias + n_head0 + c)) : make_uint4(0, 0, 0, 0);
-      const uint32_t bw[4] = {bq.x, bq.y, bq.z, bq.w};
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const float2 b2 = unpack_bf16x2(bw[jj]);
-        float x0 = __uint_as_float(acc[g * 8 + 2 * jj]) + b2.x, x1 = __uint_as_float(acc[g * 8 + 2 * jj + 1]) + b2.y;
-        bf16r2(x0, x1);
-        ss = fmaf(x0, x0, ss);
-        ss = fmaf(x1, x1, ss);
-      }
-    }
+    for (int j = 0; j < 8; ++j) ss = fmaf(x[j], x[j], ss);
   }
   const float r = rsqrtf(ss * (1.0f / 128.0f) + p.norm_eps);
   const float* cs = p.rope_cos + ((long long)p.rope_row0 + row) * 128;
   const float* sn = p.rope_sin + ((long long)p.rope_row0 + row) * 128;
-  // pass 2: normalise, weight, rotate, store
-#pragma unroll 1
-  for (int cc = 0; cc < 4; ++cc) {
-    uint32_t acc[32];
-    load_chunk(crow, cc * 32, acc);
+#pragma unroll 4
+  for (int g = 0; g < BLOCK_N / 8; ++g) {
+    const int c = g * 8;
+    float x[8];
+    unpack_bf16x8(*reinterpret_cast<const uint4*>(srow + g * 16), x);
+    const uint4 wq = __ldg(reinterpret_cast<const uint4*>(w + c));
+    const uint32_t ww[4] = {wq.x, wq.y, wq.z, wq.w};
+    const float4 c0 = __ldg(reinterpret_cast<const float4*>(cs + c)), c1 = __ldg(reinterpret_cast<const float4*>(cs + c + 4));
+    const float4 s0 = __ldg(reinterpret_cast<const float4*>(sn + c)), s1 = __ldg(reinterpret_cast<const float4*>(sn + c + 4));
+    const float cc8[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
+    const float sc8[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
+    uint32_t o[4];
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      const int c = cc * 32 + g * 8;
-      const uint4 bq = p.bias ? __ldg(reinterpret_cast<const uint4*>(p.bias + n_head0 + c)) : make_uint4(0, 0, 0, 0);
-      const uint4 wq = __ldg(reinterpret_cast<const uint4*>(w + c));
-      const uint32_t bw[4] = {bq.x, bq.y, bq.z, bq.w};
-      const uint32_t ww[4] = {wq.x, wq.y, wq.z, wq.w};
-      const float4 c0 = __ldg(reinterpret_cast<const float4*>(cs + c)), c1 = __ldg(reinterpret_cast<const float4*>(cs + c + 4));
-      const float4 s0 = __ldg(reinterpret_cast<const float4*>(sn + c)), s1 = __ldg(reinterpret_cast<const float4*>(sn + c + 4));
-      const float cc8[8] = {c0.x, c0.y, c0.z, c0.w, c1.x, c1.y, c1.z, c1.w};
-      const float sc8[8] = {s0.x, s0.y, s0.z, s0.w, s1.x, s1.y, s1.z, s1.w};
-      uint32_t o[4];
-#pragma unroll
-      for (int jj = 0; jj < 4; ++jj) {
-        const float2 b2 = unpack_bf16x2(bw[jj]);
-        const float2 w2 = unpack_bf16x2(ww[jj]);
-        float z0 = __uint_as_float(acc[g * 8 + 2 * jj]) + b2.x, z1 = __uint_as_float(acc[g * 8 + 2 * jj + 1]) + b2.y;
-        bf16r2(z0, z1);          // x
-        z0 *= r;
-        z1 *= r;
-        bf16r2(z0, z1);          // y = bf16(x * r)
-        z0 *= w2.x;
-        z1 *= w2.y;
-        bf16r2(z0, z1);          // z = bf16(y * w)
-        o[jj] = pack_bf16x2(z0 * cc8[2 * jj] - z1 * sc8[2 * jj], z1 * cc8[2 * jj + 1] + z0 * sc8[2 * jj + 1]);
-      }
-      *reinterpret_cast<uint4*>(out_row + n_head0 + c) = make_uint4(o[0], o[1], o[2], o[3]);
+    for (int jj = 0; jj < 4; ++jj) {
+      const float2 w2 = unpack_bf16x2(ww[jj]);
+      float z0 = x[2 * jj], z1 = x[2 * jj + 1];
+      z0 *= r;
+      z1 *= r;
+      bf16r2(z0, z1);          // y = bf16(x * r)
+      z0 *= w2.x;
+      z1 *= w2.y;
+      bf16r2(z0, z1);          // z = bf16(y * w)
+      o[jj] = pack_bf16x2(z0 * cc8[2 * jj] - z1 * sc8[2 * jj], z1 * cc8[2 * jj + 1] + z0 * sc8[2 * jj + 1]);
     }
+    *reinterpret_cast<uint4*>(out_row + n_head0 + c) = make_uint4(o[0], o[1], o[2], o[3]);
   }
 }
 
-// row pointer of the output; fp32 outputs (wgrad) have their pitch in floats
-__device__ __forceinline__ __nv_bfloat16* out_row_ptr(const GemmParams& p, int bidx, long long row) {
-  if (p.epi == B2F_EPI_F32 || p.epi == B2F_EPI_F32_ACC)
-    return reinterpret_cast<__nv_bfloat16*>(reinterpret_cast<float*>(p.out) + bidx * p.out_bs + row * p.ldc);
-  return p.out + bidx * p.out_bs + row * p.ldc;
+// ---------------------------------------------------------------------------------------------------- the kernel
+// Shared memory: the STAGES-deep operand ring, then one bf16 staging tile per consumer, then the ring's barriers.
+constexpr int SROW = BLOCK_N * 2 + 16;     // byte pitch of a staged bf16 row: 16-byte accesses of 8 rows hit 32 banks
+constexpr int STAGING_BYTES = BLOCK_M * SROW;
+constexpr int PP_SMEM_BYTES = STAGES * STAGE_BYTES + 2 * STAGING_BYTES + 2 * STAGES * 8 + 1024;
+// Named barriers (0 is __syncthreads):
+constexpr int BAR_TURN = 2;   // + consumer: that consumer's turn on the tensor cores (256 threads: one arrives, one waits)
+constexpr int BAR_EPI = 4;    // + consumer: its own warpgroup around the staging tile (128 threads)
+constexpr int PRODUCER_REGS = 40, CONSUMER_REGS = 232;   // 128 x 40 + 256 x 232 <= 65536
+static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= 65536, "register split exceeds the register file");
+
+__device__ __forceinline__ void tile_origin(const GemmParams& p, int t, int& n_blk, int& bb, int& mb) {
+  int m_blk;
+  tile_coords(p, t, m_blk, n_blk);
+  bb = m_blk / p.m_blocks_per_batch;
+  mb = m_blk - bb * p.m_blocks_per_batch;
 }
 
-// Epilogue of one output row for the calling thread: its `half` (0 / 1) of the tile's 128 columns, read from the
-// staged accumulators.  A fused QKV head is the whole tile: the half-0 thread of the row runs it.
-__device__ __forceinline__ void epilogue_row(const GemmParams& p, const float* crow, int half, int n_blk, bool row_ok,
-                                             long long row, __nv_bfloat16* out_row, const __nv_bfloat16* res_row,
-                                             const __nv_bfloat16* gate_row, __nv_bfloat16* out_row2) {
-  if (!row_ok) return;
-  if (p.epi == B2F_EPI_QKV_NORM_ROPE) {
-    if (half == 1) return;
-    const int n_head0 = n_blk * BLOCK_N;
-    const int which = n_head0 / p.d_model;  // 0 = Q, 1 = K, 2 = V, >= 3: second output block
-    if (which < 2 && n_head0 < p.N) {
-      epilogue_head_norm_rope(p, crow, n_head0, row, out_row, which == 1);
-      return;
-    }
-    const bool second = p.split_n > 0 && n_head0 >= p.split_n;
-    __nv_bfloat16* orow = second ? out_row2 : out_row;
-    const int epi = second ? p.epi2 : B2F_EPI_BIAS;
-#pragma unroll 1
-    for (int cc = 0; cc < 4; ++cc) {
-      if (n_head0 + cc * 32 >= p.N) break;
-      uint32_t acc[32];
-      load_chunk(crow, cc * 32, acc);
-      epilogue_chunk(p, epi, acc, n_head0 + cc * 32, orow, res_row, gate_row);
-    }
-    return;
-  }
-#pragma unroll 1
-  for (int c0 = 0; c0 < BLOCK_N / 2; c0 += 32) {
-    const int n0 = n_blk * BLOCK_N + half * (BLOCK_N / 2) + c0;
-    if (n0 >= p.N) break;
-    uint32_t acc[32];
-    load_chunk(crow, half * (BLOCK_N / 2) + c0, acc);
-    epilogue_chunk(p, p.epi, acc, n0, out_row, res_row, gate_row);
-  }
-}
-
+// Persistent, warp-specialised GEMM with ping-pong consumers.  CTA b takes tiles b, b + grid, b + 2 grid, ... in panel
+// order; its consumer warpgroups take turns on them (consumer 0: the CTA's tiles 0, 2, 4, ..., consumer 1: 1, 3, ...),
+// each owning a whole 128 x 128 tile (two m64n128k16 per k16 step).  While one runs its tile's MMAs the other runs the
+// epilogue of its previous tile, and the producer streams k-blocks through the ring across tile boundaries.
 template <int MODE>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                  const GemmParams p) {
+  constexpr int TA = MODE == 2, TB = MODE >= 1;
   extern __shared__ uint8_t smem_raw[];
-  const Smem s = carve(smem_raw);
+  uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + STAGES * STAGE_BYTES + 2 * STAGING_BYTES);
+  uint64_t* empty = full + STAGES;
   const int wg = threadIdx.x >> 7;
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    for (int i = 0; i < STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 4);   // one arrive per warp of the consumer that read the stage
+    }
+    fence_mbar_init();
   }
-  init_barriers(s);
+  __syncthreads();
 
-  int m_blk, n_blk;
-  tile_coords(p, blockIdx.x, m_blk, n_blk);
+  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
+  const int n_local = (num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // this CTA's tiles
   const int num_kb = MODE == 2 ? p.kbatch * p.kb_per_batch : (p.K + BLOCK_K - 1) / BLOCK_K;
-  const int bb = m_blk / p.m_blocks_per_batch;
-  const int mb = m_blk - bb * p.m_blocks_per_batch;
 
   if (wg == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int kb = 0; kb < num_kb; ++kb) {
-        mbar_wait(&s.empty[stage], phase ^ 1);
-        uint8_t* sa = s.ring + stage * STAGE_BYTES;
-        uint8_t* sb = sa + A_BYTES;
-        mbar_expect_tx(&s.full[stage], STAGE_BYTES);
-        if (MODE == 2) {
-          const int kbb = kb / p.kb_per_batch;
-          const int kr = (kb - kbb * p.kb_per_batch) * BLOCK_K;
+      for (int i = 0; i < n_local; ++i) {
+        int n_blk, bb, mb;
+        tile_origin(p, blockIdx.x + i * gridDim.x, n_blk, bb, mb);
+        const int m_blk = bb * p.m_blocks_per_batch + mb;
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          uint8_t* sa = ring + stage * STAGE_BYTES;
+          uint8_t* sb = sa + A_BYTES;
+          mbar_expect_tx(&full[stage], STAGE_BYTES);
+          if (MODE == 2) {
+            const int kbb = kb / p.kb_per_batch;
+            const int kr = (kb - kbb * p.kb_per_batch) * BLOCK_K;
 #pragma unroll
-          for (int i = 0; i < BLOCK_M / 64; ++i)
-            tma_load_3d(sa + i * MN_BOX_BYTES, &tmA, &s.full[stage], m_blk * BLOCK_M + 64 * i, kr, kbb);
+            for (int h = 0; h < BLOCK_M / 64; ++h)
+              tma_load_3d(sa + h * MN_BOX_BYTES, &tmA, &full[stage], m_blk * BLOCK_M + 64 * h, kr, kbb);
 #pragma unroll
-          for (int i = 0; i < BLOCK_N / 64; ++i)
-            tma_load_3d(sb + i * MN_BOX_BYTES, &tmB, &s.full[stage], n_blk * BLOCK_N + 64 * i, kr, kbb);
-        } else {
-          tma_load_3d(sa, &tmA, &s.full[stage], kb * BLOCK_K, mb * BLOCK_M, bb);
-          if (MODE == 1) {
-#pragma unroll
-            for (int i = 0; i < BLOCK_N / 64; ++i)
-              tma_load_2d(sb + i * MN_BOX_BYTES, &tmB, &s.full[stage], n_blk * BLOCK_N + 64 * i, kb * BLOCK_K);
+            for (int h = 0; h < BLOCK_N / 64; ++h)
+              tma_load_3d(sb + h * MN_BOX_BYTES, &tmB, &full[stage], n_blk * BLOCK_N + 64 * h, kr, kbb);
           } else {
-            tma_load_2d(sb, &tmB, &s.full[stage], kb * BLOCK_K, n_blk * BLOCK_N);
+            tma_load_3d(sa, &tmA, &full[stage], kb * BLOCK_K, mb * BLOCK_M, bb);
+            if (MODE == 1) {
+#pragma unroll
+              for (int h = 0; h < BLOCK_N / 64; ++h)
+                tma_load_2d(sb + h * MN_BOX_BYTES, &tmB, &full[stage], n_blk * BLOCK_N + 64 * h, kb * BLOCK_K);
+            } else {
+              tma_load_2d(sb, &tmB, &full[stage], kb * BLOCK_K, n_blk * BLOCK_N);
+            }
           }
-        }
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1;
+          if (++stage == STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
         }
       }
     }
     return;
   }
-  float acc[64];
-  mainloop<MODE == 2, MODE >= 1>(s, num_kb, wg - 1, acc);
-  stage_accumulators(s, wg - 1, acc);
+  setmaxnreg_inc<CONSUMER_REGS>();
 
-  const int e = threadIdx.x - 128;
-  const int row_in_tile = e & (BLOCK_M - 1), half = e >> 7;
-  const long long row = (long long)mb * BLOCK_M + row_in_tile;
-  const bool row_ok = row < p.M;
-  const __nv_bfloat16* gate_row = p.gate ? p.gate + (long long)bb * p.gate_ld : nullptr;
-  __nv_bfloat16* out_row = out_row_ptr(p, bb, row);
-  const __nv_bfloat16* res_row = p.resid ? p.resid + bb * p.resid_bs + row * p.ldr : nullptr;
-  __nv_bfloat16* out_row2 = p.out2 ? p.out2 + bb * p.out2_bs + row * p.ldc2 - p.split_n : nullptr;
-  epilogue_row(p, s.cbuf + row_in_tile * CROW, half, n_blk, row_ok, row, out_row, res_row, gate_row, out_row2);
+  const int c = wg - 1;                       // consumer 0 / 1
+  const int tid = threadIdx.x & 127, w = tid >> 5, lane = tid & 31;
+  uint8_t* stg = ring + STAGES * STAGE_BYTES + c * STAGING_BYTES;
+  // Descriptors of stage 0.  Rows 64..127 of the A tile start 8 KB in: 64 K-major rows of 128 B, or the second
+  // [64 k][64 m] box of an MN-major A.
+  const uint32_t ring_u = smem_u32(ring);
+  const uint64_t da0 = make_sdesc_sw128(ring_u, TA ? MN_BOX_BYTES : 16, 1024);
+  const uint64_t da1 = make_sdesc_sw128(ring_u + 8192, TA ? MN_BOX_BYTES : 16, 1024);
+  const uint64_t db0 = make_sdesc_sw128(ring_u + A_BYTES, TB ? MN_BOX_BYTES : 16, 1024);
+  constexpr int A_KSTEP = TA ? 2048 : 32;
+  constexpr int B_KSTEP = TB ? 2048 : 32;
+  if (c == 1) named_bar_arrive(BAR_TURN + 0, 256);   // consumer 0 takes the first turn
+
+  for (int i = c; i < n_local; i += 2) {
+    int n_blk, bb, mb;
+    tile_origin(p, blockIdx.x + i * gridDim.x, n_blk, bb, mb);
+
+    // ---- main loop: this consumer's turn on the tensor cores.  Its tile's k-blocks are ring slots
+    // i * num_kb .. (i + 1) * num_kb - 1 in the producer's order.
+    float acc0[64], acc1[64];   // rows 0..63 / 64..127 of the tile
+#pragma unroll
+    for (int j = 0; j < 64; ++j) {
+      acc0[j] = 0.f;
+      acc1[j] = 0.f;
+    }
+    named_bar_sync(BAR_TURN + c, 256);
+    const int slot0 = i * num_kb;
+    int stage = slot0 % STAGES, prev = -1;
+    uint32_t phase = (slot0 / STAGES) & 1;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint64_t soff = uint64_t((stage * STAGE_BYTES) >> 4);
+      reg_fence(acc0);
+      reg_fence(acc1);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BLOCK_K / 16; ++k) {
+        const uint64_t ka = soff + uint64_t((k * A_KSTEP) >> 4), kb16 = soff + uint64_t((k * B_KSTEP) >> 4);
+        wgmma_m64n128_ss<TA, TB>(acc0, da0 + ka, db0 + kb16, 1u);
+        wgmma_m64n128_ss<TA, TB>(acc1, da1 + ka, db0 + kb16, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();   // the previous stage's MMAs are complete: hand it back to the producer
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+      }
+      prev = stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    if (i + 1 < n_local) named_bar_arrive(BAR_TURN + (c ^ 1), 256);   // the other consumer's tile goes next
+    wgmma_wait<0>();
+    reg_fence(acc0);
+    reg_fence(acc1);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+
+    // ---- epilogue, overlapping the other consumer's main loop.  Accumulator element j of a thread is row
+    // 16 w + lane / 4 + 8 ((j / 2) & 1), column 8 (j / 4) + 2 (lane % 4) + (j & 1) of its 64-row half.
+    const int r_lo = 16 * w + (lane >> 2);
+    if (MODE == 2) {
+      // fp32 weight gradient straight from the registers: a quad writes 32 contiguous bytes per 8-column group.  With
+      // accumulate, the prior values of a thread's row are all read before its first store.
+      const bool acc_in = p.epi == B2F_EPI_F32_ACC;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float* a = h ? acc1 : acc0;
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const long long row = (long long)mb * BLOCK_M + 64 * h + r_lo + 8 * rr;
+          if (row >= p.M) continue;
+          float* orow = reinterpret_cast<float*>(p.out) + row * p.ldc + n_blk * BLOCK_N + 2 * (lane & 3);
+          const int n_left = p.N - n_blk * BLOCK_N - 2 * (lane & 3);   // columns 8 j of orow are valid while 8 j < n_left
+          float2 q[BLOCK_N / 8];
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            q[j] = make_float2(0.f, 0.f);
+            if (acc_in && 8 * j < n_left) q[j] = *reinterpret_cast<const float2*>(orow + 8 * j);
+          }
+#pragma unroll
+          for (int j = 0; j < BLOCK_N / 8; ++j) {
+            if (8 * j >= n_left) break;
+            float2 v = make_float2(a[4 * j + 2 * rr], a[4 * j + 2 * rr + 1]);
+            if (acc_in) {
+              v.x += q[j].x;
+              v.y += q[j].y;
+            }
+            *reinterpret_cast<float2*>(orow + 8 * j) = v;
+          }
+        }
+      }
+      continue;
+    }
+    // x = bf16(acc + bias) into this consumer's staging tile, once its previous tile's epilogue is done reading it
+    named_bar_sync(BAR_EPI + c, 128);
+#pragma unroll
+    for (int j = 0; j < BLOCK_N / 8; ++j) {
+      const int col = 8 * j + 2 * (lane & 3);
+      const int n = n_blk * BLOCK_N + col;
+      const bool has_bias = p.bias && n < p.N;
+      const float2 b2 = has_bias ? unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n))) : make_float2(0.f, 0.f);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const float* a = h ? acc1 : acc0;
+        float x0 = a[4 * j], x1 = a[4 * j + 1], x2 = a[4 * j + 2], x3 = a[4 * j + 3];
+        if (has_bias) {
+          x0 += b2.x;
+          x1 += b2.y;
+          x2 += b2.x;
+          x3 += b2.y;
+        }
+        uint8_t* s0 = stg + (64 * h + r_lo) * SROW + col * 2;
+        *reinterpret_cast<uint32_t*>(s0) = pack_bf16x2(x0, x1);
+        *reinterpret_cast<uint32_t*>(s0 + 8 * SROW) = pack_bf16x2(x2, x3);
+      }
+    }
+    named_bar_sync(BAR_EPI + c, 128);
+
+    const int n_tile0 = n_blk * BLOCK_N;
+    const __nv_bfloat16* gate_row = p.gate ? p.gate + (long long)bb * p.gate_ld : nullptr;
+    int epi = p.epi;
+    __nv_bfloat16* out_base = p.out + bb * p.out_bs;
+    long long ld = p.ldc;
+    if (epi == B2F_EPI_QKV_NORM_ROPE) {
+      const int which = n_tile0 / p.d_model;  // 0 = Q, 1 = K, 2 = V, >= 3: second output block
+      if (which < 2) {
+        // one normalised head per tile: one thread per row
+        const long long row = (long long)mb * BLOCK_M + tid;
+        if (row < p.M)
+          epilogue_head_norm_rope(p, stg + tid * SROW, n_tile0, row, out_base + row * ld, which == 1);
+        continue;
+      }
+      const bool second = p.split_n > 0 && n_tile0 >= p.split_n;
+      epi = second ? p.epi2 : B2F_EPI_BIAS;
+      if (second) {
+        out_base = p.out2 + bb * p.out2_bs - p.split_n;
+        ld = p.ldc2;
+      }
+    }
+    // 16 threads per row, one 8-column group each: a warp reads and writes two 256-byte row segments.  Rows go in
+    // batches of 4 per thread whose residual / pre-activation loads are all issued before the first store, so their
+    // latencies overlap; a batch, not all 16 rows, keeps the unrolled activation code small.
+    const int cg = tid & 15;
+    const int n = n_tile0 + 8 * cg;
+    if (n < p.N) {
+      constexpr int RB = 4;
+      const int r0 = tid >> 4;
+      const bool reads_resid = epi == B2F_EPI_GATE_RESID || epi == B2F_EPI_RESID || epi == B2F_EPI_DGELU ||
+                               epi == B2F_EPI_DSILU;
+      const uint4 gq = epi == B2F_EPI_GATE_RESID ? __ldg(reinterpret_cast<const uint4*>(gate_row + n))
+                                                 : make_uint4(0, 0, 0, 0);
+#pragma unroll 1
+      for (int rb = r0; rb < BLOCK_M; rb += 8 * RB) {     // tile rows rb + 8 r, r < RB
+        const long long row0 = (long long)mb * BLOCK_M + rb;
+        if (row0 >= p.M) break;
+        uint4 rq[RB];
+#pragma unroll
+        for (int r = 0; r < RB; ++r) {
+          const long long row = row0 + 8 * r;
+          rq[r] = make_uint4(0, 0, 0, 0);
+          if (reads_resid && row < p.M)
+            rq[r] = *reinterpret_cast<const uint4*>(p.resid + bb * p.resid_bs + row * p.ldr + n);
+        }
+#pragma unroll
+        for (int r = 0; r < RB; ++r) {
+          const long long row = row0 + 8 * r;
+          if (row >= p.M) break;
+          float v[8];
+          unpack_bf16x8(*reinterpret_cast<const uint4*>(stg + (rb + 8 * r) * SROW + cg * 16), v);
+          epilogue_group(epi, v, rq[r], gq, out_base + row * ld + n);
+        }
+      }
+    }
+  }
 }
 
 template <int MODE>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         PP_SMEM_BYTES);
     if (e != cudaSuccess) return cuda_err(e, "gemm smem attribute");
     attr_set = true;
   }
@@ -398,9 +520,10 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cu
   p.num_n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
   p.panel_n = 16;
   const int num_tiles = p.num_m_blocks * p.num_n_blocks;
+  const int grid = std::min(num_tiles, device_info().num_sms);   // persistent: at most one CTA per SM
   const double kk = MODE == 2 ? (double)p.kbatch * p.K : (double)p.K;
   prof_begin(KC_GEMM, stream);
-  gemm_bf16_kernel<MODE><<<num_tiles, THREADS, SMEM_BYTES, stream>>>(tmA, tmB, p);
+  gemm_bf16_kernel<MODE><<<grid, THREADS, PP_SMEM_BYTES, stream>>>(tmA, tmB, p);
   {
     char tag_[96];
     snprintf(tag_, sizeof tag_, "gemm m%d %dx%dx%d b%d e%d", MODE, p.M, p.N, (int)kk, p.batch, p.epi);

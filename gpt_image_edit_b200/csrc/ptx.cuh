@@ -167,6 +167,16 @@ __device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t nthreads) {
 __device__ __forceinline__ void named_bar_arrive(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }
+// Per-warpgroup register budget (every thread of the warpgroup executes it): a producer gives registers back, the
+// consumers take them.
+template <int R>
+__device__ __forceinline__ void setmaxnreg_dec() {
+  asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R));
+}
+template <int R>
+__device__ __forceinline__ void setmaxnreg_inc() {
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R));
+}
 
 // Pairwise fp32 helpers (each element rounds exactly as the scalar fma / add / mul).
 __device__ __forceinline__ float fmax3(float a, float b, float c) { return fmaxf(fmaxf(a, b), c); }

@@ -6,6 +6,9 @@ import sys
 WANT = [
     ("tests/test_gemm_gpu.py", ["test_gemm_bias[128-128-64]", "test_gemm_bias[256-512-256]", "test_gemm_bias[1000-136-72]",
                                 "test_gemm_gate_resid_batched_views", "test_gemm_gelu_silu"]),
+    # the persistent GEMM reusing its ring and staging tiles across tiles of one CTA (SMs + 1 tiles)
+    ("tests/test_gemm_persistent_gpu.py", ["test_gemm_toy_tile_counts[1]", "test_gemm_toy_tile_counts[3]",
+                                           "test_gemm_toy_tile_counts[sms+1]"]),
     ("tests/test_train_kernels_gpu.py", ["test_gemm_dgrad[1-128-128-64]", "test_gemm_dgrad[1-200-136-72]", "test_gemm_dgrad[2-300-256-512]",
                                          "test_gemm_dgrad[2-1024-1024-4096]", "test_gemm_dgrad_pitched_views_and_epilogues",
                                          "test_gemm_wgrad[1-64-128-128]", "test_gemm_wgrad[1-100-136-200]", "test_gemm_wgrad[3-150-256-384]",
