@@ -129,6 +129,20 @@ _SIGNATURES = {
     "b2f_flux_train_backward": (_i32, [_vp, _vp, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _vp, C.c_size_t,
                                        _i32, _i32, _vp]),
     "b2f_flux_train_debug_dh": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp, _vp]),
+    # LoRA
+    "b2f_gemm_bf16_lora": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _i64,
+                                  _vp, _i64, _vp, _i64, _i64, _vp, _i64, _i32, _vp]),
+    "b2f_gemm_qkv_norm_rope_lora": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp,
+                                           _vp, _i32, C.c_float, _i32, _vp, _i64, _i64, _i32, _vp, _i64, _i64, _vp, _i64, _i32,
+                                           _vp]),
+    "b2f_gemm_colscale": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, C.c_float, _vp]),
+    "b2f_lora_fuse": (_i32, [_vp, _i64, _i32, _i32, _vp, _i64, _vp, _i64, _vp, C.c_float, _i32, _vp]),
+    "b2f_flux_bind_lora": (_i32, [_vp, C.c_char_p, _vp, _vp, _vp, _i32]),
+    "b2f_flux_clear_lora": (_i32, [_vp]),
+    "b2f_flux_set_lora_scale": (_i32, [_vp, C.c_float]),
+    "b2f_flux_lora_rank": (_i32, [_vp]),
+    "b2f_flux_modulation_workspace_bytes": (C.c_size_t, [_vp, _i32]),
+    "b2f_flux_modulation_ws": (_i32, [_vp, _vp, _i32, _vp, _vp, C.c_size_t, _vp]),
 }
 
 

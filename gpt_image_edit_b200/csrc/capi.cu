@@ -109,6 +109,22 @@ int adamw_step(float* p32, float* m, float* v, const float* g, void* p16, int64_
                float eps, float wd, int step, const float* gscale, cudaStream_t st);
 int cast_bf16_f32(const void* src, void* dst, int64_t n, int to_f32, cudaStream_t st);
 int blend_bf16(const void* a, const void* b, float wa, float wb, void* out, int64_t n, cudaStream_t st);
+// LoRA (gemm.cu, lora.cu)
+int gemm_bf16_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias, void* out,
+                   int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epilogue, const void* resid,
+                   int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld, const void* T, int64_t ldt,
+                   int64_t t_bs, const void* Bc, int64_t ldbc, int r_pad, cudaStream_t stream);
+int gemm_qkv_norm_rope_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias,
+                            void* out, int64_t ldc, int64_t out_bs, int batch, int M, int d_model, int K,
+                            const void* nw_q, const void* nw_k, const float* cos, const float* sin, int rope_row0,
+                            float eps, int n_extra, void* out_extra, int64_t ld_extra, int64_t bs_extra,
+                            int epi_extra, const void* T, int64_t ldt, int64_t t_bs, const void* Bc, int64_t ldbc,
+                            int r_pad, cudaStream_t stream);
+int gemm_colscale(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, void* out, int64_t ldc,
+                  int64_t out_bs, int batch, int M, int N, int K, const float* colscale, float cs_mul,
+                  cudaStream_t stream);
+int lora_fuse(void* W, int64_t ldw, int rows, int cols, const void* Bc, int64_t ldb, const void* A, int64_t lda,
+              const float* colscale, float cs_mul, int r, cudaStream_t stream);
 }  // namespace b2f
 
 extern "C" {
@@ -126,7 +142,7 @@ const char* b2f_strerror(int code) {
   }
 }
 
-int b2f_version(void) { return 1; }
+int b2f_version(void) { return 2; }
 
 int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin) {
   int n = 0;
@@ -378,6 +394,38 @@ int b2f_cast_bf16_f32(const void* src, void* dst, int64_t n, int to_f32, b2f_str
 }
 int b2f_blend_bf16(const void* a, const void* b, float wa, float wb, void* out, int64_t n, b2f_stream_t stream) {
   return b2f::blend_bf16(a, b, wa, wb, out, n, ST);
+}
+
+// ------------------------------------------------------------------ LoRA
+int b2f_gemm_bf16_lora(const void* A, int64_t lda, int64_t a_batch_stride, const void* W, int64_t ldw,
+                       const void* bias, void* out, int64_t ldc, int64_t out_batch_stride, int batch, int M, int N,
+                       int K, int epilogue, const void* resid, int64_t ldr, int64_t resid_batch_stride,
+                       const void* gate, int64_t gate_ld, const void* T, int64_t ldt, int64_t t_batch_stride,
+                       const void* Bcat, int64_t ldbc, int r_pad, b2f_stream_t stream) {
+  return b2f::gemm_bf16_lora(A, lda, a_batch_stride, W, ldw, bias, out, ldc, out_batch_stride, batch, M, N, K,
+                             epilogue, resid, ldr, resid_batch_stride, gate, gate_ld, T, ldt, t_batch_stride, Bcat,
+                             ldbc, r_pad, ST);
+}
+int b2f_gemm_qkv_norm_rope_lora(const void* A, int64_t lda, int64_t a_batch_stride, const void* W, int64_t ldw,
+                                const void* bias, void* out, int64_t ldc, int64_t out_batch_stride, int batch, int M,
+                                int d_model, int K, const void* nw_q, const void* nw_k, const float* cos,
+                                const float* sin, int rope_row0, float eps, int n_extra, void* out_extra,
+                                int64_t ld_extra, int64_t extra_batch_stride, int epi_extra, const void* T,
+                                int64_t ldt, int64_t t_batch_stride, const void* Bcat, int64_t ldbc, int r_pad,
+                                b2f_stream_t stream) {
+  return b2f::gemm_qkv_norm_rope_lora(A, lda, a_batch_stride, W, ldw, bias, out, ldc, out_batch_stride, batch, M,
+                                      d_model, K, nw_q, nw_k, cos, sin, rope_row0, eps, n_extra, out_extra, ld_extra,
+                                      extra_batch_stride, epi_extra, T, ldt, t_batch_stride, Bcat, ldbc, r_pad, ST);
+}
+int b2f_gemm_colscale(const void* A, int64_t lda, int64_t a_batch_stride, const void* W, int64_t ldw, void* out,
+                      int64_t ldc, int64_t out_batch_stride, int batch, int M, int N, int K, const float* colscale,
+                      float cs_mul, b2f_stream_t stream) {
+  return b2f::gemm_colscale(A, lda, a_batch_stride, W, ldw, out, ldc, out_batch_stride, batch, M, N, K, colscale,
+                            cs_mul, ST);
+}
+int b2f_lora_fuse(void* W, int64_t ldw, int rows, int cols, const void* Bcat, int64_t ldb, const void* Acat,
+                  int64_t lda, const float* colscale, float cs_mul, int r, b2f_stream_t stream) {
+  return b2f::lora_fuse(W, ldw, rows, cols, Bcat, ldb, Acat, lda, colscale, cs_mul, r, ST);
 }
 #undef ST
 

@@ -10,9 +10,22 @@ namespace b2f {
 
 typedef uint16_t bf16_t;
 
+// Unfused LoRA of one linear (b2f_flux_bind_lora): Acat [r_pad, in], Bcat [out, r_pad], colscale fp32 [r_pad].
+struct LoraBind {
+  const bf16_t* A = nullptr;
+  const bf16_t* Bc = nullptr;
+  const float* cs = nullptr;
+  int r_pad = 0;
+};
 struct Lin {
   const bf16_t* w = nullptr;
   const bf16_t* b = nullptr;
+  LoraBind lora;
+};
+// LoRA of one AdaLN linear: rows [row0, row0 + rows) of the fused adaln weight
+struct AdalnLora {
+  int64_t row0 = 0, rows = 0;
+  LoraBind l;
 };
 struct DoubleW {
   Lin qkv, add_qkv, to_out, to_add_out, ff1, ff2, ffc1, ffc2;
@@ -36,6 +49,12 @@ struct FluxCtx {
   int rope_S = 0;
   bool finalized = false;
   int64_t mod_width = 0;
+  // unfused LoRA adapters: the AdaLN ones by linear name; every other one sits in its Lin.  lora_scale multiplies every
+  // colscale (the per-call `scale` of joint_attention_kwargs).
+  std::map<std::string, AdalnLora> adaln_lora;
+  float lora_scale = 1.f;
+  int lora_count = 0;
+  int lora_rmax() const;
   // fp32 gradient buffers of the trainable tensors, bound by name (flux_train.cu); an unbound name is frozen
   std::map<std::string, std::pair<float*, int64_t>> grads;
 };

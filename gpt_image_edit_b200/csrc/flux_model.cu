@@ -12,6 +12,7 @@
 //     GEMM reads cat with K = 5d.
 // Reference call sites of this path: univa/utils/flux_pipeline.py:1067-1077,
 // univa/models/modeling_univa_denoise_tower.py:103-110.
+#include <algorithm>
 #include <cstring>
 #include <map>
 #include <string>
@@ -42,6 +43,19 @@ int rmsnorm_rope(void* q, void* k, int64_t ld, int64_t batch_stride, const void*
                  const void* wk_a, const void* wq_b, const void* wk_b, const float* cos,
                  const float* sin, int batch, int S, int H, int head_dim, int n_a, float eps,
                  cudaStream_t stream);
+int gemm_bf16_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias, void* out,
+                   int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epilogue, const void* resid,
+                   int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld, const void* T, int64_t ldt,
+                   int64_t t_bs, const void* Bc, int64_t ldbc, int r_pad, cudaStream_t stream);
+int gemm_qkv_norm_rope_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias,
+                            void* out, int64_t ldc, int64_t out_bs, int batch, int M, int d_model, int K,
+                            const void* nw_q, const void* nw_k, const float* cos, const float* sin, int rope_row0,
+                            float eps, int n_extra, void* out_extra, int64_t ld_extra, int64_t bs_extra,
+                            int epi_extra, const void* T, int64_t ldt, int64_t t_bs, const void* Bc, int64_t ldbc,
+                            int r_pad, cudaStream_t stream);
+int gemm_colscale(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, void* out, int64_t ldc,
+                  int64_t out_bs, int batch, int M, int N, int K, const float* colscale, float cs_mul,
+                  cudaStream_t stream);
 int temb_sinusoid(const float* t, void* out, int rows, cudaStream_t stream);
 int temb_combine(const void* t, const void* g, const void* txt, void* temb, void* silu_temb,
                  int64_t n, cudaStream_t stream);
@@ -69,6 +83,99 @@ static int expect_lin(FluxCtx* c, const std::string& name, int64_t out_f, int64_
   int rc = expect(c, name + ".weight", out_f * in_f, &l->w);
   if (rc) return rc;
   return expect(c, name + ".bias", out_f, &l->b);
+}
+
+// Every linear a LoRA can target, by its bound name (the fused ones: attn.qkv, attn.add_qkv, qkv_mlp) or, for the
+// AdaLN linears, by its diffusers name (rows of the fused adaln weight).  f(name, lin or nullptr, row0, out, in).
+template <class F>
+static void for_each_linear(FluxCtx* c, F&& f) {
+  const b2f_flux_cfg& g = c->cfg;
+  const int64_t d = c->d;
+  f(std::string("x_embedder"), &c->x_embedder, 0, d, (int64_t)g.in_channels);
+  f(std::string("context_embedder"), &c->context_embedder, 0, d, (int64_t)g.joint_dim);
+  f(std::string("time_text_embed.timestep_embedder.linear_1"), &c->t1, 0, d, 256);
+  f(std::string("time_text_embed.timestep_embedder.linear_2"), &c->t2, 0, d, d);
+  if (g.guidance_embeds) {
+    f(std::string("time_text_embed.guidance_embedder.linear_1"), &c->g1, 0, d, 256);
+    f(std::string("time_text_embed.guidance_embedder.linear_2"), &c->g2, 0, d, d);
+  }
+  f(std::string("time_text_embed.text_embedder.linear_1"), &c->p1, 0, d, (int64_t)g.pooled_dim);
+  f(std::string("time_text_embed.text_embedder.linear_2"), &c->p2, 0, d, d);
+  f(std::string("proj_out"), &c->proj_out, 0, (int64_t)g.out_channels, d);
+  for (int i = 0; i < g.num_double; ++i) {
+    const std::string p = "transformer_blocks." + std::to_string(i) + ".";
+    DoubleW& w = c->dbl[i];
+    f(p + "attn.qkv", &w.qkv, 0, 3 * d, d);
+    f(p + "attn.add_qkv", &w.add_qkv, 0, 3 * d, d);
+    f(p + "attn.to_out.0", &w.to_out, 0, d, d);
+    f(p + "attn.to_add_out", &w.to_add_out, 0, d, d);
+    f(p + "ff.net.0.proj", &w.ff1, 0, 4 * d, d);
+    f(p + "ff.net.2", &w.ff2, 0, d, 4 * d);
+    f(p + "ff_context.net.0.proj", &w.ffc1, 0, 4 * d, d);
+    f(p + "ff_context.net.2", &w.ffc2, 0, d, 4 * d);
+    f(p + "norm1.linear", nullptr, (int64_t)i * 12 * d, 6 * d, d);
+    f(p + "norm1_context.linear", nullptr, (int64_t)i * 12 * d + 6 * d, 6 * d, d);
+  }
+  for (int i = 0; i < g.num_single; ++i) {
+    const std::string p = "single_transformer_blocks." + std::to_string(i) + ".";
+    SingleW& w = c->sgl[i];
+    f(p + "qkv_mlp", &w.qkv_mlp, 0, 7 * d, d);
+    f(p + "proj_out", &w.proj_out, 0, d, 5 * d);
+    f(p + "norm.linear", nullptr, (int64_t)g.num_double * 12 * d + (int64_t)i * 3 * d, 3 * d, d);
+  }
+  f(std::string("norm_out.linear"), nullptr, (int64_t)g.num_double * 12 * d + (int64_t)g.num_single * 3 * d, 2 * d, d);
+}
+
+static int adaln_rmax(const FluxCtx* c) {
+  int r = 0;
+  for (const auto& kv : c->adaln_lora) r = std::max(r, kv.second.l.r_pad);
+  return r;
+}
+
+// A linear layer of the forward with its unfused LoRA, if one is bound:
+//   T = bf16(colscale * cs_mul * (A Acat^T))  into tb [batch, M, r_pad]    (gemm_colscale)
+//   out = epi(A W^T + T Bcat^T + bias)                                      (gemm_bf16_lora: r_pad / 64 more k-blocks)
+// Without one it is exactly the plain gemm_bf16 launch.
+static int lin_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_t lda, int64_t a_bs, int64_t ldw,
+                   void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epi, const void* resid,
+                   int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld, cudaStream_t st) {
+  if (!l.lora.A)
+    return gemm_bf16(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, N, K, epi, resid, ldr, resid_bs, gate,
+                     gate_ld, st);
+  const int r = l.lora.r_pad;
+  const int64_t t_bs = (int64_t)M * r;
+  int rc = gemm_colscale(A, lda, a_bs, l.lora.A, K, tb, r, t_bs, batch, M, r, K, l.lora.cs, cs_mul, st);
+  if (rc) return rc;
+  return gemm_bf16_lora(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, N, K, epi, resid, ldr, resid_bs,
+                        gate, gate_ld, tb, r, t_bs, l.lora.Bc, r, r, st);
+}
+static int qkv_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_t lda, int64_t a_bs, int64_t ldw,
+                   void* out, int64_t ldc, int64_t out_bs, int batch, int M, int d_model, int K, const void* nw_q,
+                   const void* nw_k, const float* cos, const float* sin, int rope_row0, float eps, int n_extra,
+                   void* out_extra, int64_t ld_extra, int64_t bs_extra, int epi_extra, cudaStream_t st) {
+  if (!l.lora.A)
+    return gemm_qkv_norm_rope(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, d_model, K, nw_q, nw_k, cos,
+                              sin, rope_row0, eps, n_extra, out_extra, ld_extra, bs_extra, epi_extra, st);
+  const int r = l.lora.r_pad;
+  const int64_t t_bs = (int64_t)M * r;
+  int rc = gemm_colscale(A, lda, a_bs, l.lora.A, K, tb, r, t_bs, batch, M, r, K, l.lora.cs, cs_mul, st);
+  if (rc) return rc;
+  return gemm_qkv_norm_rope_lora(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, d_model, K, nw_q, nw_k, cos,
+                                 sin, rope_row0, eps, n_extra, out_extra, ld_extra, bs_extra, epi_extra, tb, r, t_bs,
+                                 l.lora.Bc, r, r, st);
+}
+
+int FluxCtx::lora_rmax() const {
+  int r = adaln_rmax(this);
+  auto upd = [&](const Lin& l) { r = std::max(r, l.lora.r_pad); };
+  for (const Lin* l : {&x_embedder, &context_embedder, &proj_out, &t1, &t2, &g1, &g2, &p1, &p2}) upd(*l);
+  for (const DoubleW& w : dbl)
+    for (const Lin* l : {&w.qkv, &w.add_qkv, &w.to_out, &w.to_add_out, &w.ff1, &w.ff2, &w.ffc1, &w.ffc2}) upd(*l);
+  for (const SingleW& w : sgl) {
+    upd(w.qkv_mlp);
+    upd(w.proj_out);
+  }
+  return r;
 }
 
 }  // namespace b2f
@@ -159,6 +266,11 @@ int b2f_flux_finalize(b2f_flux* h) {
   }
 #undef EL
 #undef EW
+  // (re)binding weights drops every LoRA binding
+  for_each_linear(c, [](const std::string&, Lin* l, int64_t, int64_t, int64_t) {
+    if (l) l->lora = LoraBind();
+  });
+  c->adaln_lora.clear();
   c->finalized = true;
   return B2F_OK;
 }
@@ -177,15 +289,15 @@ size_t b2f_flux_workspace_bytes(const b2f_flux* h, int B, int S_img, int S_txt) 
   const FluxCtx* c = reinterpret_cast<const FluxCtx*>(h);
   if (!c || B <= 0 || S_img <= 0 || S_txt < 0) return 0;
   const size_t S = (size_t)S_img + S_txt;
-  // h[d] + xn[d] + qkv[3d] + cat[5d] per token, bf16
-  return (size_t)B * S * (size_t)c->d * 10 * 2 + 1024;
+  // h[d] + xn[d] + qkv[3d] + cat[5d] per token, bf16; with unfused LoRA adapters bound, T[r_pad] per token
+  return (size_t)B * S * ((size_t)c->d * 10 + (size_t)c->lora_rmax()) * 2 + 1024;
 }
 
 size_t b2f_flux_temb_workspace_bytes(const b2f_flux* h, int rows) {
   const FluxCtx* c = reinterpret_cast<const FluxCtx*>(h);
   if (!c || rows <= 0) return 0;
-  // 2 sinusoid tables [rows,256] + 6 activations [rows,d]
-  return ((size_t)rows * 256 * 2 + (size_t)rows * c->d * 6) * 2 + 1024;
+  // 2 sinusoid tables [rows,256] + 6 activations [rows,d] (+ LoRA T [rows, r_pad] with adapters bound)
+  return ((size_t)rows * 256 * 2 + (size_t)rows * c->d * 6 + (size_t)rows * c->lora_rmax()) * 2 + 1024;
 }
 
 int b2f_flux_temb(b2f_flux* h, const float* timestep, const float* guidance, const void* pooled,
@@ -205,29 +317,31 @@ int b2f_flux_temb(b2f_flux* h, const float* timestep, const float* guidance, con
   bf16_t* et = a1 + (size_t)rows * d;
   bf16_t* eg = et + (size_t)rows * d;
   bf16_t* ep = eg + (size_t)rows * d;
+  bf16_t* tb = ep + (size_t)rows * d;   // LoRA T
+  const float ls = c->lora_scale;
   int rc;
   if ((rc = temb_sinusoid(timestep, sin_t, rows, st))) return rc;
-  if ((rc = gemm_bf16(sin_t, 256, 0, c->t1.w, 256, c->t1.b, a1, d, 0, 1, rows, d, 256, B2F_EPI_SILU,
+  if ((rc = lin_fwd(c->t1, tb, ls, sin_t, 256, 0, 256, a1, d, 0, 1, rows, d, 256, B2F_EPI_SILU,
                       nullptr, 0, 0, nullptr, 0, st)))
     return rc;
-  if ((rc = gemm_bf16(a1, d, 0, c->t2.w, d, c->t2.b, et, d, 0, 1, rows, d, d, B2F_EPI_BIAS, nullptr,
+  if ((rc = lin_fwd(c->t2, tb, ls, a1, d, 0, d, et, d, 0, 1, rows, d, d, B2F_EPI_BIAS, nullptr,
                       0, 0, nullptr, 0, st)))
     return rc;
   const bf16_t* eg_ptr = nullptr;
   if (c->cfg.guidance_embeds) {
     if ((rc = temb_sinusoid(guidance, sin_g, rows, st))) return rc;
-    if ((rc = gemm_bf16(sin_g, 256, 0, c->g1.w, 256, c->g1.b, a1, d, 0, 1, rows, d, 256,
+    if ((rc = lin_fwd(c->g1, tb, ls, sin_g, 256, 0, 256, a1, d, 0, 1, rows, d, 256,
                         B2F_EPI_SILU, nullptr, 0, 0, nullptr, 0, st)))
       return rc;
-    if ((rc = gemm_bf16(a1, d, 0, c->g2.w, d, c->g2.b, eg, d, 0, 1, rows, d, d, B2F_EPI_BIAS,
+    if ((rc = lin_fwd(c->g2, tb, ls, a1, d, 0, d, eg, d, 0, 1, rows, d, d, B2F_EPI_BIAS,
                         nullptr, 0, 0, nullptr, 0, st)))
       return rc;
     eg_ptr = eg;
   }
-  if ((rc = gemm_bf16(pooled, pooled_ld, 0, c->p1.w, c->cfg.pooled_dim, c->p1.b, a1, d, 0, 1, rows, d,
+  if ((rc = lin_fwd(c->p1, tb, ls, pooled, pooled_ld, 0, c->cfg.pooled_dim, a1, d, 0, 1, rows, d,
                       c->cfg.pooled_dim, B2F_EPI_SILU, nullptr, 0, 0, nullptr, 0, st)))
     return rc;
-  if ((rc = gemm_bf16(a1, d, 0, c->p2.w, d, c->p2.b, ep, d, 0, 1, rows, d, d, B2F_EPI_BIAS, nullptr,
+  if ((rc = lin_fwd(c->p2, tb, ls, a1, d, 0, d, ep, d, 0, 1, rows, d, d, B2F_EPI_BIAS, nullptr,
                       0, 0, nullptr, 0, st)))
     return rc;
   return temb_combine(et, eg_ptr, ep, temb, silu_temb, (int64_t)rows * d, st);
@@ -236,9 +350,109 @@ int b2f_flux_temb(b2f_flux* h, const float* timestep, const float* guidance, con
 int b2f_flux_modulation(b2f_flux* h, const void* silu_temb, int rows, void* mod, b2f_stream_t stream_) {
   FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
   if (!c || !c->finalized || !silu_temb || !mod || rows <= 0) return B2F_ERR_INVALID;
+  if (!c->adaln_lora.empty()) {
+    fprintf(stderr, "[b2f] flux_modulation: AdaLN LoRA adapters are bound; use b2f_flux_modulation_ws\n");
+    return B2F_ERR_WORKSPACE;
+  }
   return gemm_bf16(silu_temb, c->d, 0, c->adaln.w, c->d, c->adaln.b, mod, c->mod_width, 0, 1, rows,
                    (int)c->mod_width, c->d, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0,
                    static_cast<cudaStream_t>(stream_));
+}
+
+size_t b2f_flux_modulation_workspace_bytes(const b2f_flux* h, int rows) {
+  const FluxCtx* c = reinterpret_cast<const FluxCtx*>(h);
+  if (!c || rows <= 0) return 0;
+  return (size_t)rows * adaln_rmax(c) * 2 + 256;
+}
+
+int b2f_flux_modulation_ws(b2f_flux* h, const void* silu_temb, int rows, void* mod, void* ws, size_t ws_bytes,
+                           b2f_stream_t stream_) {
+  FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
+  if (!c || !c->finalized || !silu_temb || !mod || rows <= 0 || !ws) return B2F_ERR_INVALID;
+  if (ws_bytes < b2f_flux_modulation_workspace_bytes(h, rows)) return B2F_ERR_WORKSPACE;
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  const int64_t d = c->d;
+  int rc = gemm_bf16(silu_temb, d, 0, c->adaln.w, d, c->adaln.b, mod, c->mod_width, 0, 1, rows, (int)c->mod_width,
+                     (int)d, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st);
+  if (rc) return rc;
+  // each AdaLN linear with an adapter: its own K-extended launch over its rows of adaln, overwriting its columns of mod
+  bf16_t* tb = reinterpret_cast<bf16_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255));
+  bf16_t* m = static_cast<bf16_t*>(mod);
+  for (const auto& kv : c->adaln_lora) {
+    const AdalnLora& a = kv.second;
+    Lin l;
+    l.w = c->adaln.w + a.row0 * d;
+    l.b = c->adaln.b + a.row0;
+    l.lora = a.l;
+    if ((rc = lin_fwd(l, tb, c->lora_scale, silu_temb, d, 0, d, m + a.row0, c->mod_width, 0, 1, rows, (int)a.rows,
+                      (int)d, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st)))
+      return rc;
+  }
+  return B2F_OK;
+}
+
+int b2f_flux_bind_lora(b2f_flux* h, const char* target, const void* Acat, const void* Bcat, const float* colscale,
+                       int r_pad) {
+  FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
+  if (!c || !c->finalized || !target) return B2F_ERR_INVALID;
+  const bool unbind = Acat == nullptr;
+  if (!unbind) {
+    if (!Bcat || !colscale || r_pad <= 0 || r_pad % 64) return B2F_ERR_INVALID;
+    if ((reinterpret_cast<uintptr_t>(Acat) | reinterpret_cast<uintptr_t>(Bcat) |
+         reinterpret_cast<uintptr_t>(colscale)) & 15)
+      return B2F_ERR_ALIGN;
+  }
+  LoraBind lb;
+  if (!unbind) {
+    lb.A = static_cast<const bf16_t*>(Acat);
+    lb.Bc = static_cast<const bf16_t*>(Bcat);
+    lb.cs = colscale;
+    lb.r_pad = r_pad;
+  }
+  const std::string key(target);
+  bool found = false;
+  for_each_linear(c, [&](const std::string& name, Lin* l, int64_t row0, int64_t out_f, int64_t) {
+    if (found || name != key) return;
+    found = true;
+    if (l) {
+      l->lora = lb;
+    } else if (unbind) {
+      c->adaln_lora.erase(key);
+    } else {
+      AdalnLora a;
+      a.row0 = row0;
+      a.rows = out_f;
+      a.l = lb;
+      c->adaln_lora[key] = a;
+    }
+  });
+  if (!found) {
+    fprintf(stderr, "[b2f] flux_bind_lora: no linear named '%s'\n", target);
+    return B2F_ERR_INVALID;
+  }
+  return B2F_OK;
+}
+
+int b2f_flux_clear_lora(b2f_flux* h) {
+  FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
+  if (!c || !c->finalized) return B2F_ERR_INVALID;
+  for_each_linear(c, [](const std::string&, Lin* l, int64_t, int64_t, int64_t) {
+    if (l) l->lora = LoraBind();
+  });
+  c->adaln_lora.clear();
+  return B2F_OK;
+}
+
+int b2f_flux_set_lora_scale(b2f_flux* h, float scale) {
+  FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
+  if (!c) return B2F_ERR_INVALID;
+  c->lora_scale = scale;
+  return B2F_OK;
+}
+
+int b2f_flux_lora_rank(const b2f_flux* h) {
+  const FluxCtx* c = reinterpret_cast<const FluxCtx*>(h);
+  return c && c->finalized ? c->lora_rmax() : 0;
 }
 
 int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const void* mod,
@@ -269,6 +483,8 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
   bf16_t* xn = hb + BS * d;        // [B,S,d]
   bf16_t* qkv = xn + BS * d;       // [B,S,3d]
   bf16_t* cat = qkv + BS * 3 * d;  // [B,S,5d]
+  bf16_t* tb = cat + BS * 5 * d;   // LoRA T [B,S,r_pad] (only with adapters bound)
+  const float ls = c->lora_scale;
   const int64_t h_bs = (int64_t)S * d, qkv_bs = (int64_t)S * 3 * d, cat_bs = (int64_t)S * 5 * d;
   bf16_t* h_img = hb + (int64_t)S_txt * d;
   bf16_t* h_txt = hb;
@@ -288,12 +504,10 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
 
   if (first_block == 0) {
     // x = x_embedder(hidden) -> h[:, S_txt:],  c = context_embedder(enc) -> h[:, :S_txt]
-    RUN(gemm_bf16(hidden, g.in_channels, (int64_t)S_img * g.in_channels, c->x_embedder.w,
-                  g.in_channels, c->x_embedder.b, h_img, d, h_bs, B, S_img, (int)d, g.in_channels,
-                  B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
-    RUN(gemm_bf16(enc, g.joint_dim, (int64_t)S_txt * g.joint_dim, c->context_embedder.w, g.joint_dim,
-                  c->context_embedder.b, h_txt, d, h_bs, B, S_txt, (int)d, g.joint_dim, B2F_EPI_BIAS,
-                  nullptr, 0, 0, nullptr, 0, st));
+    RUN(lin_fwd(c->x_embedder, tb, ls, hidden, g.in_channels, (int64_t)S_img * g.in_channels, g.in_channels, h_img,
+                d, h_bs, B, S_img, (int)d, g.in_channels, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
+    RUN(lin_fwd(c->context_embedder, tb, ls, enc, g.joint_dim, (int64_t)S_txt * g.joint_dim, g.joint_dim, h_txt, d,
+                h_bs, B, S_txt, (int)d, g.joint_dim, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
   }
 
   for (int blk = first_block; blk < last_block; ++blk) {
@@ -306,26 +520,26 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
       RUN(ln_modulate(hb, d, h_bs, mt + d, mt, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt, mi + d, mi, st));
       // QKV projections with per-head RMSNorm + RoPE fused into the GEMM epilogue; both streams write
       // straight into the joint [txt; img] qkv buffer
-      RUN(gemm_qkv_norm_rope(xn_img, d, h_bs, w.qkv.w, d, w.qkv.b, qkv_img, 3 * d, qkv_bs, B, S_img, (int)d,
+      RUN(qkv_fwd(w.qkv, tb, ls, xn_img, d, h_bs, d, qkv_img, 3 * d, qkv_bs, B, S_img, (int)d,
                              (int)d, w.norm_q, w.norm_k, c->rope_cos, c->rope_sin, S_txt, eps, 0, nullptr, 0, 0, 0, st));
-      RUN(gemm_qkv_norm_rope(xn_txt, d, h_bs, w.add_qkv.w, d, w.add_qkv.b, qkv_txt, 3 * d, qkv_bs, B, S_txt,
+      RUN(qkv_fwd(w.add_qkv, tb, ls, xn_txt, d, h_bs, d, qkv_txt, 3 * d, qkv_bs, B, S_txt,
                              (int)d, (int)d, w.norm_added_q, w.norm_added_k, c->rope_cos, c->rope_sin, 0, eps, 0,
                              nullptr, 0, 0, 0, st));
       RUN(attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S,
                         g.head_dim, scale, 0, st));
-      RUN(gemm_bf16(cat_img, 5 * d, cat_bs, w.to_out.w, d, w.to_out.b, h_img, d, h_bs, B, S_img,
+      RUN(lin_fwd(w.to_out, tb, ls, cat_img, 5 * d, cat_bs, d, h_img, d, h_bs, B, S_img,
                     (int)d, (int)d, B2F_EPI_GATE_RESID, h_img, d, h_bs, mi + 2 * d, mod_ld, st));
-      RUN(gemm_bf16(cat_txt, 5 * d, cat_bs, w.to_add_out.w, d, w.to_add_out.b, h_txt, d, h_bs, B,
+      RUN(lin_fwd(w.to_add_out, tb, ls, cat_txt, 5 * d, cat_bs, d, h_txt, d, h_bs, B,
                     S_txt, (int)d, (int)d, B2F_EPI_GATE_RESID, h_txt, d, h_bs, mt + 2 * d, mod_ld, st));
       RUN(ln_modulate(hb, d, h_bs, mt + 4 * d, mt + 3 * d, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt,
                       mi + 4 * d, mi + 3 * d, st));
-      RUN(gemm_bf16(xn_img, d, h_bs, w.ff1.w, d, w.ff1.b, cat_img + d, 5 * d, cat_bs, B, S_img,
+      RUN(lin_fwd(w.ff1, tb, ls, xn_img, d, h_bs, d, cat_img + d, 5 * d, cat_bs, B, S_img,
                     (int)(4 * d), (int)d, B2F_EPI_GELU_TANH, nullptr, 0, 0, nullptr, 0, st));
-      RUN(gemm_bf16(xn_txt, d, h_bs, w.ffc1.w, d, w.ffc1.b, cat_txt + d, 5 * d, cat_bs, B, S_txt,
+      RUN(lin_fwd(w.ffc1, tb, ls, xn_txt, d, h_bs, d, cat_txt + d, 5 * d, cat_bs, B, S_txt,
                     (int)(4 * d), (int)d, B2F_EPI_GELU_TANH, nullptr, 0, 0, nullptr, 0, st));
-      RUN(gemm_bf16(cat_img + d, 5 * d, cat_bs, w.ff2.w, 4 * d, w.ff2.b, h_img, d, h_bs, B, S_img,
+      RUN(lin_fwd(w.ff2, tb, ls, cat_img + d, 5 * d, cat_bs, 4 * d, h_img, d, h_bs, B, S_img,
                     (int)d, (int)(4 * d), B2F_EPI_GATE_RESID, h_img, d, h_bs, mi + 5 * d, mod_ld, st));
-      RUN(gemm_bf16(cat_txt + d, 5 * d, cat_bs, w.ffc2.w, 4 * d, w.ffc2.b, h_txt, d, h_bs, B, S_txt,
+      RUN(lin_fwd(w.ffc2, tb, ls, cat_txt + d, 5 * d, cat_bs, 4 * d, h_txt, d, h_bs, B, S_txt,
                     (int)d, (int)(4 * d), B2F_EPI_GATE_RESID, h_txt, d, h_bs, mt + 5 * d, mod_ld, st));
     } else {
       const int si = blk - g.num_double;
@@ -335,12 +549,12 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
       RUN(ln_modulate(hb, d, h_bs, ms + d, ms, mod_ld, xn, d, h_bs, B, S, (int)d, eps, 0, nullptr, nullptr, st));
       // ONE launch for [to_q;to_k;to_v;proj_mlp] (N = 7d): Q/K get RMSNorm+RoPE, V passes through into
       // qkv, the MLP columns are GELU'd straight into cat[:, :, d:5d]
-      RUN(gemm_qkv_norm_rope(xn, d, h_bs, w.qkv_mlp.w, d, w.qkv_mlp.b, qkv, 3 * d, qkv_bs, B, S, (int)d, (int)d,
+      RUN(qkv_fwd(w.qkv_mlp, tb, ls, xn, d, h_bs, d, qkv, 3 * d, qkv_bs, B, S, (int)d, (int)d,
                              w.norm_q, w.norm_k, c->rope_cos, c->rope_sin, 0, eps, (int)(4 * d), cat + d, 5 * d,
                              cat_bs, B2F_EPI_GELU_TANH, st));
       RUN(attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S,
                         g.head_dim, scale, 0, st));
-      RUN(gemm_bf16(cat, 5 * d, cat_bs, w.proj_out.w, 5 * d, w.proj_out.b, hb, d, h_bs, B, S, (int)d,
+      RUN(lin_fwd(w.proj_out, tb, ls, cat, 5 * d, cat_bs, 5 * d, hb, d, h_bs, B, S, (int)d,
                     (int)(5 * d), B2F_EPI_GATE_RESID, hb, d, h_bs, ms + 2 * d, mod_ld, st));
     }
   }
@@ -350,7 +564,7 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
     const bf16_t* mo = modp + (int64_t)g.num_double * 12 * d + (int64_t)g.num_single * 3 * d;
     RUN(ln_modulate(h_img, d, h_bs, mo, mo + d, mod_ld, xn_img, d, h_bs, B, n_out_rows, (int)d, eps, 0, nullptr,
                     nullptr, st));
-    RUN(gemm_bf16(xn_img, d, h_bs, c->proj_out.w, d, c->proj_out.b, out, g.out_channels,
+    RUN(lin_fwd(c->proj_out, tb, ls, xn_img, d, h_bs, d, out, g.out_channels,
                   (int64_t)n_out_rows * g.out_channels, B, n_out_rows, g.out_channels, (int)d,
                   B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
   }

@@ -169,6 +169,10 @@ int b2f_flux_train_forward(b2f_flux* h, const void* hidden, const void* enc, con
                            int B, int S_img, int S_txt, int n_out_rows, void* ws, size_t ws_bytes, b2f_stream_t stream_) {
   FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
   if (!c || !c->finalized || !ws) return B2F_ERR_INVALID;
+  if (c->lora_rmax() > 0) {   // the backward does not see unfused adapters: fuse or unbind them first
+    fprintf(stderr, "[b2f] flux_train_forward: unfused LoRA adapters are bound\n");
+    return B2F_ERR_UNSUPPORTED;
+  }
   if (ws_bytes < b2f_flux_train_workspace_bytes(h, B, S_img, S_txt)) return B2F_ERR_WORKSPACE;
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   const size_t infer = b2f_flux_workspace_bytes(h, B, S_img, S_txt);

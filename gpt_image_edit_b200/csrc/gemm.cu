@@ -258,10 +258,25 @@ __device__ __forceinline__ void tile_origin(const GemmParams& p, int t, int& n_b
 // order; its consumer warpgroups take turns on them (consumer 0: the CTA's tiles 0, 2, 4, ..., consumer 1: 1, 3, ...),
 // each owning a whole 128 x 128 tile (two m64n128k16 per k16 step).  While one runs its tile's MMAs the other runs the
 // epilogue of its previous tile, and the producer streams k-blocks through the ring across tile boundaries.
-template <int MODE>
+// LoRA K-extension of the forward GEMM (LORA = true, MODE 0 only): after a tile's K/64 k-blocks of (A, W) the
+// producer streams num_kb2 more from (T [batch, M, r_pad], Bcat [N, r_pad]) through the same ring and the consumers
+// run them into the same accumulators, so acc = A W^T + T Bcat^T before an unchanged epilogue.  With colscale set
+// (the down projection T = bf16(colscale[n] cs_mul (X Acat^T)), bias NULL, epilogue BIAS), the staged value is
+// bf16(acc * fp32(colscale[n] * cs_mul)).  LORA = false has an empty parameter and compiles to the plain kernel.
+template <bool LORA>
+struct LoraParams {};
+template <>
+struct LoraParams<true> {
+  CUtensorMap tmT, tmBc;
+  int num_kb2;
+  const float* colscale;
+  float cs_mul;
+};
+
+template <int MODE, bool LORA = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const GemmParams p) {
+                 const GemmParams p, const __grid_constant__ LoraParams<LORA> lx) {
   constexpr int TA = MODE == 2, TB = MODE >= 1;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -271,6 +286,12 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
+    if constexpr (LORA) {
+      if (lx.num_kb2 > 0) {
+        tma_prefetch_desc(&lx.tmT);
+        tma_prefetch_desc(&lx.tmBc);
+      }
+    }
     for (int i = 0; i < STAGES; ++i) {
       mbar_init(&full[i], 1);
       mbar_init(&empty[i], 4);   // one arrive per warp of the consumer that read the stage
@@ -282,6 +303,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const int num_tiles = p.num_m_blocks * p.num_n_blocks;
   const int n_local = (num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // this CTA's tiles
   const int num_kb = MODE == 2 ? p.kbatch * p.kb_per_batch : (p.K + BLOCK_K - 1) / BLOCK_K;
+  int num_kb_all = num_kb;   // k-blocks per tile, the LoRA ones last
+  if constexpr (LORA) num_kb_all += lx.num_kb2;
 
   if (wg == 0) {
     setmaxnreg_dec<PRODUCER_REGS>();
@@ -292,7 +315,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
         int n_blk, bb, mb;
         tile_origin(p, blockIdx.x + i * gridDim.x, n_blk, bb, mb);
         const int m_blk = bb * p.m_blocks_per_batch + mb;
-        for (int kb = 0; kb < num_kb; ++kb) {
+        for (int kb = 0; kb < num_kb_all; ++kb) {
           mbar_wait(&empty[stage], phase ^ 1);
           uint8_t* sa = ring + stage * STAGE_BYTES;
           uint8_t* sb = sa + A_BYTES;
@@ -307,13 +330,23 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             for (int h = 0; h < BLOCK_N / 64; ++h)
               tma_load_3d(sb + h * MN_BOX_BYTES, &tmB, &full[stage], n_blk * BLOCK_N + 64 * h, kr, kbb);
           } else {
-            tma_load_3d(sa, &tmA, &full[stage], kb * BLOCK_K, mb * BLOCK_M, bb);
+            const CUtensorMap* mapA = &tmA;
+            const CUtensorMap* mapB = &tmB;
+            int kc = kb * BLOCK_K;
+            if constexpr (LORA) {
+              if (kb >= num_kb) {   // the LoRA k-blocks: (T, Bcat) in place of (A, W)
+                mapA = &lx.tmT;
+                mapB = &lx.tmBc;
+                kc = (kb - num_kb) * BLOCK_K;
+              }
+            }
+            tma_load_3d(sa, mapA, &full[stage], kc, mb * BLOCK_M, bb);
             if (MODE == 1) {
 #pragma unroll
               for (int h = 0; h < BLOCK_N / 64; ++h)
-                tma_load_2d(sb + h * MN_BOX_BYTES, &tmB, &full[stage], n_blk * BLOCK_N + 64 * h, kb * BLOCK_K);
+                tma_load_2d(sb + h * MN_BOX_BYTES, mapB, &full[stage], n_blk * BLOCK_N + 64 * h, kc);
             } else {
-              tma_load_2d(sb, &tmB, &full[stage], kb * BLOCK_K, n_blk * BLOCK_N);
+              tma_load_2d(sb, mapB, &full[stage], kc, n_blk * BLOCK_N);
             }
           }
           if (++stage == STAGES) {
@@ -345,7 +378,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     tile_origin(p, blockIdx.x + i * gridDim.x, n_blk, bb, mb);
 
     // ---- main loop: this consumer's turn on the tensor cores.  Its tile's k-blocks are ring slots
-    // i * num_kb .. (i + 1) * num_kb - 1 in the producer's order.
+    // i * num_kb_all .. (i + 1) * num_kb_all - 1 in the producer's order.
     float acc0[64], acc1[64];   // rows 0..63 / 64..127 of the tile
 #pragma unroll
     for (int j = 0; j < 64; ++j) {
@@ -353,10 +386,10 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       acc1[j] = 0.f;
     }
     named_bar_sync(BAR_TURN + c, 256);
-    const int slot0 = i * num_kb;
+    const int slot0 = i * num_kb_all;
     int stage = slot0 % STAGES, prev = -1;
     uint32_t phase = (slot0 / STAGES) & 1;
-    for (int kb = 0; kb < num_kb; ++kb) {
+    for (int kb = 0; kb < num_kb_all; ++kb) {
       mbar_wait(&full[stage], phase);
       const uint64_t soff = uint64_t((stage * STAGE_BYTES) >> 4);
       reg_fence(acc0);
@@ -431,6 +464,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int n = n_blk * BLOCK_N + col;
       const bool has_bias = p.bias && n < p.N;
       const float2 b2 = has_bias ? unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n))) : make_float2(0.f, 0.f);
+      float2 cs2 = make_float2(1.f, 1.f);
+      if constexpr (LORA) {
+        if (lx.colscale && n < p.N) {
+          cs2 = __ldg(reinterpret_cast<const float2*>(lx.colscale + n));
+          cs2.x *= lx.cs_mul;
+          cs2.y *= lx.cs_mul;
+        }
+      }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const float* a = h ? acc1 : acc0;
@@ -440,6 +481,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           x1 += b2.y;
           x2 += b2.x;
           x3 += b2.y;
+        }
+        if constexpr (LORA) {
+          if (lx.colscale) {
+            x0 *= cs2.x;
+            x1 *= cs2.y;
+            x2 *= cs2.x;
+            x3 *= cs2.y;
+          }
         }
         uint8_t* s0 = stg + (64 * h + r_lo) * SROW + col * 2;
         *reinterpret_cast<uint32_t*>(s0) = pack_bf16x2(x0, x1);
@@ -506,11 +555,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 }
 
-template <int MODE>
-int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream) {
+template <int MODE, bool LORA = false>
+int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream,
+                const LoraParams<LORA>& lx = LoraParams<LORA>{}) {
+  static_assert(!LORA || MODE == 0, "the LoRA K-extension is forward-only");
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<MODE, LORA>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          PP_SMEM_BYTES);
     if (e != cudaSuccess) return cuda_err(e, "gemm smem attribute");
     attr_set = true;
@@ -521,12 +572,22 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cu
   p.panel_n = 16;
   const int num_tiles = p.num_m_blocks * p.num_n_blocks;
   const int grid = std::min(num_tiles, device_info().num_sms);   // persistent: at most one CTA per SM
-  const double kk = MODE == 2 ? (double)p.kbatch * p.K : (double)p.K;
+  int k_ext = 0;
+  bool down = false;
+  if constexpr (LORA) {
+    k_ext = lx.num_kb2 * BLOCK_K;
+    down = lx.colscale != nullptr;
+  }
+  const double kk = MODE == 2 ? (double)p.kbatch * p.K : (double)p.K + k_ext;
   prof_begin(KC_GEMM, stream);
-  gemm_bf16_kernel<MODE><<<grid, THREADS, PP_SMEM_BYTES, stream>>>(tmA, tmB, p);
+  gemm_bf16_kernel<MODE, LORA><<<grid, THREADS, PP_SMEM_BYTES, stream>>>(tmA, tmB, p, lx);
   {
     char tag_[96];
-    snprintf(tag_, sizeof tag_, "gemm m%d %dx%dx%d b%d e%d", MODE, p.M, p.N, (int)kk, p.batch, p.epi);
+    if (LORA)
+      snprintf(tag_, sizeof tag_, "gemm lora %dx%dx%d+%d b%d e%d%s", p.M, p.N, p.K, k_ext, p.batch, p.epi,
+               down ? " down" : "");
+    else
+      snprintf(tag_, sizeof tag_, "gemm m%d %dx%dx%d b%d e%d", MODE, p.M, p.N, (int)kk, p.batch, p.epi);
     prof_end_tagged(KC_GEMM, stream, 2.0 * p.batch * (double)p.M * p.N * kk,
                     2.0 * ((double)p.batch * p.M * kk + (double)p.N * kk + (double)p.batch * p.M * p.N), tag_);
   }
@@ -547,10 +608,23 @@ struct QkvExtra {
   int64_t ld_extra, bs_extra;
 };
 
+// LoRA operands of one forward launch (see LoraParams): T [batch, M, r_pad] (row pitch ldt, batch pitch t_bs) and
+// Bcat [N, r_pad] (pitch ldbc) extend the contraction by r_pad (a multiple of 64; 0: no extension); colscale != NULL
+// makes the launch a down projection.
+struct LoraExt {
+  const void* T;
+  int64_t ldt, t_bs;
+  const void* Bc;
+  int64_t ldbc;
+  int r_pad;
+  const float* colscale;
+  float cs_mul;
+};
+
 static int gemm_bf16_impl(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
               const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N,
               int K, int epilogue, const void* resid, int64_t ldr, int64_t resid_bs, const void* gate,
-              int64_t gate_ld, const QkvExtra* qx, cudaStream_t stream) {
+              int64_t gate_ld, const QkvExtra* qx, cudaStream_t stream, const LoraExt* lx = nullptr) {
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (batch <= 0 || M <= 0 || N <= 0 || K <= 0 || !A || !W || !out) return B2F_ERR_INVALID;
   if ((K & 7) || (N & 7) || (lda & 7) || (ldw & 7) || (ldc & 7) || (a_bs & 7) || (out_bs & 7))
@@ -614,7 +688,30 @@ static int gemm_bf16_impl(const void* A, int64_t lda, int64_t a_bs, const void* 
   if (rc != B2F_OK) return rc;
   rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, BLOCK_N, BLOCK_K);
   if (rc != B2F_OK) return rc;
-  return launch_gemm<0>(tmA, tmB, p, stream);
+  if (!lx) return launch_gemm<0>(tmA, tmB, p, stream);
+
+  if (lx->r_pad < 0 || (lx->r_pad % BLOCK_K)) return B2F_ERR_INVALID;
+  if (lx->colscale && (lx->r_pad || bias || epilogue != B2F_EPI_BIAS)) return B2F_ERR_INVALID;
+  if (!lx->colscale && !lx->r_pad) return B2F_ERR_INVALID;
+  if (lx->colscale && (reinterpret_cast<uintptr_t>(lx->colscale) & 15)) return B2F_ERR_ALIGN;
+  LoraParams<true> lp;
+  lp.tmT = tmA;   // unread without an extension
+  lp.tmBc = tmB;
+  lp.num_kb2 = lx->r_pad / BLOCK_K;
+  lp.colscale = lx->colscale;
+  lp.cs_mul = lx->cs_mul;
+  if (lx->r_pad) {
+    if (!lx->T || !lx->Bc) return B2F_ERR_INVALID;
+    if ((lx->ldt & 7) || (lx->t_bs & 7) || (lx->ldbc & 7) || lx->ldt < lx->r_pad || lx->ldbc < lx->r_pad ||
+        ((reinterpret_cast<uintptr_t>(lx->T) | reinterpret_cast<uintptr_t>(lx->Bc)) & 15))
+      return B2F_ERR_ALIGN;
+    rc = make_tmap_3d_rows(&lp.tmT, lx->T, (uint64_t)lx->r_pad, (uint64_t)M, (uint64_t)batch, (uint64_t)lx->ldt,
+                           batch > 1 ? (uint64_t)lx->t_bs : (uint64_t)M * lx->ldt);
+    if (rc != B2F_OK) return rc;
+    rc = make_tmap_2d_bf16(&lp.tmBc, lx->Bc, (uint64_t)N, (uint64_t)lx->r_pad, (uint64_t)lx->ldbc, BLOCK_N, BLOCK_K);
+    if (rc != B2F_OK) return rc;
+  }
+  return launch_gemm<0, true>(tmA, tmB, p, stream, lp);
 }
 
 int gemm_bf16(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
@@ -702,6 +799,41 @@ int gemm_qkv_norm_rope(const void* A, int64_t lda, int64_t a_bs, const void* W, 
   QkvExtra qx{nw_q, nw_k, cos, sin, rope_row0, d_model, eps, n_extra, epi_extra, out_extra, ld_extra, bs_extra};
   return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, 3 * d_model + n_extra, K,
                         B2F_EPI_QKV_NORM_ROPE, nullptr, 0, 0, nullptr, 0, &qx, stream);
+}
+
+// ---------------------------------------------------------------------------------------------------- LoRA
+// out = epi(A W^T + T Bcat^T + bias): the forward GEMM with r_pad / 64 extra k-blocks per tile (LoraExt).
+int gemm_bf16_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias, void* out,
+                   int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epilogue, const void* resid,
+                   int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld, const void* T, int64_t ldt,
+                   int64_t t_bs, const void* Bc, int64_t ldbc, int r_pad, cudaStream_t stream) {
+  if (epilogue == B2F_EPI_QKV_NORM_ROPE || r_pad <= 0) return B2F_ERR_INVALID;
+  const LoraExt lx{T, ldt, t_bs, Bc, ldbc, r_pad, nullptr, 1.f};
+  return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, N, K, epilogue, resid, ldr,
+                        resid_bs, gate, gate_ld, nullptr, stream, &lx);
+}
+
+int gemm_qkv_norm_rope_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias,
+                            void* out, int64_t ldc, int64_t out_bs, int batch, int M, int d_model, int K,
+                            const void* nw_q, const void* nw_k, const float* cos, const float* sin, int rope_row0,
+                            float eps, int n_extra, void* out_extra, int64_t ld_extra, int64_t bs_extra,
+                            int epi_extra, const void* T, int64_t ldt, int64_t t_bs, const void* Bc, int64_t ldbc,
+                            int r_pad, cudaStream_t stream) {
+  if (r_pad <= 0) return B2F_ERR_INVALID;
+  QkvExtra qx{nw_q, nw_k, cos, sin, rope_row0, d_model, eps, n_extra, epi_extra, out_extra, ld_extra, bs_extra};
+  const LoraExt lx{T, ldt, t_bs, Bc, ldbc, r_pad, nullptr, 1.f};
+  return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, 3 * d_model + n_extra, K,
+                        B2F_EPI_QKV_NORM_ROPE, nullptr, 0, 0, nullptr, 0, &qx, stream, &lx);
+}
+
+// LoRA down projection: out[batch, M, N] = bf16((A W^T)[., n] * fp32(colscale[n] * cs_mul)), W = Acat [N, K].
+int gemm_colscale(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, void* out, int64_t ldc,
+                  int64_t out_bs, int batch, int M, int N, int K, const float* colscale, float cs_mul,
+                  cudaStream_t stream) {
+  if (!colscale) return B2F_ERR_INVALID;
+  const LoraExt lx{nullptr, 0, 0, nullptr, 0, 0, colscale, cs_mul};
+  return gemm_bf16_impl(A, lda, a_bs, W, ldw, nullptr, out, ldc, out_bs, batch, M, N, K, B2F_EPI_BIAS, nullptr, 0, 0,
+                        nullptr, 0, nullptr, stream, &lx);
 }
 
 }  // namespace b2f

@@ -18,6 +18,7 @@ import torch
 
 from . import _lib
 from ._lib import check, ptr, stream_ptr
+from .lora import FluxLoraMixin
 
 
 class FluxTransformerConfig(SimpleNamespace):
@@ -86,7 +87,7 @@ def _norm_weights(cfg: FluxTransformerConfig):
     return out
 
 
-class B200FluxTransformer2DModel(torch.nn.Module):
+class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
     def __init__(self, config: FluxTransformerConfig | None = None, device="cuda", **kw):
         super().__init__()
         self.config = config or FluxTransformerConfig(**kw)
@@ -131,6 +132,7 @@ class B200FluxTransformer2DModel(torch.nn.Module):
         self._rope = None
         self._schedule = None
         self.gradient_checkpointing = False
+        self._lora_init()
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -215,7 +217,14 @@ class B200FluxTransformer2DModel(torch.nn.Module):
         ws = self._workspace(nws, "temb")
         check(_lib.lib.b2f_flux_temb(self._h, ptr(t1000), ptr(g1000), ptr(pooled), pooled.stride(0), rows,
                                      ptr(temb), ptr(stemb), ptr(ws), nws, stream_ptr()), "b2f_flux_temb")
-        check(_lib.lib.b2f_flux_modulation(self._h, ptr(stemb), rows, ptr(mod), stream_ptr()), "b2f_flux_modulation")
+        if self._lora_bound:   # AdaLN adapters run as their own K-extended launches over their rows of adaln
+            nws = int(_lib.lib.b2f_flux_modulation_workspace_bytes(self._h, rows))
+            ws = self._workspace(nws, "mod")
+            check(_lib.lib.b2f_flux_modulation_ws(self._h, ptr(stemb), rows, ptr(mod), ptr(ws), nws, stream_ptr()),
+                  "b2f_flux_modulation_ws")
+        else:
+            check(_lib.lib.b2f_flux_modulation(self._h, ptr(stemb), rows, ptr(mod), stream_ptr()),
+                  "b2f_flux_modulation")
         if want_silu:
             return temb, mod, stemb
         return temb, mod
@@ -227,11 +236,14 @@ class B200FluxTransformer2DModel(torch.nn.Module):
         return (x.to(torch.bfloat16) * 1000).float().contiguous()
 
     def prepare_schedule(self, timesteps_over_1000: torch.Tensor, guidance: torch.Tensor | None,
-                         pooled_projections: torch.Tensor):
+                         pooled_projections: torch.Tensor, lora_scale: float = 1.0):
         """Hoist the AdaLN modulation of a whole sampling schedule (one weight-streaming GEMM
         with M = steps*B instead of `steps` GEMMs with M = B).  timesteps_over_1000: [n_steps]
-        values exactly as the loop will pass them (bf16, already divided by 1000)."""
+        values exactly as the loop will pass them (bf16, already divided by 1000).  lora_scale: the
+        joint_attention_kwargs["scale"] the loop will pass (unfused AdaLN adapters act at that scale); a
+        forward whose scale or adapters differ from the schedule's computes its own modulation."""
         n = timesteps_over_1000.numel()
+        self._set_lora_scale(lora_scale)
         B = pooled_projections.shape[0]
         t = self._times1000(timesteps_over_1000.reshape(n, 1).expand(n, B).reshape(-1))
         g = None
@@ -239,8 +251,12 @@ class B200FluxTransformer2DModel(torch.nn.Module):
             g = self._times1000(guidance.reshape(1, B).expand(n, B).reshape(-1))
         pooled = pooled_projections.to(torch.bfloat16).repeat(n, 1).contiguous()
         _, mod = self._temb_mod(t, g, pooled)
-        self._schedule = SimpleNamespace(n=n, B=B, mod=mod.view(n, B, self.mod_width))
+        self._schedule = SimpleNamespace(n=n, B=B, mod=mod.view(n, B, self.mod_width),
+                                         lora_key=(self._lora_version, float(lora_scale)))
         return self._schedule
+
+    def _set_lora_scale(self, s: float):
+        check(_lib.lib.b2f_flux_set_lora_scale(self._h, float(s)), "b2f_flux_set_lora_scale")
 
     def _set_rope(self, txt_ids, img_ids, S_txt: int, S_img: int):
         """FluxPosEmbed tables for [txt; img] ids, handed to the engine (rebuilt only when the ids change)."""
@@ -273,8 +289,11 @@ class B200FluxTransformer2DModel(torch.nn.Module):
         enc = encoder_hidden_states.to(torch.bfloat16).contiguous()
         self._set_rope(txt_ids, img_ids, S_txt, S_img)
 
+        lora_scale = float(jak.pop("scale", 1.0))   # diffusers pops `scale` the same way (PEFT per-call scale)
+        self._set_lora_scale(lora_scale)
         step = jak.get("_b2f_schedule_step")
-        if step is not None and self._schedule is not None and self._schedule.B == B:
+        if (step is not None and self._schedule is not None and self._schedule.B == B
+                and self._schedule.lora_key == (self._lora_version, lora_scale)):
             mod = self._schedule.mod[int(step)]
         else:
             t = self._times1000(timestep.reshape(-1).expand(B))

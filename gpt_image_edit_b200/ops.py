@@ -293,3 +293,81 @@ def blend(a, b, wa: float, wb: float, *, out=None) -> torch.Tensor:
         out = torch.empty_like(a)
     check(_lib.lib.b2f_blend_bf16(ptr(a), ptr(b), float(wa), float(wb), ptr(out), a.numel(), stream_ptr()), "b2f_blend_bf16")
     return out
+
+
+# ------------------------------------------------------------------------------------------------ LoRA
+def lora_down(x, acat, colscale, *, cs_mul: float = 1.0, out=None) -> torch.Tensor:
+    """T = bf16(fp32(x @ acat^T) * fp32(colscale * cs_mul)) via b2f_gemm_colscale.  x [.., K], acat [r_pad, K],
+    colscale fp32 [r_pad]."""
+    _req(x, "x")
+    _req(acat, "acat")
+    _req(colscale, "colscale", torch.float32)
+    x3 = _as3(x)
+    B, M, K = x3.shape
+    N = acat.shape[0]
+    if out is None:
+        out = torch.empty((*x.shape[:-1], N), device=x.device, dtype=torch.bfloat16)
+    o3 = _as3(out)
+    check(_lib.lib.b2f_gemm_colscale(ptr(x3), x3.stride(1), x3.stride(0), ptr(acat), acat.stride(0), ptr(o3),
+                                     o3.stride(1), o3.stride(0), B, M, N, K, ptr(colscale), float(cs_mul), stream_ptr()),
+          "b2f_gemm_colscale")
+    return out
+
+
+def linear_lora(x, weight, bias, t, bcat, *, epilogue: int = EPI_BIAS, out=None, resid=None, gate=None) -> torch.Tensor:
+    """out = epilogue(x @ weight^T + t @ bcat^T + bias) via b2f_gemm_bf16_lora (one fp32 accumulation).
+    t [.., r_pad] (rows as x), bcat [N, r_pad]."""
+    _req(x, "x")
+    _req(weight, "weight")
+    _req(t, "t")
+    _req(bcat, "bcat")
+    x3, t3 = _as3(x), _as3(t)
+    B, M, K = x3.shape
+    N = weight.shape[0]
+    if out is None:
+        out = torch.empty((*x.shape[:-1], N), device=x.device, dtype=torch.bfloat16)
+    o3 = _as3(out)
+    ldr = rbs = gld = 0
+    if epilogue in (EPI_GATE_RESID, EPI_RESID):
+        r3 = _as3(resid)
+        ldr, rbs = r3.stride(1), r3.stride(0)
+        if epilogue == EPI_GATE_RESID:
+            gld = gate.stride(0) if gate.dim() == 2 else 0
+    check(_lib.lib.b2f_gemm_bf16_lora(ptr(x3), x3.stride(1), x3.stride(0), ptr(weight), weight.stride(0), ptr(bias),
+                                      ptr(o3), o3.stride(1), o3.stride(0), B, M, N, K, epilogue, ptr(resid), ldr, rbs,
+                                      ptr(gate), gld, ptr(t3), t3.stride(1), t3.stride(0), ptr(bcat), bcat.stride(0),
+                                      bcat.shape[1], stream_ptr()), "b2f_gemm_bf16_lora")
+    return out
+
+
+def linear_qkv_norm_rope_lora(x, weight, bias, wq, wk, cos, sin, t, bcat, *, rope_row0: int = 0, out=None,
+                              eps: float = 1e-6, out_extra=None, epi_extra: int = EPI_BIAS):
+    """linear_qkv_norm_rope with the LoRA K-extension (t, bcat) of linear_lora."""
+    _req(x, "x")
+    _req(t, "t")
+    _req(bcat, "bcat")
+    x3, t3 = _as3(x), _as3(t)
+    B, M, K = x3.shape
+    n_extra = 0 if out_extra is None else out_extra.shape[-1]
+    N = weight.shape[0] - n_extra
+    if out is None:
+        out = torch.empty((*x.shape[:-1], N), device=x.device, dtype=torch.bfloat16)
+    o3 = _as3(out)
+    e3 = None if out_extra is None else _as3(out_extra)
+    check(_lib.lib.b2f_gemm_qkv_norm_rope_lora(
+        ptr(x3), x3.stride(1), x3.stride(0), ptr(weight), weight.stride(0), ptr(bias), ptr(o3), o3.stride(1),
+        o3.stride(0), B, M, N // 3, K, ptr(wq), ptr(wk), ptr(cos), ptr(sin), rope_row0, eps, n_extra, ptr(e3),
+        0 if e3 is None else e3.stride(1), 0 if e3 is None else e3.stride(0), epi_extra, ptr(t3), t3.stride(1),
+        t3.stride(0), ptr(bcat), bcat.stride(0), bcat.shape[1], stream_ptr()), "b2f_gemm_qkv_norm_rope_lora")
+    return out
+
+
+def lora_fuse_(weight, bcat, acat, colscale, *, cs_mul: float = 1.0) -> torch.Tensor:
+    """In place: weight <- bf16(weight + sum_k fp32(bcat[:, k] * colscale[k] * cs_mul) acat[k]) (b2f_lora_fuse)."""
+    for t, n in ((weight, "weight"), (bcat, "bcat"), (acat, "acat")):
+        _req(t, n)
+    _req(colscale, "colscale", torch.float32)
+    check(_lib.lib.b2f_lora_fuse(ptr(weight), weight.stride(0), weight.shape[0], weight.shape[1], ptr(bcat),
+                                 bcat.stride(0), ptr(acat), acat.stride(0), ptr(colscale), float(cs_mul), acat.shape[0],
+                                 stream_ptr()), "b2f_lora_fuse")
+    return weight

@@ -209,6 +209,50 @@ class FluxKontextPipeline:
     def disable_vae_tiling(self):
         self.vae.disable_tiling()
 
+    # LoRA (diffusers FluxLoraLoaderMixin, which the reference's pipeline inherits: flux_pipeline.py:30, 193-195).  Only
+    # the transformer takes adapters; each call delegates to the matching B200FluxTransformer2DModel method.
+    def load_lora_weights(self, pretrained_model_name_or_path_or_dict, adapter_name=None, weight_name=None, **kw):
+        """Load a LoRA (diffusers / PEFT, BFL or kohya layout; a dict or a local .safetensors file) onto the transformer.
+        The new adapter joins the active set with weight 1.0; see FluxLoraMixin for the rules."""
+        return self.transformer.load_lora_adapter(pretrained_model_name_or_path_or_dict, adapter_name=adapter_name,
+                                                  weight_name=weight_name, **kw)
+
+    def set_adapters(self, adapter_names, adapter_weights=None):
+        self.transformer.set_adapters(adapter_names, adapter_weights)
+
+    def get_active_adapters(self):
+        return self.transformer.get_active_adapters()
+
+    def get_list_adapters(self):
+        return self.transformer.get_list_adapters()
+
+    def delete_adapters(self, adapter_names):
+        self.transformer.delete_adapters(adapter_names)
+
+    def disable_lora(self):
+        self.transformer.disable_lora()
+
+    def enable_lora(self):
+        self.transformer.enable_lora()
+
+    def unload_lora_weights(self):
+        self.transformer.unload_lora()
+
+    @staticmethod
+    def _lora_components(components):
+        comps = [components] if isinstance(components, str) else list(components)
+        bad = [c for c in comps if c != "transformer"]
+        if bad:
+            raise ValueError(f"LoRA is supported on the transformer only, not on {bad}")
+
+    def fuse_lora(self, components=("transformer",), lora_scale: float = 1.0, adapter_names=None, **kw):
+        self._lora_components(components)
+        self.transformer.fuse_lora(lora_scale=lora_scale, adapter_names=adapter_names)
+
+    def unfuse_lora(self, components=("transformer",)):
+        self._lora_components(components)
+        self.transformer.unfuse_lora()
+
     @classmethod
     def from_pretrained(cls, flux_path, transformer=None, torch_dtype=torch.bfloat16, **kw):
         """Reference univa/serve/cli.py:64-68.  Builds scheduler + VAE from `flux_path` when a
@@ -464,7 +508,8 @@ class FluxKontextPipeline:
         hoist = hasattr(self.transformer, "prepare_schedule")
         if hoist:
             # the loop passes timestep = t.to(dtype) / 1000 (reference :1065-1069): hoist with exactly those values
-            self.transformer.prepare_schedule(timesteps.to(dtype) / 1000, guidance, pooled_prompt_embeds)
+            sched_kw = {"lora_scale": float(jak["scale"])} if "scale" in jak else {}
+            self.transformer.prepare_schedule(timesteps.to(dtype) / 1000, guidance, pooled_prompt_embeds, **sched_kw)
             jak["_b2f_out_rows"] = n_tgt
 
         self.scheduler.set_begin_index(0)

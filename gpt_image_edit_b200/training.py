@@ -297,6 +297,9 @@ class FluxTrainGraph:
     def __init__(self, model, params, on_block_done=None):
         self.model = model
         self.den = model.denoise_tower.denoiser
+        if getattr(self.den, "lora_unfused_active", lambda: False)():
+            raise _lib.B2FError("the denoiser has unfused LoRA adapters active and the training backward does not see them: "
+                           "fuse_lora() or disable / unload them first")
         self.proj = getattr(model.denoise_tower, "denoise_projector", None)
         self.params = params
         self.on_block_done = on_block_done          # callback(bucket) after a block's gradients are complete

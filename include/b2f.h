@@ -33,7 +33,7 @@ extern "C" {
 typedef void* b2f_stream_t; /* cudaStream_t */
 
 const char* b2f_strerror(int code);
-/* ABI version; bumped on any signature change. */
+/* ABI version; bumped on any signature change or addition (2: LoRA entry points). */
 int b2f_version(void);
 /* Device facts the host needs for grid sizing / reporting. Returns B2F_ERR_NODEVICE without GPU. */
 int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin);
@@ -105,6 +105,50 @@ int b2f_gemm_qkv_norm_rope(const void* A, int64_t lda, int64_t a_batch_stride, c
                            const void* nw_q, const void* nw_k, const float* cos, const float* sin,
                            int rope_row0, float eps, int n_extra, void* out_extra, int64_t ld_extra,
                            int64_t extra_batch_stride, int epi_extra, b2f_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * LoRA (low-rank adapters) on the linear layers.  Replaces the PEFT LoraLayer forward / merge that diffusers'
+ * FluxLoraLoaderMixin installs on FluxTransformer2DModel (reference univa/utils/flux_pipeline.py:30, 193-195 inherits
+ * load_lora_weights / set_adapters / fuse_lora; the per-call scale is joint_attention_kwargs["scale"], :922-924).
+ *
+ * Adapters i = 1..n on one linear, of ranks r_i, are held concatenated: Acat [r_pad, in] (rows of every A_i),
+ * Bcat [out, r_pad] (columns of every B_i), colscale fp32 [r_pad] (alpha_i / r_i x adapter weight_i on adapter i's
+ * columns); r_pad = sum r_i rounded up to 64 with zero rows / columns / scales.  An unfused forward is two launches:
+ *   down projection  T = bf16(fp32(X Acat^T)[:, k] * fp32(colscale[k] * s))           (b2f_gemm_colscale)
+ *   K-extended GEMM  out = epilogue(fp32(X W^T + T Bcat^T) + bias)                    (b2f_gemm_bf16_lora)
+ * where s is the call scale and the second launch accumulates both products into the same fp32 accumulators (r_pad/64
+ * extra k-blocks per tile) before the unchanged epilogue.  Rounding chain: T is rounded to bf16 once; base and LoRA
+ * products share one fp32 accumulation and the epilogue's roundings.  PEFT differs: it rounds the base output
+ * bf16(X W^T + b) and the LoRA output bf16(bf16(bf16(X A^T) B^T) * scaling) separately and adds them in bf16 — so
+ * outputs agree with PEFT to bf16 rounding, not bit for bit.
+ */
+/* b2f_gemm_bf16 (every forward epilogue, same arguments) with the contraction extended by T [batch, M, r_pad] (row pitch
+ * ldt, batch pitch t_batch_stride) against Bcat [N, r_pad] (pitch ldbc); r_pad % 64 == 0, r_pad > 0. */
+int b2f_gemm_bf16_lora(const void* A, int64_t lda, int64_t a_batch_stride, const void* W, int64_t ldw,
+                       const void* bias, void* out, int64_t ldc, int64_t out_batch_stride, int batch,
+                       int M, int N, int K, int epilogue, const void* resid, int64_t ldr,
+                       int64_t resid_batch_stride, const void* gate, int64_t gate_ld, const void* T, int64_t ldt,
+                       int64_t t_batch_stride, const void* Bcat, int64_t ldbc, int r_pad, b2f_stream_t stream);
+/* b2f_gemm_qkv_norm_rope (including the n_extra second output block) with the same K-extension: the LoRA lands on the
+ * projection before RMSNorm / RoPE / GELU, where PEFT adds it. */
+int b2f_gemm_qkv_norm_rope_lora(const void* A, int64_t lda, int64_t a_batch_stride, const void* W,
+                                int64_t ldw, const void* bias, void* out, int64_t ldc,
+                                int64_t out_batch_stride, int batch, int M, int d_model, int K,
+                                const void* nw_q, const void* nw_k, const float* cos, const float* sin,
+                                int rope_row0, float eps, int n_extra, void* out_extra, int64_t ld_extra,
+                                int64_t extra_batch_stride, int epi_extra, const void* T, int64_t ldt,
+                                int64_t t_batch_stride, const void* Bcat, int64_t ldbc, int r_pad,
+                                b2f_stream_t stream);
+/* LoRA down projection: out[batch, M, N] = bf16(fp32(A W^T)[., n] * fp32(colscale[n] * cs_mul)), W = Acat [N, K],
+ * colscale fp32 [N] (16-byte aligned).  The forward GEMM with N = r_pad and a per-column scale in its epilogue. */
+int b2f_gemm_colscale(const void* A, int64_t lda, int64_t a_batch_stride, const void* W, int64_t ldw, void* out,
+                      int64_t ldc, int64_t out_batch_stride, int batch, int M, int N, int K, const float* colscale,
+                      float cs_mul, b2f_stream_t stream);
+/* Merge in place: W[rows, cols] <- bf16(W + sum_{k<r} fp32(Bcat[:, k] * fp32(colscale[k] * cs_mul)) Acat[k, :]), one
+ * fp32 accumulation in ascending k (fmaf) and one rounding (PEFT merge / diffusers fuse_lora).  Bcat [rows, r] (pitch
+ * ldb), Acat [r, cols] (pitch lda).  Unfusing is the caller's: restore a saved copy of W. */
+int b2f_lora_fuse(void* W, int64_t ldw, int rows, int cols, const void* Bcat, int64_t ldb, const void* Acat,
+                  int64_t lda, const float* colscale, float cs_mul, int r, b2f_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * AdaLN modulate (HBM-bound): out = LayerNorm(x; eps, no affine) * (1 + scale[b]) + shift[b].
@@ -257,6 +301,26 @@ int b2f_flux_temb(b2f_flux* ctx, const float* timestep, const float* guidance, c
  * pooled), so the 6.46 GB of AdaLN weights are read once per image instead of once per step. */
 int b2f_flux_modulation(b2f_flux* ctx, const void* silu_temb, int rows, void* mod,
                         b2f_stream_t stream);
+/* Unfused LoRA adapters (diffusers load_lora_weights / set_adapters, see b2f_gemm_bf16_lora): bind (Acat, Bcat, colscale)
+ * of r_pad ranks (multiple of 64; borrowed device pointers) to one linear; Acat == NULL unbinds it.  Targets: every
+ * linear bound by b2f_flux_bind_weight under its bound name (transformer_blocks.{i}.attn.qkv / attn.add_qkv,
+ * single_transformer_blocks.{i}.qkv_mlp, attn.to_out.0, ff.net.2, x_embedder, time_text_embed.*.linear_{1,2},
+ * proj_out, ...), and each AdaLN linear under its diffusers name (transformer_blocks.{i}.norm1.linear,
+ * norm1_context.linear, single_transformer_blocks.{i}.norm.linear, norm_out.linear): those act on their rows of the
+ * fused adaln weight only, through their own K-extended launch in b2f_flux_modulation_ws.  Bindings are dropped by
+ * b2f_flux_finalize.  With any adapter bound b2f_flux_workspace_bytes / b2f_flux_temb_workspace_bytes add room for
+ * T ([rows, largest r_pad]); without one they are unchanged.  The training step refuses while adapters are bound. */
+int b2f_flux_bind_lora(b2f_flux* ctx, const char* target, const void* Acat, const void* Bcat, const float* colscale,
+                       int r_pad);
+int b2f_flux_clear_lora(b2f_flux* ctx);
+/* Call scale s multiplying every colscale (joint_attention_kwargs["scale"]); read when a forward is enqueued. */
+int b2f_flux_set_lora_scale(b2f_flux* ctx, float scale);
+/* Largest bound r_pad (0: no adapter bound). */
+int b2f_flux_lora_rank(const b2f_flux* ctx);
+/* b2f_flux_modulation with the AdaLN adapters applied (b2f_flux_modulation itself refuses while one is bound). */
+size_t b2f_flux_modulation_workspace_bytes(const b2f_flux* ctx, int rows);
+int b2f_flux_modulation_ws(b2f_flux* ctx, const void* silu_temb, int rows, void* mod, void* ws, size_t ws_bytes,
+                           b2f_stream_t stream);
 /* One MMDiT forward.  hidden [B,S_img,in_channels], enc [B,S_txt,joint_dim], mod: pointer to the
  * first batch item's modulation row (pitch mod_ld between batch items), out
  * [B,n_out_rows,out_channels] (the first n_out_rows image tokens; the pipeline only consumes the

@@ -9,6 +9,9 @@ WANT = [
     # the persistent GEMM reusing its ring and staging tiles across tiles of one CTA (SMs + 1 tiles)
     ("tests/test_gemm_persistent_gpu.py", ["test_gemm_toy_tile_counts[1]", "test_gemm_toy_tile_counts[3]",
                                            "test_gemm_toy_tile_counts[sms+1]"]),
+    # the LoRA K-extended GEMM (extra k-blocks of T / Bcat through the same ring), its down projection and the merge
+    ("tests/test_lora_gpu.py", ["test_lora_gemm_ranks_and_shapes[True-0]", "test_lora_gemm_ranks_and_shapes[False-4]",
+                                "test_lora_gemm_qkv_norm_rope[True]", "test_lora_fuse_kernel"]),
     ("tests/test_train_kernels_gpu.py", ["test_gemm_dgrad[1-128-128-64]", "test_gemm_dgrad[1-200-136-72]", "test_gemm_dgrad[2-300-256-512]",
                                          "test_gemm_dgrad[2-1024-1024-4096]", "test_gemm_dgrad_pitched_views_and_epilogues",
                                          "test_gemm_wgrad[1-64-128-128]", "test_gemm_wgrad[1-100-136-200]", "test_gemm_wgrad[3-150-256-384]",
