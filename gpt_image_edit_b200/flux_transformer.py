@@ -319,3 +319,15 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         off = (-ws.data_ptr()) % 256
         n = B * (S_img + S_txt) * self.inner_dim
         return ws[off:off + 2 * n].view(torch.bfloat16).view(B, S_img + S_txt, self.inner_dim)
+
+    def debug_buffers(self, B: int, S_img: int, S_txt: int) -> SimpleNamespace:
+        """Views of the whole forward workspace in b2f_flux_forward's layout (text rows first): h and xn [B, S, d],
+        qkv [B, S, 3d], cat [B, S, 5d].  After a partial-range forward they hold what the last block left (stage-level
+        parity tests read them); the views are only for reading."""
+        ws = self._ws["fwd"]
+        off = (-ws.data_ptr()) % 256
+        S, d = S_img + S_txt, self.inner_dim
+        n = B * S * d
+        h, xn, qkv, cat = ws[off:off + 20 * n].view(torch.bfloat16).split([n, n, 3 * n, 5 * n])
+        return SimpleNamespace(h=h.view(B, S, d), xn=xn.view(B, S, d), qkv=qkv.view(B, S, 3 * d),
+                               cat=cat.view(B, S, 5 * d))
