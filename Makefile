@@ -8,6 +8,8 @@ LIBDIR    := gpt_image_edit_b200/lib
 SRCS      := $(wildcard $(CSRC)/*.cu)
 OBJS      := $(patsubst $(CSRC)/%.cu,build/%.o,$(SRCS))
 HDRS      := $(wildcard $(CSRC)/*.cuh) $(wildcard $(CSRC)/*.h) include/b2f.h
+# only the b2f_* functions of include/b2f.h are exported
+VERSION_SCRIPT := $(CSRC)/libb2f.map
 
 all: $(LIBDIR)/libb2f.so
 
@@ -16,9 +18,10 @@ build/%.o: $(CSRC)/%.cu $(HDRS)
 	$(NVCC) $(NVFLAGS) -c $< -o $@ 2> build/$*.ptxas.log || (cat build/$*.ptxas.log; exit 1)
 	@grep -E "error|warning|spill|registers" build/$*.ptxas.log | grep -v "0 bytes spill" | head -40 || true
 
-$(LIBDIR)/libb2f.so: $(OBJS)
+$(LIBDIR)/libb2f.so: $(OBJS) $(VERSION_SCRIPT)
 	@mkdir -p $(LIBDIR)
-	$(NVCC) $(ARCH) -shared -cudart shared -o $@ $(OBJS) -Xlinker -rpath -Xlinker /usr/local/cuda/lib64
+	$(NVCC) $(ARCH) -shared -cudart shared -o $@ $(OBJS) -Xlinker -rpath -Xlinker /usr/local/cuda/lib64 \
+		-Xlinker --version-script=$(VERSION_SCRIPT)
 
 clean:
 	rm -rf build $(LIBDIR)/libb2f.so

@@ -32,7 +32,6 @@ def _load() -> C.CDLL:
 
 lib = _load()
 
-_vp, _i64, _i32 = C.c_void_p, C.c_int64, C.c_int
 
 class VaeCfg(C.Structure):
     _fields_ = [("block_out", C.c_int * 4), ("layers_per_block", C.c_int), ("latent_channels", C.c_int),
@@ -45,112 +44,55 @@ class FluxCfg(C.Structure):
         "joint_dim", "pooled_dim", "guidance_embeds", "mlp_ratio")]
 
 
-_SIGNATURES = {
-    "b2f_strerror": (C.c_char_p, [_i32]),
-    "b2f_version": (_i32, []),
-    "b2f_device_info": (_i32, [C.POINTER(_i32), C.POINTER(_i32), C.POINTER(_i32), C.POINTER(C.c_size_t)]),
-    "b2f_launch_count": (C.c_uint64, []),
-    "b2f_prof_enable": (None, [_i32]),
-    "b2f_prof_shapes": (_i32, [C.c_char_p, _i32]),
-    "b2f_prof_collect": (_i32, [_i32, C.POINTER(C.c_double), C.POINTER(_i64), C.POINTER(C.c_double), C.POINTER(C.c_double)]),
-    "b2f_gemm_bf16": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _i64, _vp, _i64, _vp]),
-    "b2f_gemm_qkv_norm_rope": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _i32, C.c_float, _i32, _vp, _i64, _i64, _i32, _vp]),
-    "b2f_ln_modulate": (_i32, [_vp, _i64, _i64, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _i32, _i32, C.c_float, _i32, _vp, _vp, _vp]),
-    "b2f_rmsnorm_rope": (_i32, [_vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, C.c_float, _vp]),
-    "b2f_euler_step": (_i32, [_vp, _i64, _vp, _i64, _i64, _i32, C.c_float, _vp]),
-    "b2f_silu": (_i32, [_vp, _vp, _i64, _vp]),
-    "b2f_temb_sinusoid": (_i32, [_vp, _vp, _i32, _vp]),
-    "b2f_temb_combine": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, _vp]),
-    "b2f_rope_tables": (_i32, [_vp, _i32, C.POINTER(_i32), C.c_double, _vp, _vp, _vp]),
-    "b2f_rmsnorm": (_i32, [_vp, _i64, _vp, _vp, _i64, _i64, _i32, C.c_float, _vp]),
-    "b2f_rope_half": (_i32, [_vp, _i64, _i32, _i32, _vp, _vp, _i32, _i64, _i32, _vp]),
-    "b2f_swiglu": (_i32, [_vp, _i64, _vp, _i64, _i64, _i32, _vp]),
-    "b2f_move_rows": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _vp]),
-    "b2f_conv3x3": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32, _i32, _vp]),
-    "b2f_groupnorm_silu": (_i32, [_vp, _vp, _vp, _vp, _vp, _i32, _i64, _i32, C.c_float, _i32, _vp]),
-    "b2f_upsample2x": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp]),
-    "b2f_nchw_to_nhwc_pad": (_i32, [_vp, _i32, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
-    "b2f_softmax_rows": (_i32, [_vp, _i64, _i32, _i32, C.c_float, _vp]),
-    "b2f_transpose_bf16": (_i32, [_vp, _i64, _vp, _i64, _i32, _i32, _vp]),
-    "b2f_vae_create": (_i32, [C.POINTER(_vp), _vp]),
-    "b2f_vae_destroy": (None, [_vp]),
-    "b2f_vae_bind_weight": (_i32, [_vp, C.c_char_p, _vp, _i64]),
-    "b2f_vae_workspace_bytes": (C.c_size_t, [_vp, _i32, _i32, _i32]),
-    "b2f_vae_encode": (_i32, [_vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, C.c_size_t, _vp]),
-    "b2f_vae_decode": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, C.c_size_t, _vp]),
-    "b2f_vae_decode_u8": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, C.c_size_t, _vp]),
-    "b2f_flux_create": (_i32, [C.POINTER(_vp), _vp]),
-    "b2f_flux_destroy": (None, [_vp]),
-    "b2f_flux_bind_weight": (_i32, [_vp, C.c_char_p, _vp, _i64]),
-    "b2f_flux_finalize": (_i32, [_vp]),
-    "b2f_flux_mod_width": (_i64, [_vp]),
-    "b2f_flux_set_rope": (_i32, [_vp, _vp, _vp, _i32]),
-    "b2f_flux_workspace_bytes": (C.c_size_t, [_vp, _i32, _i32, _i32]),
-    "b2f_flux_temb_workspace_bytes": (C.c_size_t, [_vp, _i32]),
-    "b2f_flux_temb": (_i32, [_vp, _vp, _vp, _vp, _i64, _i32, _vp, _vp, _vp, C.c_size_t, _vp]),
-    "b2f_flux_modulation": (_i32, [_vp, _vp, _i32, _vp, _vp]),
-    "b2f_flux_forward": (_i32, [_vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _vp, C.c_size_t, _i32, _i32, _vp]),
-    "b2f_attention_fwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, C.c_float, _i32, _vp]),
-    "b2f_attention_bias_fwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, C.c_float, _i32,
-                                      _vp, _i64, _i64, _vp]),
-    "b2f_geglu": (_i32, [_vp, _i64, _vp, _i64, _i64, _i32, _vp]),
-    "b2f_layernorm": (_i32, [_vp, _i64, _vp, _vp, _vp, _i64, _i64, _i32, C.c_float, _vp]),
-    "b2f_embed": (_i32, [_vp, _i64, _vp, _vp, _i64, _i32, _vp, _i64, _i64, _i32, _vp]),
-    # training step
-    "b2f_gemm_dgrad": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _i64, _vp]),
-    "b2f_gemm_wgrad": (_i32, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _vp]),
-    "b2f_attention_fwd_lse": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _i32, _i32, C.c_float, _i32,
-                                     _vp, _i64, _vp]),
-    "b2f_attn_delta": (_i32, [_vp, _i64, _vp, _i64, _vp, _vp, _i32, _i32, _i32, _i32, _vp]),
-    "b2f_attention_bwd": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _vp, _i64, _vp, _i64, _vp, _i64, _vp, _i64,
-                                 _i32, _i32, _i32, _i32, C.c_float, _vp]),
-    "b2f_train_chunks": (_i32, [_i32]),
-    "b2f_train_ln_chunks": (_i32, [_i32]),
-    "b2f_gate_resid_fwd": (_i32, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _i64, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp]),
-    "b2f_gate_bwd": (_i32, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _i64, _vp, _i64, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _vp]),
-    "b2f_col_reduce": (_i32, [_vp, _i32, _i32, _vp, _i64, _i32, _i32, _vp]),
-    "b2f_ln_modulate_bwd": (_i32, [_vp, _i64, _i64, _vp, _i64, _i64, _vp, _vp, _i64, _vp, _i64, _i64, _vp, _i64, _i64, _vp,
-                                   _i32, _i32, _i32, C.c_float, _i32, _i32, _vp]),
-    "b2f_rmsnorm_rope_out": (_i32, [_vp, _vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32,
-                                    C.c_float, _vp]),
-    "b2f_rmsnorm_rope_bwd": (_i32, [_vp, _vp, _i64, _i64, _vp, _vp, _i64, _i64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32,
-                                    _i32, C.c_float, _vp]),
-    "b2f_gelu_rows": (_i32, [_vp, _i64, _vp, _i64, _i64, _i32, _vp]),
-    "b2f_outer_acc": (_i32, [_vp, _i64, _vp, _i64, _vp, _i64, _i32, _i32, _i32, _i32, _vp]),
-    "b2f_mse_loss": (_i32, [_vp, _vp, _vp, _vp, _vp, _vp, _i64, C.c_float, _vp]),
-    "b2f_grad_sumsq": (_i32, [_vp, _i64, _vp, _vp, _i32, _vp]),
-    "b2f_clip_coef": (_i32, [_vp, C.c_float, C.c_float, _vp, _vp, _vp]),
-    "b2f_adamw_step": (_i32, [_vp, _vp, _vp, _vp, _vp, _i64, C.c_float, C.c_float, C.c_float, C.c_float, C.c_float, _i32, _vp, _vp]),
-    "b2f_cast_bf16_f32": (_i32, [_vp, _vp, _i64, _i32, _vp]),
-    "b2f_blend_bf16": (_i32, [_vp, _vp, C.c_float, C.c_float, _vp, _i64, _vp]),
-    "b2f_flux_bind_grad": (_i32, [_vp, C.c_char_p, _vp, _i64]),
-    "b2f_flux_train_workspace_bytes": (C.c_size_t, [_vp, _i32, _i32, _i32]),
-    "b2f_flux_train_forward": (_i32, [_vp, _vp, _vp, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _vp, C.c_size_t, _vp]),
-    "b2f_flux_train_backward": (_i32, [_vp, _vp, _vp, _i64, _vp, _i64, _vp, _i32, _i32, _i32, _i32, _i32, _vp, C.c_size_t,
-                                       _i32, _i32, _vp]),
-    "b2f_flux_train_debug_dh": (_i32, [_vp, _vp, _i32, _i32, _i32, _vp, _vp]),
-    # LoRA
-    "b2f_gemm_bf16_lora": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _i32, _vp, _i64, _i64,
-                                  _vp, _i64, _vp, _i64, _i64, _vp, _i64, _i32, _vp]),
-    "b2f_gemm_qkv_norm_rope_lora": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, _vp, _vp,
-                                           _vp, _i32, C.c_float, _i32, _vp, _i64, _i64, _i32, _vp, _i64, _i64, _vp, _i64, _i32,
-                                           _vp]),
-    "b2f_gemm_colscale": (_i32, [_vp, _i64, _i64, _vp, _i64, _vp, _i64, _i64, _i32, _i32, _i32, _i32, _vp, C.c_float, _vp]),
-    "b2f_lora_fuse": (_i32, [_vp, _i64, _i32, _i32, _vp, _i64, _vp, _i64, _vp, C.c_float, _i32, _vp]),
-    "b2f_flux_bind_lora": (_i32, [_vp, C.c_char_p, _vp, _vp, _vp, _i32]),
-    "b2f_flux_clear_lora": (_i32, [_vp]),
-    "b2f_flux_set_lora_scale": (_i32, [_vp, C.c_float]),
-    "b2f_flux_lora_rank": (_i32, [_vp]),
-    "b2f_flux_modulation_workspace_bytes": (C.c_size_t, [_vp, _i32]),
-    "b2f_flux_modulation_ws": (_i32, [_vp, _vp, _i32, _vp, _vp, C.c_size_t, _vp]),
-}
+# ctypes type of every scalar type include/b2f.h uses; pointers are c_void_p (c_char_p for char*), so ctypes
+# arrays and byref() out-parameters both pass.
+_SCALARS = {"int": C.c_int, "int64_t": C.c_int64, "uint64_t": C.c_uint64, "size_t": C.c_size_t,
+            "float": C.c_float, "double": C.c_double, "b2f_stream_t": C.c_void_p}
+
+
+def _header_text() -> str:
+    return re.sub(r"/\*.*?\*/", "", HEADER_PATH.read_text(), flags=re.S)
+
+
+def _ctype(decl: str, where: str):
+    """ctypes type of one declared type (`const void*`, `int64_t`, `b2f_flux**`, ...); None for void."""
+    words = decl.replace("*", " * ").split()
+    stars = words.count("*")
+    base = [w for w in words if w not in ("*", "const")]
+    if len(base) != 1:
+        raise B2FError(f"include/b2f.h: cannot bind type '{decl}' in {where}")
+    if stars:
+        return C.c_char_p if base[0] == "char" and stars == 1 else C.c_void_p
+    if base[0] == "void":
+        return None
+    if base[0] not in _SCALARS:
+        raise B2FError(f"include/b2f.h: no ctypes binding for type '{decl}' in {where}")
+    return _SCALARS[base[0]]
+
+
+def _signatures() -> dict:
+    """{name: (restype, argtypes)} of every function prototype in include/b2f.h."""
+    sigs = {}
+    for ret, name, params in re.findall(r"^\s*((?:const\s+)?\w+[\s*]*?)\s*(b2f_\w+)\s*\(([^)]*)\)\s*;",
+                                        _header_text(), flags=re.M):
+        params = params.strip()
+        args = []
+        if params not in ("", "void"):
+            for prm in params.split(","):
+                m = re.fullmatch(r"(.*?[\s*])(\w+)", prm.strip(), flags=re.S)
+                if not m:
+                    raise B2FError(f"include/b2f.h: cannot parse parameter '{prm.strip()}' of {name}")
+                args.append(_ctype(m.group(1), name))
+        sigs[name] = (_ctype(ret, name), args)
+    return sigs
+
+
+_SIGNATURES = _signatures()
 
 
 def declared_symbols() -> list[str]:
     """Every function name include/b2f.h declares (used by the CPU-side export test)."""
-    text = HEADER_PATH.read_text()
-    text = re.sub(r"/\*.*?\*/", "", text, flags=re.S)
-    return sorted(set(re.findall(r"\b(b2f_[a-z0-9_]+)\s*\(", text)))
+    return sorted(set(re.findall(r"\b(b2f_[a-z0-9_]+)\s*\(", _header_text())))
 
 
 def _bind() -> None:
@@ -189,7 +131,7 @@ def prof_collect() -> dict:
     """{class: dict(ms, launches, flops, bytes)} since the last collect (synchronises the events)."""
     out = {}
     for i, name in enumerate(KERNEL_CLASSES):
-        ms, n, fl, by = C.c_double(), _i64(), C.c_double(), C.c_double()
+        ms, n, fl, by = C.c_double(), C.c_int64(), C.c_double(), C.c_double()
         check(lib.b2f_prof_collect(i, C.byref(ms), C.byref(n), C.byref(fl), C.byref(by)), "b2f_prof_collect")
         out[name] = dict(ms=ms.value, launches=n.value, flops=fl.value, bytes=by.value)
     return out

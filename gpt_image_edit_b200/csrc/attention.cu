@@ -14,14 +14,11 @@
 // Replaces F.scaled_dot_product_attention as reached by diffusers FluxAttnProcessor2_0
 // (SURVEY.md A.2; reference call site univa/utils/flux_pipeline.py:1067) and flash_attn as reached
 // through transformers' attn_implementation="flash_attention_2" (univa/serve/cli.py:40).
-#include <atomic>
 #include <cmath>
 
 #include "attention_common.cuh"
 
 namespace b2f {
-
-extern std::atomic<uint64_t> g_launch_count;
 
 using namespace attn;
 
@@ -258,8 +255,7 @@ static int attention_impl(const void* q, int64_t ldq, const void* k, int64_t ldk
     attn_fwd_kernel<true><<<grid_b, ATTN_THREADS, ATTN_SMEM, stream>>>(tmQ, tmK, tmV, p);
     prof_end(KC_ATTN, stream, (causal ? 2.0 : 4.0) * B * H * (double)Sq * Skv * DH,
              2.0 * DH * B * (2.0 * H * Sq + 2.0 * Hkv * Skv) + 2.0 * H * (double)Sq * Skv);
-    g_launch_count.fetch_add(1, std::memory_order_relaxed);
-    B2F_CHECK_LAUNCH("attn_fwd_kernel<bias>");
+    B2F_LAUNCHED("attn_fwd_kernel<bias>", 1);
     return B2F_OK;
   }
   dim3 grid((Sq + BQ - 1) / BQ, H, B);
@@ -267,31 +263,33 @@ static int attention_impl(const void* q, int64_t ldq, const void* k, int64_t ldk
   attn_fwd_kernel<false><<<grid, ATTN_THREADS, ATTN_SMEM, stream>>>(tmQ, tmK, tmV, p);
   prof_end(KC_ATTN, stream, (causal ? 2.0 : 4.0) * B * H * (double)Sq * Skv * DH,
            2.0 * DH * B * (2.0 * H * Sq + 2.0 * Hkv * Skv));
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("attn_fwd_kernel");
+  B2F_LAUNCHED("attn_fwd_kernel", 1);
   return B2F_OK;
 }
 
-int attention_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
-                  int64_t ldv, void* out, int64_t ldo, int B, int H, int Hkv, int Sq, int Skv,
-                  int head_dim, float scale, int causal, cudaStream_t stream) {
+extern "C" int b2f_attention_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                                 void* out, int64_t ldo, int B, int H, int Hkv, int Sq, int Skv, int head_dim,
+                                 float scale, int causal, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   return attention_impl(q, ldq, k, ldk, v, ldv, out, ldo, B, H, Hkv, Sq, Skv, head_dim, scale, causal,
                         nullptr, 0, 0, nullptr, 0, stream);
 }
 
 // forward that also emits the base-2 log-sum-exp rows the backward kernels need (attention_bwd.cu)
-int attention_fwd_lse(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out,
-                      int64_t ldo, int B, int H, int Hkv, int Sq, int Skv, int head_dim, float scale, int causal,
-                      float* lse, int64_t lse_stride, cudaStream_t stream) {
+extern "C" int b2f_attention_fwd_lse(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                                     void* out, int64_t ldo, int B, int H, int Hkv, int Sq, int Skv, int head_dim,
+                                     float scale, int causal, float* lse, int64_t lse_stride, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!lse) return B2F_ERR_INVALID;
   return attention_impl(q, ldq, k, ldk, v, ldv, out, ldo, B, H, Hkv, Sq, Skv, head_dim, scale, causal, nullptr, 0, 0,
                         lse, lse_stride, stream);
 }
 
-int attention_bias_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
-                       int64_t ldv, void* out, int64_t ldo, int B, int H, int Hkv, int Sq, int Skv,
-                       int head_dim, float scale, int causal, const void* bias, int64_t bias_h_stride,
-                       int64_t bias_row_stride, cudaStream_t stream) {
+extern "C" int b2f_attention_bias_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                                      int64_t ldv, void* out, int64_t ldo, int B, int H, int Hkv, int Sq, int Skv,
+                                      int head_dim, float scale, int causal, const void* bias, int64_t bias_h_stride,
+                                      int64_t bias_row_stride, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!bias || bias_row_stride < Skv || bias_h_stride < 0) return B2F_ERR_INVALID;
   return attention_impl(q, ldq, k, ldk, v, ldv, out, ldo, B, H, Hkv, Sq, Skv, head_dim, scale, causal,
                         bias, bias_h_stride, bias_row_stride, nullptr, 0, stream);

@@ -21,14 +21,11 @@
 //
 // Replaces the autograd of F.scaled_dot_product_attention / flash_attn backward reached by
 // accelerator.backward(loss) in the reference (train_denoiser.py:1172) for every FLUX block.
-#include <atomic>
 #include <cmath>
 
 #include "attention_common.cuh"
 
 namespace b2f {
-
-extern std::atomic<uint64_t> g_launch_count;
 
 using namespace attn;
 
@@ -236,10 +233,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_constant_
 
 // q/k/v/dout: token-major [B, S, H*128] views (pitches ld*); lse, delta: fp32 [B, H, S_pad] with S_pad a multiple of
 // 128, lse = +inf and delta = 0 in the padding (attn_delta writes both); dq/dk/dv: [B, S, H*128] views.
-int attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* dout,
-                  int64_t lddo, const float* lse, const float* delta, int64_t S_pad, void* dq, int64_t lddq, void* dk,
-                  int64_t lddk, void* dv, int64_t lddv, int B, int H, int S, int head_dim, float scale,
-                  cudaStream_t stream) {
+extern "C" int b2f_attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                                 const void* dout, int64_t lddo, const float* lse, const float* delta, int64_t S_pad,
+                                 void* dq, int64_t lddq, void* dk, int64_t lddk, void* dv, int64_t lddv, int B, int H,
+                                 int S, int head_dim, float scale, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!q || !k || !v || !dout || !lse || !delta || !dq || !dk || !dv || B <= 0 || H <= 0 || S <= 0) return B2F_ERR_INVALID;
   if (head_dim != DH) return B2F_ERR_UNSUPPORTED;
@@ -287,16 +285,14 @@ int attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const 
   prof_begin(KC_ATTN, stream);
   attn_bwd_kernel<0><<<grid, BWD_THREADS, BWD_SMEM, stream>>>(tK, tV, sQ, sO, p);
   prof_end(KC_ATTN, stream, 4.0 * unit, 2.0 * DH * B * H * 6.0 * S);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("attn_bwd_kernel<dKdV>");
+  B2F_LAUNCHED("attn_bwd_kernel<dKdV>", 1);
   p.g0 = static_cast<__nv_bfloat16*>(dq);
   p.ld0 = lddq;
   p.g1 = nullptr;
   prof_begin(KC_ATTN, stream);
   attn_bwd_kernel<1><<<grid, BWD_THREADS, BWD_SMEM, stream>>>(tQ, tO, sK, sV, p);
   prof_end(KC_ATTN, stream, 3.0 * unit, 2.0 * DH * B * H * 5.0 * S);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("attn_bwd_kernel<dQ>");
+  B2F_LAUNCHED("attn_bwd_kernel<dQ>", 1);
   return B2F_OK;
 }
 

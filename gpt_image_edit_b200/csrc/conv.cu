@@ -14,13 +14,9 @@
 // Replaces cuDNN conv as reached by diffusers AutoencoderKL (ResnetBlock2D conv1/conv2, Downsample2D,
 // Upsample2D conv, conv_in/conv_out; SURVEY.md A.4; reference call sites
 // univa/utils/flux_pipeline.py:600-613, 1127-1129).
-#include <atomic>
-
 #include "gemm_sm90.cuh"
 
 namespace b2f {
-
-extern std::atomic<uint64_t> g_launch_count;
 
 namespace {
 
@@ -179,15 +175,15 @@ int launch_conv(const CUtensorMap& tmIn, const CUtensorMap& tmW, ConvParams p, c
   const double pix = (double)p.N * p.Ho * p.Wo;
   prof_end(KC_CONV, stream, 2.0 * pix * 9.0 * p.Cin * p.Cout,
            2.0 * (pix * p.stride * p.stride * p.Cin + pix * p.Cout + 9.0 * p.Cin * p.Cout));
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("conv3x3_kernel");
+  B2F_LAUNCHED("conv3x3_kernel", 1);
   return B2F_OK;
 }
 
 }  // namespace
 
-int conv3x3(const void* in, const void* w, const void* bias, void* out, const void* resid, int N,
-            int Hin, int Win, int Cin, int Cout, int stride, int out_nchw, cudaStream_t stream) {
+extern "C" int b2f_conv3x3(const void* in, const void* w, const void* bias, void* out, const void* resid, int N,
+                           int Hin, int Win, int Cin, int Cout, int stride, int out_nchw, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!in || !w || !out || N <= 0 || Hin <= 0 || Win <= 0) return B2F_ERR_INVALID;
   if (Cin % 64 || Cout <= 0 || (stride != 1 && stride != 2)) return B2F_ERR_UNSUPPORTED;

@@ -1,14 +1,10 @@
 // HBM-bound fused row kernels of the MMDiT block (SURVEY.md §2b "ATen elementwise / norm kernels").
 // Each replaces a chain of separate torch-eager kernels in diffusers; every intermediate that torch
 // would have rounded to bf16 is rounded here too, so results track the reference's rounding chain.
-#include <atomic>
-
 #include "host_common.h"
 #include "ptx.cuh"
 
 namespace b2f {
-
-extern std::atomic<uint64_t> g_launch_count;
 
 namespace {
 
@@ -307,30 +303,31 @@ __global__ void __launch_bounds__(64) rope_tables_kernel(const RopeTabParams p) 
 
 }  // namespace
 
-int rope_tables(const float* ids, int S, const int* axes_dim, double theta, float* cos, float* sin,
-                cudaStream_t stream) {
+extern "C" int b2f_rope_tables(const float* ids, int S, const int* axes_dim, double theta, float* cos, float* sin,
+                               b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!ids || !cos || !sin || !axes_dim || S <= 0) return B2F_ERR_INVALID;
   if (axes_dim[0] + axes_dim[1] + axes_dim[2] != 128 || (axes_dim[0] | axes_dim[1] | axes_dim[2]) & 1)
     return B2F_ERR_UNSUPPORTED;
   RopeTabParams p{ids, cos, sin, S, {axes_dim[0], axes_dim[1], axes_dim[2]}, theta};
   rope_tables_kernel<<<S, 64, 0, stream>>>(p);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("rope_tables_kernel");
+  B2F_LAUNCHED("rope_tables_kernel", 1);
   return B2F_OK;
 }
 
-int temb_sinusoid(const float* t, void* out, int rows, cudaStream_t stream) {
+extern "C" int b2f_temb_sinusoid(const float* t, void* out, int rows, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!t || !out || rows <= 0) return B2F_ERR_INVALID;
   temb_sinusoid_kernel<<<rows, 128, 0, stream>>>(t, static_cast<__nv_bfloat16*>(out), rows);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("temb_sinusoid_kernel");
+  B2F_LAUNCHED("temb_sinusoid_kernel", 1);
   return B2F_OK;
 }
 
-int temb_combine(const void* t, const void* g, const void* txt, void* temb, void* silu_temb,
-                 int64_t n, cudaStream_t stream) {
+extern "C" int b2f_temb_combine(const void* t, const void* g, const void* txt, void* temb, void* silu_temb, int64_t n,
+                                b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!t || !txt || !temb || !silu_temb || n <= 0 || (n & 7)) return B2F_ERR_INVALID;
   const long long n8 = n >> 3;
@@ -338,15 +335,15 @@ int temb_combine(const void* t, const void* g, const void* txt, void* temb, void
       static_cast<const __nv_bfloat16*>(t), static_cast<const __nv_bfloat16*>(g),
       static_cast<const __nv_bfloat16*>(txt), static_cast<__nv_bfloat16*>(temb),
       static_cast<__nv_bfloat16*>(silu_temb), n8);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("temb_combine_kernel");
+  B2F_LAUNCHED("temb_combine_kernel", 1);
   return B2F_OK;
 }
 
-int ln_modulate(const void* x, int64_t ldx, int64_t x_batch_stride, const void* scale,
-                const void* shift, int64_t mod_ld, void* out, int64_t ldo, int64_t out_batch_stride,
-                int batch, int rows, int D, float eps, int split_row, const void* scale_b,
-                const void* shift_b, cudaStream_t stream) {
+extern "C" int b2f_ln_modulate(const void* x, int64_t ldx, int64_t x_batch_stride, const void* scale, const void* shift,
+                               int64_t mod_ld, void* out, int64_t ldo, int64_t out_batch_stride, int batch, int rows,
+                               int D, float eps, int split_row, const void* scale_b, const void* shift_b,
+                               b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!x || !scale || !shift || !out || batch <= 0 || rows <= 0) return B2F_ERR_INVALID;
   if (D <= 0 || (D & 255) || D > 256 * LN_MAXC) return B2F_ERR_UNSUPPORTED;
@@ -373,15 +370,14 @@ int ln_modulate(const void* x, int64_t ldx, int64_t x_batch_stride, const void* 
     ln_modulate_kernel<12><<<grid, 128, 0, stream>>>(p);
   else
     ln_modulate_kernel<LN_MAXC><<<grid, 128, 0, stream>>>(p);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("ln_modulate_kernel");
+  B2F_LAUNCHED("ln_modulate_kernel", 1);
   return B2F_OK;
 }
 
-int rmsnorm_rope(void* q, void* k, int64_t ld, int64_t batch_stride, const void* wq_a,
-                 const void* wk_a, const void* wq_b, const void* wk_b, const float* cos,
-                 const float* sin, int batch, int S, int H, int head_dim, int n_a, float eps,
-                 cudaStream_t stream) {
+extern "C" int b2f_rmsnorm_rope(void* q, void* k, int64_t ld, int64_t batch_stride, const void* wq_a, const void* wk_a,
+                                const void* wq_b, const void* wk_b, const float* cos, const float* sin, int batch,
+                                int S, int H, int head_dim, int n_a, float eps, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!q || !k || !wq_b || !wk_b || !cos || !sin || batch <= 0 || S <= 0 || H <= 0)
     return B2F_ERR_INVALID;
@@ -396,13 +392,13 @@ int rmsnorm_rope(void* q, void* k, int64_t ld, int64_t batch_stride, const void*
   prof_begin(KC_NORMROPE, stream);
   rmsnorm_rope_kernel<<<(unsigned)((total + 7) / 8), 256, 0, stream>>>(p);
   prof_end(KC_NORMROPE, stream, 0.0, 8.0 * (double)total * H * 128);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("rmsnorm_rope_kernel");
+  B2F_LAUNCHED("rmsnorm_rope_kernel", 1);
   return B2F_OK;
 }
 
-int euler_step(void* x, int64_t ldx, const void* v, int64_t ldv, int64_t rows, int cols, float dt,
-               cudaStream_t stream) {
+extern "C" int b2f_euler_step(void* x, int64_t ldx, const void* v, int64_t ldv, int64_t rows, int cols, float dt,
+                              b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!x || !v || rows <= 0 || cols <= 0) return B2F_ERR_INVALID;
   if ((cols & 7) || (ldx & 7) || (ldv & 7)) return B2F_ERR_ALIGN;
@@ -410,19 +406,18 @@ int euler_step(void* x, int64_t ldx, const void* v, int64_t ldv, int64_t rows, i
                 cols, dt};
   const long long n = rows * (cols >> 3);
   euler_step_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(p);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("euler_step_kernel");
+  B2F_LAUNCHED("euler_step_kernel", 1);
   return B2F_OK;
 }
 
-int silu(const void* x, void* y, int64_t n, cudaStream_t stream) {
+extern "C" int b2f_silu(const void* x, void* y, int64_t n, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!x || !y || n <= 0 || (n & 7)) return B2F_ERR_INVALID;
   const long long n8 = n >> 3;
   silu_kernel<<<(unsigned)((n8 + 255) / 256), 256, 0, stream>>>(
       static_cast<const __nv_bfloat16*>(x), static_cast<__nv_bfloat16*>(y), n8);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("silu_kernel");
+  B2F_LAUNCHED("silu_kernel", 1);
   return B2F_OK;
 }
 

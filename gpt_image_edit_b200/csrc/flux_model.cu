@@ -23,43 +23,6 @@
 
 namespace b2f {
 
-int gemm_bf16(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
-              const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N,
-              int K, int epilogue, const void* resid, int64_t ldr, int64_t resid_bs, const void* gate,
-              int64_t gate_ld, cudaStream_t stream);
-int gemm_qkv_norm_rope(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
-                       const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M,
-                       int d_model, int K, const void* nw_q, const void* nw_k, const float* cos,
-                       const float* sin, int rope_row0, float eps, int n_extra, void* out_extra,
-                       int64_t ld_extra, int64_t bs_extra, int epi_extra, cudaStream_t stream);
-int attention_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
-                  int64_t ldv, void* out, int64_t ldo, int B, int H, int Hkv, int Sq, int Skv,
-                  int head_dim, float scale, int causal, cudaStream_t stream);
-int ln_modulate(const void* x, int64_t ldx, int64_t x_batch_stride, const void* scale,
-                const void* shift, int64_t mod_ld, void* out, int64_t ldo, int64_t out_batch_stride,
-                int batch, int rows, int D, float eps, int split_row, const void* scale_b,
-                const void* shift_b, cudaStream_t stream);
-int rmsnorm_rope(void* q, void* k, int64_t ld, int64_t batch_stride, const void* wq_a,
-                 const void* wk_a, const void* wq_b, const void* wk_b, const float* cos,
-                 const float* sin, int batch, int S, int H, int head_dim, int n_a, float eps,
-                 cudaStream_t stream);
-int gemm_bf16_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias, void* out,
-                   int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epilogue, const void* resid,
-                   int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld, const void* T, int64_t ldt,
-                   int64_t t_bs, const void* Bc, int64_t ldbc, int r_pad, cudaStream_t stream);
-int gemm_qkv_norm_rope_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias,
-                            void* out, int64_t ldc, int64_t out_bs, int batch, int M, int d_model, int K,
-                            const void* nw_q, const void* nw_k, const float* cos, const float* sin, int rope_row0,
-                            float eps, int n_extra, void* out_extra, int64_t ld_extra, int64_t bs_extra,
-                            int epi_extra, const void* T, int64_t ldt, int64_t t_bs, const void* Bc, int64_t ldbc,
-                            int r_pad, cudaStream_t stream);
-int gemm_colscale(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, void* out, int64_t ldc,
-                  int64_t out_bs, int batch, int M, int N, int K, const float* colscale, float cs_mul,
-                  cudaStream_t stream);
-int temb_sinusoid(const float* t, void* out, int rows, cudaStream_t stream);
-int temb_combine(const void* t, const void* g, const void* txt, void* temb, void* silu_temb,
-                 int64_t n, cudaStream_t stream);
-
 static int64_t mod_width_of(const b2f_flux_cfg& c) {
   const int64_t d = (int64_t)c.num_heads * c.head_dim;
   return (int64_t)c.num_double * 12 * d + (int64_t)c.num_single * 3 * d + 2 * d;
@@ -140,29 +103,29 @@ static int lin_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_
                    void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epi, const void* resid,
                    int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld, cudaStream_t st) {
   if (!l.lora.A)
-    return gemm_bf16(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, N, K, epi, resid, ldr, resid_bs, gate,
-                     gate_ld, st);
+    return b2f_gemm_bf16(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, N, K, epi, resid, ldr, resid_bs, gate,
+                         gate_ld, st);
   const int r = l.lora.r_pad;
   const int64_t t_bs = (int64_t)M * r;
-  int rc = gemm_colscale(A, lda, a_bs, l.lora.A, K, tb, r, t_bs, batch, M, r, K, l.lora.cs, cs_mul, st);
+  int rc = b2f_gemm_colscale(A, lda, a_bs, l.lora.A, K, tb, r, t_bs, batch, M, r, K, l.lora.cs, cs_mul, st);
   if (rc) return rc;
-  return gemm_bf16_lora(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, N, K, epi, resid, ldr, resid_bs,
-                        gate, gate_ld, tb, r, t_bs, l.lora.Bc, r, r, st);
+  return b2f_gemm_bf16_lora(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, N, K, epi, resid, ldr, resid_bs,
+                            gate, gate_ld, tb, r, t_bs, l.lora.Bc, r, r, st);
 }
 static int qkv_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_t lda, int64_t a_bs, int64_t ldw,
                    void* out, int64_t ldc, int64_t out_bs, int batch, int M, int d_model, int K, const void* nw_q,
                    const void* nw_k, const float* cos, const float* sin, int rope_row0, float eps, int n_extra,
                    void* out_extra, int64_t ld_extra, int64_t bs_extra, int epi_extra, cudaStream_t st) {
   if (!l.lora.A)
-    return gemm_qkv_norm_rope(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, d_model, K, nw_q, nw_k, cos,
-                              sin, rope_row0, eps, n_extra, out_extra, ld_extra, bs_extra, epi_extra, st);
+    return b2f_gemm_qkv_norm_rope(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, d_model, K, nw_q, nw_k, cos,
+                                  sin, rope_row0, eps, n_extra, out_extra, ld_extra, bs_extra, epi_extra, st);
   const int r = l.lora.r_pad;
   const int64_t t_bs = (int64_t)M * r;
-  int rc = gemm_colscale(A, lda, a_bs, l.lora.A, K, tb, r, t_bs, batch, M, r, K, l.lora.cs, cs_mul, st);
+  int rc = b2f_gemm_colscale(A, lda, a_bs, l.lora.A, K, tb, r, t_bs, batch, M, r, K, l.lora.cs, cs_mul, st);
   if (rc) return rc;
-  return gemm_qkv_norm_rope_lora(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, d_model, K, nw_q, nw_k, cos,
-                                 sin, rope_row0, eps, n_extra, out_extra, ld_extra, bs_extra, epi_extra, tb, r, t_bs,
-                                 l.lora.Bc, r, r, st);
+  return b2f_gemm_qkv_norm_rope_lora(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, d_model, K, nw_q, nw_k, cos,
+                                     sin, rope_row0, eps, n_extra, out_extra, ld_extra, bs_extra, epi_extra, tb, r, t_bs,
+                                     l.lora.Bc, r, r, st);
 }
 
 int FluxCtx::lora_rmax() const {
@@ -320,7 +283,7 @@ int b2f_flux_temb(b2f_flux* h, const float* timestep, const float* guidance, con
   bf16_t* tb = ep + (size_t)rows * d;   // LoRA T
   const float ls = c->lora_scale;
   int rc;
-  if ((rc = temb_sinusoid(timestep, sin_t, rows, st))) return rc;
+  if ((rc = b2f_temb_sinusoid(timestep, sin_t, rows, st))) return rc;
   if ((rc = lin_fwd(c->t1, tb, ls, sin_t, 256, 0, 256, a1, d, 0, 1, rows, d, 256, B2F_EPI_SILU,
                       nullptr, 0, 0, nullptr, 0, st)))
     return rc;
@@ -329,7 +292,7 @@ int b2f_flux_temb(b2f_flux* h, const float* timestep, const float* guidance, con
     return rc;
   const bf16_t* eg_ptr = nullptr;
   if (c->cfg.guidance_embeds) {
-    if ((rc = temb_sinusoid(guidance, sin_g, rows, st))) return rc;
+    if ((rc = b2f_temb_sinusoid(guidance, sin_g, rows, st))) return rc;
     if ((rc = lin_fwd(c->g1, tb, ls, sin_g, 256, 0, 256, a1, d, 0, 1, rows, d, 256,
                         B2F_EPI_SILU, nullptr, 0, 0, nullptr, 0, st)))
       return rc;
@@ -344,7 +307,7 @@ int b2f_flux_temb(b2f_flux* h, const float* timestep, const float* guidance, con
   if ((rc = lin_fwd(c->p2, tb, ls, a1, d, 0, d, ep, d, 0, 1, rows, d, d, B2F_EPI_BIAS, nullptr,
                       0, 0, nullptr, 0, st)))
     return rc;
-  return temb_combine(et, eg_ptr, ep, temb, silu_temb, (int64_t)rows * d, st);
+  return b2f_temb_combine(et, eg_ptr, ep, temb, silu_temb, (int64_t)rows * d, st);
 }
 
 int b2f_flux_modulation(b2f_flux* h, const void* silu_temb, int rows, void* mod, b2f_stream_t stream_) {
@@ -354,9 +317,9 @@ int b2f_flux_modulation(b2f_flux* h, const void* silu_temb, int rows, void* mod,
     fprintf(stderr, "[b2f] flux_modulation: AdaLN LoRA adapters are bound; use b2f_flux_modulation_ws\n");
     return B2F_ERR_WORKSPACE;
   }
-  return gemm_bf16(silu_temb, c->d, 0, c->adaln.w, c->d, c->adaln.b, mod, c->mod_width, 0, 1, rows,
-                   (int)c->mod_width, c->d, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0,
-                   static_cast<cudaStream_t>(stream_));
+  return b2f_gemm_bf16(silu_temb, c->d, 0, c->adaln.w, c->d, c->adaln.b, mod, c->mod_width, 0, 1, rows,
+                       (int)c->mod_width, c->d, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0,
+                       static_cast<cudaStream_t>(stream_));
 }
 
 size_t b2f_flux_modulation_workspace_bytes(const b2f_flux* h, int rows) {
@@ -372,8 +335,8 @@ int b2f_flux_modulation_ws(b2f_flux* h, const void* silu_temb, int rows, void* m
   if (ws_bytes < b2f_flux_modulation_workspace_bytes(h, rows)) return B2F_ERR_WORKSPACE;
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   const int64_t d = c->d;
-  int rc = gemm_bf16(silu_temb, d, 0, c->adaln.w, d, c->adaln.b, mod, c->mod_width, 0, 1, rows, (int)c->mod_width,
-                     (int)d, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st);
+  int rc = b2f_gemm_bf16(silu_temb, d, 0, c->adaln.w, d, c->adaln.b, mod, c->mod_width, 0, 1, rows, (int)c->mod_width,
+                         (int)d, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st);
   if (rc) return rc;
   // each AdaLN linear with an adapter: its own K-extended launch over its rows of adaln, overwriting its columns of mod
   bf16_t* tb = reinterpret_cast<bf16_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255));
@@ -517,7 +480,7 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
       const bf16_t* mi = modp + (int64_t)blk * 12 * d;
       const bf16_t* mt = mi + 6 * d;
       // both streams in one launch over the joint buffer: text rows use the context modulation
-      RUN(ln_modulate(hb, d, h_bs, mt + d, mt, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt, mi + d, mi, st));
+      RUN(b2f_ln_modulate(hb, d, h_bs, mt + d, mt, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt, mi + d, mi, st));
       // QKV projections with per-head RMSNorm + RoPE fused into the GEMM epilogue; both streams write
       // straight into the joint [txt; img] qkv buffer
       RUN(qkv_fwd(w.qkv, tb, ls, xn_img, d, h_bs, d, qkv_img, 3 * d, qkv_bs, B, S_img, (int)d,
@@ -525,14 +488,14 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
       RUN(qkv_fwd(w.add_qkv, tb, ls, xn_txt, d, h_bs, d, qkv_txt, 3 * d, qkv_bs, B, S_txt,
                              (int)d, (int)d, w.norm_added_q, w.norm_added_k, c->rope_cos, c->rope_sin, 0, eps, 0,
                              nullptr, 0, 0, 0, st));
-      RUN(attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S,
-                        g.head_dim, scale, 0, st));
+      RUN(b2f_attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S,
+                            g.head_dim, scale, 0, st));
       RUN(lin_fwd(w.to_out, tb, ls, cat_img, 5 * d, cat_bs, d, h_img, d, h_bs, B, S_img,
                     (int)d, (int)d, B2F_EPI_GATE_RESID, h_img, d, h_bs, mi + 2 * d, mod_ld, st));
       RUN(lin_fwd(w.to_add_out, tb, ls, cat_txt, 5 * d, cat_bs, d, h_txt, d, h_bs, B,
                     S_txt, (int)d, (int)d, B2F_EPI_GATE_RESID, h_txt, d, h_bs, mt + 2 * d, mod_ld, st));
-      RUN(ln_modulate(hb, d, h_bs, mt + 4 * d, mt + 3 * d, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt,
-                      mi + 4 * d, mi + 3 * d, st));
+      RUN(b2f_ln_modulate(hb, d, h_bs, mt + 4 * d, mt + 3 * d, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt,
+                          mi + 4 * d, mi + 3 * d, st));
       RUN(lin_fwd(w.ff1, tb, ls, xn_img, d, h_bs, d, cat_img + d, 5 * d, cat_bs, B, S_img,
                     (int)(4 * d), (int)d, B2F_EPI_GELU_TANH, nullptr, 0, 0, nullptr, 0, st));
       RUN(lin_fwd(w.ffc1, tb, ls, xn_txt, d, h_bs, d, cat_txt + d, 5 * d, cat_bs, B, S_txt,
@@ -546,14 +509,14 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
       const SingleW& w = c->sgl[si];
       // mod columns: [shift, scale, gate]
       const bf16_t* ms = modp + (int64_t)g.num_double * 12 * d + (int64_t)si * 3 * d;
-      RUN(ln_modulate(hb, d, h_bs, ms + d, ms, mod_ld, xn, d, h_bs, B, S, (int)d, eps, 0, nullptr, nullptr, st));
+      RUN(b2f_ln_modulate(hb, d, h_bs, ms + d, ms, mod_ld, xn, d, h_bs, B, S, (int)d, eps, 0, nullptr, nullptr, st));
       // ONE launch for [to_q;to_k;to_v;proj_mlp] (N = 7d): Q/K get RMSNorm+RoPE, V passes through into
       // qkv, the MLP columns are GELU'd straight into cat[:, :, d:5d]
       RUN(qkv_fwd(w.qkv_mlp, tb, ls, xn, d, h_bs, d, qkv, 3 * d, qkv_bs, B, S, (int)d, (int)d,
                              w.norm_q, w.norm_k, c->rope_cos, c->rope_sin, 0, eps, (int)(4 * d), cat + d, 5 * d,
                              cat_bs, B2F_EPI_GELU_TANH, st));
-      RUN(attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S,
-                        g.head_dim, scale, 0, st));
+      RUN(b2f_attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S,
+                            g.head_dim, scale, 0, st));
       RUN(lin_fwd(w.proj_out, tb, ls, cat, 5 * d, cat_bs, 5 * d, hb, d, h_bs, B, S, (int)d,
                     (int)(5 * d), B2F_EPI_GATE_RESID, hb, d, h_bs, ms + 2 * d, mod_ld, st));
     }
@@ -562,8 +525,8 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
   if (last_block == total_blocks) {
     // norm_out (AdaLayerNormContinuous: chunk order scale, shift) + proj_out on the image rows
     const bf16_t* mo = modp + (int64_t)g.num_double * 12 * d + (int64_t)g.num_single * 3 * d;
-    RUN(ln_modulate(h_img, d, h_bs, mo, mo + d, mod_ld, xn_img, d, h_bs, B, n_out_rows, (int)d, eps, 0, nullptr,
-                    nullptr, st));
+    RUN(b2f_ln_modulate(h_img, d, h_bs, mo, mo + d, mod_ld, xn_img, d, h_bs, B, n_out_rows, (int)d, eps, 0, nullptr,
+                        nullptr, st));
     RUN(lin_fwd(c->proj_out, tb, ls, xn_img, d, h_bs, d, out, g.out_channels,
                   (int64_t)n_out_rows * g.out_channels, B, n_out_rows, g.out_channels, (int)d,
                   B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));

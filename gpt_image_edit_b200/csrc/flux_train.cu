@@ -23,50 +23,6 @@
 
 namespace b2f {
 
-int gemm_bf16(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias, void* out,
-              int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epilogue, const void* resid, int64_t ldr,
-              int64_t resid_bs, const void* gate, int64_t gate_ld, cudaStream_t stream);
-int gemm_dgrad(const void* dY, int64_t ldy, int64_t dy_bs, const void* W, int64_t ldw, void* dX, int64_t ldx,
-               int64_t dx_bs, int batch, int M, int N, int K, int epilogue, const void* aux, int64_t ld_aux,
-               int64_t aux_bs, cudaStream_t stream);
-int gemm_wgrad(const void* dY, int64_t ldy, int64_t dy_bs, const void* X, int64_t ldx, int64_t x_bs, float* dW,
-               int64_t ldw, int batch, int rows, int M, int N, int accumulate, cudaStream_t stream);
-int attention_fwd_lse(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* out,
-                      int64_t ldo, int B, int H, int Hkv, int Sq, int Skv, int head_dim, float scale, int causal,
-                      float* lse, int64_t lse_stride, cudaStream_t stream);
-int attention_bwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, const void* dout,
-                  int64_t lddo, const float* lse, const float* delta, int64_t S_pad, void* dq, int64_t lddq, void* dk,
-                  int64_t lddk, void* dv, int64_t lddv, int B, int H, int S, int head_dim, float scale,
-                  cudaStream_t stream);
-int ln_modulate(const void* x, int64_t ldx, int64_t x_batch_stride, const void* scale, const void* shift,
-                int64_t mod_ld, void* out, int64_t ldo, int64_t out_batch_stride, int batch, int rows, int D, float eps,
-                int split_row, const void* scale_b, const void* shift_b, cudaStream_t stream);
-int train_chunks(int rows);
-int train_ln_chunks(int rows);
-int gate_resid_fwd(const void* x, int64_t ldx, int64_t x_bs, const void* y, int64_t ldy, int64_t y_bs, const void* gate,
-                   const void* gate_b, int64_t gate_ld, void* out, int64_t ldo, int64_t o_bs, int batch, int rows, int D,
-                   int split_row, cudaStream_t st);
-int gate_bwd(const void* dout, int64_t ldd, int64_t d_bs, const void* y, int64_t ldy, int64_t y_bs, const void* gate,
-             const void* gate_b, int64_t gate_ld, void* dy, int64_t ldo, int64_t o_bs, float* partial, int batch,
-             int rows, int D, int split_row, int part_row0, cudaStream_t st);
-int col_reduce(const float* partial, int nchunks, int D, float* out, int64_t out_ld, int batch, int accumulate,
-               cudaStream_t st);
-int ln_modulate_bwd(const void* x, int64_t ldx, int64_t x_bs, const void* dy, int64_t ldy, int64_t dy_bs,
-                    const void* scale, const void* scale_b, int64_t mod_ld, const void* dres_in, int64_t ldr, int64_t r_bs,
-                    void* dres_out, int64_t ldo, int64_t o_bs, float* partial, int batch, int rows, int D, float eps,
-                    int split_row, int part_row0, cudaStream_t st);
-int rmsnorm_rope_out(const void* xq, const void* xk, int64_t ldx, int64_t x_bs, void* oq, void* ok, int64_t ldo,
-                     int64_t o_bs, const void* wq_a, const void* wk_a, const void* wq_b, const void* wk_b,
-                     const float* cos, const float* sin, int batch, int S, int H, int n_a, float eps, cudaStream_t st);
-int rmsnorm_rope_bwd(void* dq, void* dk, int64_t ld, int64_t bs, const void* xq, const void* xk, int64_t ldx, int64_t x_bs,
-                     const void* wq_a, const void* wk_a, const void* wq_b, const void* wk_b, const float* cos,
-                     const float* sin, float* partial, int batch, int S, int H, int n_a, float eps, cudaStream_t st);
-int gelu_rows(const void* x, int64_t ldx, void* y, int64_t ldy, int64_t rows, int D, cudaStream_t st);
-int outer_acc(const float* dmod, int64_t dmod_ld, const void* act, int64_t act_ld, float* dW, int64_t ldw, int B, int N,
-              int K, int accumulate, cudaStream_t st);
-int attn_delta(const void* o, int64_t ldo, const void* dout, int64_t lddo, float* delta, float* lse, int B, int H, int S,
-               int S_pad, cudaStream_t st);
-
 namespace {
 
 inline size_t al256(size_t n) { return (n + 255) & ~size_t(255); }
@@ -112,7 +68,7 @@ TrainWs carve(const FluxCtx* c, void* ws, int B, int S_img, int S_txt, size_t in
   w.lse = reinterpret_cast<float*>(take((size_t)B * c->cfg.num_heads * S_pad, 4));
   w.delta = reinterpret_cast<float*>(take((size_t)B * c->cfg.num_heads * S_pad, 4));
   // column-sum partials: the largest user is ln_modulate_bwd (B x chunks x 2d); RMSNorm: ceil(B*S/8) x 512
-  const size_t p1 = (size_t)B * train_ln_chunks((int)S) * 2 * d, p2 = (size_t)B * train_chunks((int)S) * 3 * d,
+  const size_t p1 = (size_t)B * b2f_train_ln_chunks((int)S) * 2 * d, p2 = (size_t)B * b2f_train_chunks((int)S) * 3 * d,
                p3 = (BS + 7) / 8 * 512;
   w.partial = reinterpret_cast<float*>(take(p1 > p2 ? (p1 > p3 ? p1 : p3) : (p2 > p3 ? p2 : p3), 4));
   w.dmod = reinterpret_cast<float*>(take((size_t)B * 6 * d, 4));
@@ -224,15 +180,15 @@ int b2f_flux_train_backward(b2f_flux* h, const void* dout, const void* mod, int6
   if ((rc = (expr)) != 0) return rc
   // row-offset helpers into [B, S, width] buffers (text rows first)
   auto img = [&](bf16_t* p, int64_t width) { return p + (int64_t)S_txt * width; };
-  const int nch = train_chunks(S), nlch = train_ln_chunks(S);
+  const int nch = b2f_train_chunks(S), nlch = b2f_train_ln_chunks(S);
 
   // column sums of a [B, rows, D] view into a flat fp32 gradient (summed over the batch as well)
   auto bias_grad = [&](const bf16_t* dy, int64_t ld, int64_t bs, int rows, int D, float* dst) -> int {
-    const int ch = train_chunks(rows);
-    int r = gate_bwd(dy, ld, bs, nullptr, 0, 0, nullptr, nullptr, 0, nullptr, 0, 0, w.partial, B, rows, D, 0, 0, st);
+    const int ch = b2f_train_chunks(rows);
+    int r = b2f_gate_bwd(dy, ld, bs, nullptr, 0, 0, nullptr, nullptr, 0, nullptr, 0, 0, w.partial, B, rows, D, 0, 0, st);
     if (r) return r;
     // partial is [B, ch, D]: reduce it as one batch of B*ch chunks
-    return col_reduce(w.partial, B * ch, D, dst, D, 1, acc0, st);
+    return b2f_col_reduce(w.partial, B * ch, D, dst, D, 1, acc0, st);
   };
   // AdaLN-linear gradients of one block from dmod[B, n_mod*d] (fp32) and silu(temb)
   auto adaln_grads = [&](const std::string& name, int n_mod) -> int {
@@ -241,8 +197,8 @@ int b2f_flux_train_backward(b2f_flux* h, const void* dout, const void* mod, int6
     Grad gb = find_grad(c, name + ".bias", (int64_t)n_mod * d, &r);
     if (r) return r;
     // dmod is [B, n_mod*d] with pitch n_mod*d (6d in a double block, 3d in a single block)
-    if (gw.p && (r = outer_acc(w.dmod, n_mod * d, silu_temb, silu_ld, gw.p, d, B, (int)(n_mod * d), (int)d, acc0, st))) return r;
-    if (gb.p && (r = col_reduce(w.dmod, B, (int)(n_mod * d), gb.p, n_mod * d, 1, acc0, st))) return r;
+    if (gw.p && (r = b2f_outer_acc(w.dmod, n_mod * d, silu_temb, silu_ld, gw.p, d, B, (int)(n_mod * d), (int)d, acc0, st))) return r;
+    if (gb.p && (r = b2f_col_reduce(w.dmod, B, (int)(n_mod * d), gb.p, n_mod * d, 1, acc0, st))) return r;
     return B2F_OK;
   };
 
@@ -252,10 +208,10 @@ int b2f_flux_train_backward(b2f_flux* h, const void* dout, const void* mod, int6
     const bf16_t* mo = modp + (int64_t)g.num_double * 12 * d + (int64_t)g.num_single * 3 * d;
     const bf16_t* hfin = w.ckpt + (int64_t)nblk * BS * d;
     // dxn[img rows < n_out] = dout . proj_out.weight     ([B, n_out, 64] x [64, d])
-    RUN(gemm_dgrad(dout, g.out_channels, (int64_t)n_out_rows * g.out_channels, c->proj_out.w, d, img(w.dxn, d), d, bs1, B,
-                   n_out_rows, (int)d, g.out_channels, B2F_EPI_BIAS, nullptr, 0, 0, st));
-    RUN(ln_modulate_bwd(img(const_cast<bf16_t*>(hfin), d), d, bs1, img(w.dxn, d), d, bs1, mo, nullptr, mod_ld, nullptr, 0, 0,
-                        img(w.dh, d), d, bs1, nullptr, B, n_out_rows, (int)d, eps, 0, 0, st));
+    RUN(b2f_gemm_dgrad(dout, g.out_channels, (int64_t)n_out_rows * g.out_channels, c->proj_out.w, d, img(w.dxn, d), d, bs1, B,
+                       n_out_rows, (int)d, g.out_channels, B2F_EPI_BIAS, nullptr, 0, 0, st));
+    RUN(b2f_ln_modulate_bwd(img(const_cast<bf16_t*>(hfin), d), d, bs1, img(w.dxn, d), d, bs1, mo, nullptr, mod_ld, nullptr, 0, 0,
+                            img(w.dh, d), d, bs1, nullptr, B, n_out_rows, (int)d, eps, 0, 0, st));
   }
 
   for (int blk = last_block - 1; blk >= first_block; --blk) {
@@ -266,96 +222,96 @@ int b2f_flux_train_backward(b2f_flux* h, const void* dout, const void* mod, int6
       const bf16_t* mi = modp + (int64_t)blk * 12 * d;
       const bf16_t* mt = mi + 6 * d;
       // ------------------------------------------------ recompute, unfused, keeping what the backward reads
-      RUN(ln_modulate(hin, d, bs1, mt + d, mt, mod_ld, w.xn, d, bs1, B, S, (int)d, eps, S_txt, mi + d, mi, st));
-      RUN(gemm_bf16(img(w.xn, d), d, bs1, wt.qkv.w, d, wt.qkv.b, img(w.pre, 3 * d), 3 * d, bs3, B, S_img, (int)(3 * d),
-                    (int)d, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
-      RUN(gemm_bf16(w.xn, d, bs1, wt.add_qkv.w, d, wt.add_qkv.b, w.pre, 3 * d, bs3, B, S_txt, (int)(3 * d), (int)d,
-                    B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
-      RUN(rmsnorm_rope_out(w.pre, w.pre + d, 3 * d, bs3, w.qkv, w.qkv + d, 3 * d, bs3, wt.norm_added_q, wt.norm_added_k,
-                           wt.norm_q, wt.norm_k, c->rope_cos, c->rope_sin, B, S, H, S_txt, eps, st));
-      RUN(attention_fwd_lse(w.qkv, 3 * d, w.qkv + d, 3 * d, w.pre + 2 * d, 3 * d, w.cat, 5 * d, B, H, H, S, S, g.head_dim,
-                            scale, 0, w.lse, S_pad, st));
-      RUN(gemm_bf16(img(w.cat, 5 * d), 5 * d, bs5, wt.to_out.w, d, wt.to_out.b, img(w.y1, d), d, bs1, B, S_img, (int)d, (int)d,
-                    B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
-      RUN(gemm_bf16(w.cat, 5 * d, bs5, wt.to_add_out.w, d, wt.to_add_out.b, w.y1, d, bs1, B, S_txt, (int)d, (int)d,
-                    B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
-      RUN(gate_resid_fwd(hin, d, bs1, w.y1, d, bs1, mt + 2 * d, mi + 2 * d, mod_ld, w.h1, d, bs1, B, S, (int)d, S_txt, st));
-      RUN(ln_modulate(w.h1, d, bs1, mt + 4 * d, mt + 3 * d, mod_ld, w.xn2, d, bs1, B, S, (int)d, eps, S_txt, mi + 4 * d,
-                      mi + 3 * d, st));
+      RUN(b2f_ln_modulate(hin, d, bs1, mt + d, mt, mod_ld, w.xn, d, bs1, B, S, (int)d, eps, S_txt, mi + d, mi, st));
+      RUN(b2f_gemm_bf16(img(w.xn, d), d, bs1, wt.qkv.w, d, wt.qkv.b, img(w.pre, 3 * d), 3 * d, bs3, B, S_img, (int)(3 * d),
+                        (int)d, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
+      RUN(b2f_gemm_bf16(w.xn, d, bs1, wt.add_qkv.w, d, wt.add_qkv.b, w.pre, 3 * d, bs3, B, S_txt, (int)(3 * d), (int)d,
+                        B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
+      RUN(b2f_rmsnorm_rope_out(w.pre, w.pre + d, 3 * d, bs3, w.qkv, w.qkv + d, 3 * d, bs3, wt.norm_added_q, wt.norm_added_k,
+                               wt.norm_q, wt.norm_k, c->rope_cos, c->rope_sin, B, S, H, S_txt, eps, st));
+      RUN(b2f_attention_fwd_lse(w.qkv, 3 * d, w.qkv + d, 3 * d, w.pre + 2 * d, 3 * d, w.cat, 5 * d, B, H, H, S, S, g.head_dim,
+                                scale, 0, w.lse, S_pad, st));
+      RUN(b2f_gemm_bf16(img(w.cat, 5 * d), 5 * d, bs5, wt.to_out.w, d, wt.to_out.b, img(w.y1, d), d, bs1, B, S_img, (int)d, (int)d,
+                        B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
+      RUN(b2f_gemm_bf16(w.cat, 5 * d, bs5, wt.to_add_out.w, d, wt.to_add_out.b, w.y1, d, bs1, B, S_txt, (int)d, (int)d,
+                        B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
+      RUN(b2f_gate_resid_fwd(hin, d, bs1, w.y1, d, bs1, mt + 2 * d, mi + 2 * d, mod_ld, w.h1, d, bs1, B, S, (int)d, S_txt, st));
+      RUN(b2f_ln_modulate(w.h1, d, bs1, mt + 4 * d, mt + 3 * d, mod_ld, w.xn2, d, bs1, B, S, (int)d, eps, S_txt, mi + 4 * d,
+                          mi + 3 * d, st));
       // u = pre-GELU MLP activations -> dpre buffer columns [0, 4d) are free until the backward of this block: keep u
       // in `pre` columns... the QKV pre-activations own pre[.., 0:3d]; u lives in pre[.., 3d:7d] (pitch 7d is not
       // shared with the 3d-pitched QKV view, so u gets its own region at the end of the buffer)
       bf16_t* u = w.pre + BS * 3 * d;   // [B, S, 4d], contiguous
       const int64_t bs4 = 4 * bs1;
-      RUN(gemm_bf16(img(w.xn2, d), d, bs1, wt.ff1.w, d, wt.ff1.b, img(u, 4 * d), 4 * d, bs4, B, S_img, (int)(4 * d), (int)d,
-                    B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
-      RUN(gemm_bf16(w.xn2, d, bs1, wt.ffc1.w, d, wt.ffc1.b, u, 4 * d, bs4, B, S_txt, (int)(4 * d), (int)d, B2F_EPI_BIAS,
-                    nullptr, 0, 0, nullptr, 0, st));
-      RUN(gelu_rows(u, 4 * d, w.cat + d, 5 * d, BS, (int)(4 * d), st));
-      RUN(gemm_bf16(img(w.cat, 5 * d) + d, 5 * d, bs5, wt.ff2.w, 4 * d, wt.ff2.b, img(w.y2, d), d, bs1, B, S_img, (int)d,
-                    (int)(4 * d), B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
-      RUN(gemm_bf16(w.cat + d, 5 * d, bs5, wt.ffc2.w, 4 * d, wt.ffc2.b, w.y2, d, bs1, B, S_txt, (int)d, (int)(4 * d),
-                    B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
+      RUN(b2f_gemm_bf16(img(w.xn2, d), d, bs1, wt.ff1.w, d, wt.ff1.b, img(u, 4 * d), 4 * d, bs4, B, S_img, (int)(4 * d), (int)d,
+                        B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
+      RUN(b2f_gemm_bf16(w.xn2, d, bs1, wt.ffc1.w, d, wt.ffc1.b, u, 4 * d, bs4, B, S_txt, (int)(4 * d), (int)d, B2F_EPI_BIAS,
+                        nullptr, 0, 0, nullptr, 0, st));
+      RUN(b2f_gelu_rows(u, 4 * d, w.cat + d, 5 * d, BS, (int)(4 * d), st));
+      RUN(b2f_gemm_bf16(img(w.cat, 5 * d) + d, 5 * d, bs5, wt.ff2.w, 4 * d, wt.ff2.b, img(w.y2, d), d, bs1, B, S_img, (int)d,
+                        (int)(4 * d), B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
+      RUN(b2f_gemm_bf16(w.cat + d, 5 * d, bs5, wt.ffc2.w, 4 * d, wt.ffc2.b, w.y2, d, bs1, B, S_txt, (int)d, (int)(4 * d),
+                        B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
       // ------------------------------------------------ backward
       // h2 = h1 + gate_mlp * y2
-      RUN(gate_bwd(w.dh, d, bs1, w.y2, d, bs1, mt + 5 * d, mi + 5 * d, mod_ld, w.dy, d, bs1, w.partial, B, S, (int)d, S_txt,
-                   S_txt, st));
-      RUN(col_reduce(w.partial, nch, (int)d, w.dmod + 5 * d, 6 * d, B, 0, st));
+      RUN(b2f_gate_bwd(w.dh, d, bs1, w.y2, d, bs1, mt + 5 * d, mi + 5 * d, mod_ld, w.dy, d, bs1, w.partial, B, S, (int)d, S_txt,
+                       S_txt, st));
+      RUN(b2f_col_reduce(w.partial, nch, (int)d, w.dmod + 5 * d, 6 * d, B, 0, st));
       // y2 = gelu(u) W2^T + b2:  du = (dy . W2) * gelu'(u)   -> dpre[.., 0:4d] viewed with pitch 4d
       bf16_t* du = w.dpre;   // [B, S, 4d]
-      RUN(gemm_dgrad(img(w.dy, d), d, bs1, wt.ff2.w, 4 * d, img(du, 4 * d), 4 * d, bs4, B, S_img, (int)(4 * d), (int)d,
-                     B2F_EPI_DGELU, img(u, 4 * d), 4 * d, bs4, st));
-      RUN(gemm_dgrad(w.dy, d, bs1, wt.ffc2.w, 4 * d, du, 4 * d, bs4, B, S_txt, (int)(4 * d), (int)d, B2F_EPI_DGELU, u, 4 * d,
-                     bs4, st));
+      RUN(b2f_gemm_dgrad(img(w.dy, d), d, bs1, wt.ff2.w, 4 * d, img(du, 4 * d), 4 * d, bs4, B, S_img, (int)(4 * d), (int)d,
+                         B2F_EPI_DGELU, img(u, 4 * d), 4 * d, bs4, st));
+      RUN(b2f_gemm_dgrad(w.dy, d, bs1, wt.ffc2.w, 4 * d, du, 4 * d, bs4, B, S_txt, (int)(4 * d), (int)d, B2F_EPI_DGELU, u, 4 * d,
+                         bs4, st));
       // u = xn2 W1^T + b1
-      RUN(gemm_dgrad(img(du, 4 * d), 4 * d, bs4, wt.ff1.w, d, img(w.dxn, d), d, bs1, B, S_img, (int)d, (int)(4 * d),
-                     B2F_EPI_BIAS, nullptr, 0, 0, st));
-      RUN(gemm_dgrad(du, 4 * d, bs4, wt.ffc1.w, d, w.dxn, d, bs1, B, S_txt, (int)d, (int)(4 * d), B2F_EPI_BIAS, nullptr, 0, 0,
-                     st));
+      RUN(b2f_gemm_dgrad(img(du, 4 * d), 4 * d, bs4, wt.ff1.w, d, img(w.dxn, d), d, bs1, B, S_img, (int)d, (int)(4 * d),
+                         B2F_EPI_BIAS, nullptr, 0, 0, st));
+      RUN(b2f_gemm_dgrad(du, 4 * d, bs4, wt.ffc1.w, d, w.dxn, d, bs1, B, S_txt, (int)d, (int)(4 * d), B2F_EPI_BIAS, nullptr, 0, 0,
+                         st));
       // xn2 = LN(h1) (1 + scale_mlp) + shift_mlp;  dh <- dh + dLN
-      RUN(ln_modulate_bwd(w.h1, d, bs1, w.dxn, d, bs1, mt + 4 * d, mi + 4 * d, mod_ld, w.dh, d, bs1, w.dh, d, bs1, w.partial,
-                          B, S, (int)d, eps, S_txt, S_txt, st));
+      RUN(b2f_ln_modulate_bwd(w.h1, d, bs1, w.dxn, d, bs1, mt + 4 * d, mi + 4 * d, mod_ld, w.dh, d, bs1, w.dh, d, bs1, w.partial,
+                              B, S, (int)d, eps, S_txt, S_txt, st));
       // partial rows are [dscale | dshift]; dmod columns are [.., shift_mlp (3d), scale_mlp (4d), ..]
-      RUN(col_reduce(w.partial, nlch, (int)(2 * d), w.red, 2 * d, B, 0, st));
+      RUN(b2f_col_reduce(w.partial, nlch, (int)(2 * d), w.red, 2 * d, B, 0, st));
       RUN(cuda_err(cudaMemcpy2DAsync(w.dmod + 4 * d, 6 * d * 4, w.red, 2 * d * 4, d * 4, B, cudaMemcpyDeviceToDevice, st),
                    "dscale copy"));
       RUN(cuda_err(cudaMemcpy2DAsync(w.dmod + 3 * d, 6 * d * 4, w.red + d, 2 * d * 4, d * 4, B, cudaMemcpyDeviceToDevice, st),
                    "dshift copy"));
       // h1 = h + gate_msa * y1
-      RUN(gate_bwd(w.dh, d, bs1, w.y1, d, bs1, mt + 2 * d, mi + 2 * d, mod_ld, w.dy, d, bs1, w.partial, B, S, (int)d, S_txt,
-                   S_txt, st));
-      RUN(col_reduce(w.partial, nch, (int)d, w.dmod + 2 * d, 6 * d, B, 0, st));
+      RUN(b2f_gate_bwd(w.dh, d, bs1, w.y1, d, bs1, mt + 2 * d, mi + 2 * d, mod_ld, w.dy, d, bs1, w.partial, B, S, (int)d, S_txt,
+                       S_txt, st));
+      RUN(b2f_col_reduce(w.partial, nch, (int)d, w.dmod + 2 * d, 6 * d, B, 0, st));
       // y1 = attn W_o^T + b_o   (image stream: to_out is trainable)
       {
         Grad gw = find_grad(c, pn + "attn.to_out.0.weight", d * d, &rc);
         Grad gb = find_grad(c, pn + "attn.to_out.0.bias", d, &rc);
         if (rc) return rc;
         if (gw.p)
-          RUN(gemm_wgrad(img(w.dy, d), d, bs1, img(w.cat, 5 * d), 5 * d, bs5, gw.p, d, B, S_img, (int)d, (int)d, acc0, st));
+          RUN(b2f_gemm_wgrad(img(w.dy, d), d, bs1, img(w.cat, 5 * d), 5 * d, bs5, gw.p, d, B, S_img, (int)d, (int)d, acc0, st));
         if (gb.p) RUN(bias_grad(img(w.dy, d), d, bs1, S_img, (int)d, gb.p));
       }
-      RUN(gemm_dgrad(img(w.dy, d), d, bs1, wt.to_out.w, d, img(w.dattn, d), d, bs1, B, S_img, (int)d, (int)d, B2F_EPI_BIAS,
-                     nullptr, 0, 0, st));
-      RUN(gemm_dgrad(w.dy, d, bs1, wt.to_add_out.w, d, w.dattn, d, bs1, B, S_txt, (int)d, (int)d, B2F_EPI_BIAS, nullptr, 0, 0,
-                     st));
+      RUN(b2f_gemm_dgrad(img(w.dy, d), d, bs1, wt.to_out.w, d, img(w.dattn, d), d, bs1, B, S_img, (int)d, (int)d, B2F_EPI_BIAS,
+                         nullptr, 0, 0, st));
+      RUN(b2f_gemm_dgrad(w.dy, d, bs1, wt.to_add_out.w, d, w.dattn, d, bs1, B, S_txt, (int)d, (int)d, B2F_EPI_BIAS, nullptr, 0, 0,
+                         st));
       // joint attention
       bf16_t* dqkv = w.dpre + BS * 4 * d;   // [B, S, 3d] after the du region
-      RUN(attn_delta(w.cat, 5 * d, w.dattn, d, w.delta, w.lse, B, H, S, (int)S_pad, st));
-      RUN(attention_bwd(w.qkv, 3 * d, w.qkv + d, 3 * d, w.pre + 2 * d, 3 * d, w.dattn, d, w.lse, w.delta, S_pad, dqkv, 3 * d,
-                        dqkv + d, 3 * d, dqkv + 2 * d, 3 * d, B, H, S, g.head_dim, scale, st));
+      RUN(b2f_attn_delta(w.cat, 5 * d, w.dattn, d, w.delta, w.lse, B, H, S, (int)S_pad, st));
+      RUN(b2f_attention_bwd(w.qkv, 3 * d, w.qkv + d, 3 * d, w.pre + 2 * d, 3 * d, w.dattn, d, w.lse, w.delta, S_pad, dqkv, 3 * d,
+                            dqkv + d, 3 * d, dqkv + 2 * d, 3 * d, B, H, S, g.head_dim, scale, st));
       // per-head RMSNorm + RoPE of q, k
       {
         Grad gq = find_grad(c, pn + "attn.norm_q.weight", g.head_dim, &rc);
         Grad gk = find_grad(c, pn + "attn.norm_k.weight", g.head_dim, &rc);
         if (rc) return rc;
         const bool want = gq.p || gk.p;
-        RUN(rmsnorm_rope_bwd(dqkv, dqkv + d, 3 * d, bs3, w.pre, w.pre + d, 3 * d, bs3, wt.norm_added_q, wt.norm_added_k,
-                             wt.norm_q, wt.norm_k, c->rope_cos, c->rope_sin, want ? w.partial : nullptr, B, S, H, S_txt, eps, st));
+        RUN(b2f_rmsnorm_rope_bwd(dqkv, dqkv + d, 3 * d, bs3, w.pre, w.pre + d, 3 * d, bs3, wt.norm_added_q, wt.norm_added_k,
+                                 wt.norm_q, wt.norm_k, c->rope_cos, c->rope_sin, want ? w.partial : nullptr, B, S, H, S_txt, eps, st));
         if (want) {
-          RUN(col_reduce(w.partial, (int)((BS + 7) / 8), 512, w.red, 512, 1, 0, st));
+          RUN(b2f_col_reduce(w.partial, (int)((BS + 7) / 8), 512, w.red, 512, 1, 0, st));
           // red = [wq_a | wk_a | wq_b | wk_b]: the image stream's norm_q / norm_k are set b
-          if (gq.p) RUN(col_reduce(w.red + 256, 1, 128, gq.p, 128, 1, acc0, st));
-          if (gk.p) RUN(col_reduce(w.red + 384, 1, 128, gk.p, 128, 1, acc0, st));
+          if (gq.p) RUN(b2f_col_reduce(w.red + 256, 1, 128, gq.p, 128, 1, acc0, st));
+          if (gk.p) RUN(b2f_col_reduce(w.red + 384, 1, 128, gk.p, 128, 1, acc0, st));
         }
       }
       // qkv = xn1 Wqkv^T + b
@@ -364,17 +320,17 @@ int b2f_flux_train_backward(b2f_flux* h, const void* dout, const void* mod, int6
         Grad gb = find_grad(c, pn + "attn.qkv.bias", 3 * d, &rc);
         if (rc) return rc;
         if (gw.p)
-          RUN(gemm_wgrad(img(dqkv, 3 * d), 3 * d, bs3, img(w.xn, d), d, bs1, gw.p, d, B, S_img, (int)(3 * d), (int)d, acc0, st));
+          RUN(b2f_gemm_wgrad(img(dqkv, 3 * d), 3 * d, bs3, img(w.xn, d), d, bs1, gw.p, d, B, S_img, (int)(3 * d), (int)d, acc0, st));
         if (gb.p) RUN(bias_grad(img(dqkv, 3 * d), 3 * d, bs3, S_img, (int)(3 * d), gb.p));
       }
-      RUN(gemm_dgrad(img(dqkv, 3 * d), 3 * d, bs3, wt.qkv.w, d, img(w.dxn, d), d, bs1, B, S_img, (int)d, (int)(3 * d),
-                     B2F_EPI_BIAS, nullptr, 0, 0, st));
-      RUN(gemm_dgrad(dqkv, 3 * d, bs3, wt.add_qkv.w, d, w.dxn, d, bs1, B, S_txt, (int)d, (int)(3 * d), B2F_EPI_BIAS, nullptr,
-                     0, 0, st));
+      RUN(b2f_gemm_dgrad(img(dqkv, 3 * d), 3 * d, bs3, wt.qkv.w, d, img(w.dxn, d), d, bs1, B, S_img, (int)d, (int)(3 * d),
+                         B2F_EPI_BIAS, nullptr, 0, 0, st));
+      RUN(b2f_gemm_dgrad(dqkv, 3 * d, bs3, wt.add_qkv.w, d, w.dxn, d, bs1, B, S_txt, (int)d, (int)(3 * d), B2F_EPI_BIAS, nullptr,
+                         0, 0, st));
       // xn1 = LN(h) (1 + scale_msa) + shift_msa
-      RUN(ln_modulate_bwd(hin, d, bs1, w.dxn, d, bs1, mt + d, mi + d, mod_ld, w.dh, d, bs1, w.dh, d, bs1, w.partial, B, S,
-                          (int)d, eps, S_txt, S_txt, st));
-      RUN(col_reduce(w.partial, nlch, (int)(2 * d), w.red, 2 * d, B, 0, st));
+      RUN(b2f_ln_modulate_bwd(hin, d, bs1, w.dxn, d, bs1, mt + d, mi + d, mod_ld, w.dh, d, bs1, w.dh, d, bs1, w.partial, B, S,
+                              (int)d, eps, S_txt, S_txt, st));
+      RUN(b2f_col_reduce(w.partial, nlch, (int)(2 * d), w.red, 2 * d, B, 0, st));
       RUN(cuda_err(cudaMemcpy2DAsync(w.dmod + d, 6 * d * 4, w.red, 2 * d * 4, d * 4, B, cudaMemcpyDeviceToDevice, st),
                    "dscale copy"));
       RUN(cuda_err(cudaMemcpy2DAsync(w.dmod, 6 * d * 4, w.red + d, 2 * d * 4, d * 4, B, cudaMemcpyDeviceToDevice, st),
@@ -386,51 +342,51 @@ int b2f_flux_train_backward(b2f_flux* h, const void* dout, const void* mod, int6
       const std::string pn = "single_transformer_blocks." + std::to_string(si) + ".";
       const bf16_t* ms = modp + (int64_t)g.num_double * 12 * d + (int64_t)si * 3 * d;
       // ------------------------------------------------ recompute
-      RUN(ln_modulate(hin, d, bs1, ms + d, ms, mod_ld, w.xn, d, bs1, B, S, (int)d, eps, 0, nullptr, nullptr, st));
-      RUN(gemm_bf16(w.xn, d, bs1, wt.qkv_mlp.w, d, wt.qkv_mlp.b, w.pre, 7 * d, bs7, B, S, (int)(7 * d), (int)d, B2F_EPI_BIAS,
-                    nullptr, 0, 0, nullptr, 0, st));
-      RUN(rmsnorm_rope_out(w.pre, w.pre + d, 7 * d, bs7, w.qkv, w.qkv + d, 3 * d, bs3, nullptr, nullptr, wt.norm_q, wt.norm_k,
-                           c->rope_cos, c->rope_sin, B, S, H, 0, eps, st));
-      RUN(attention_fwd_lse(w.qkv, 3 * d, w.qkv + d, 3 * d, w.pre + 2 * d, 7 * d, w.cat, 5 * d, B, H, H, S, S, g.head_dim,
-                            scale, 0, w.lse, S_pad, st));
-      RUN(gelu_rows(w.pre + 3 * d, 7 * d, w.cat + d, 5 * d, BS, (int)(4 * d), st));
-      RUN(gemm_bf16(w.cat, 5 * d, bs5, wt.proj_out.w, 5 * d, wt.proj_out.b, w.y1, d, bs1, B, S, (int)d, (int)(5 * d),
-                    B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
+      RUN(b2f_ln_modulate(hin, d, bs1, ms + d, ms, mod_ld, w.xn, d, bs1, B, S, (int)d, eps, 0, nullptr, nullptr, st));
+      RUN(b2f_gemm_bf16(w.xn, d, bs1, wt.qkv_mlp.w, d, wt.qkv_mlp.b, w.pre, 7 * d, bs7, B, S, (int)(7 * d), (int)d, B2F_EPI_BIAS,
+                        nullptr, 0, 0, nullptr, 0, st));
+      RUN(b2f_rmsnorm_rope_out(w.pre, w.pre + d, 7 * d, bs7, w.qkv, w.qkv + d, 3 * d, bs3, nullptr, nullptr, wt.norm_q, wt.norm_k,
+                               c->rope_cos, c->rope_sin, B, S, H, 0, eps, st));
+      RUN(b2f_attention_fwd_lse(w.qkv, 3 * d, w.qkv + d, 3 * d, w.pre + 2 * d, 7 * d, w.cat, 5 * d, B, H, H, S, S, g.head_dim,
+                                scale, 0, w.lse, S_pad, st));
+      RUN(b2f_gelu_rows(w.pre + 3 * d, 7 * d, w.cat + d, 5 * d, BS, (int)(4 * d), st));
+      RUN(b2f_gemm_bf16(w.cat, 5 * d, bs5, wt.proj_out.w, 5 * d, wt.proj_out.b, w.y1, d, bs1, B, S, (int)d, (int)(5 * d),
+                        B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
       // ------------------------------------------------ backward
-      RUN(gate_bwd(w.dh, d, bs1, w.y1, d, bs1, ms + 2 * d, nullptr, mod_ld, w.dy, d, bs1, w.partial, B, S, (int)d, 0, 0, st));
-      RUN(col_reduce(w.partial, nch, (int)d, w.dmod + 2 * d, 3 * d, B, 0, st));
+      RUN(b2f_gate_bwd(w.dh, d, bs1, w.y1, d, bs1, ms + 2 * d, nullptr, mod_ld, w.dy, d, bs1, w.partial, B, S, (int)d, 0, 0, st));
+      RUN(b2f_col_reduce(w.partial, nch, (int)d, w.dmod + 2 * d, 3 * d, B, 0, st));
       // y = [attn | gelu(u)] Wp^T + b:  dattn = dy . Wp[:, :d];  du = (dy . Wp[:, d:]) * gelu'(u)  -> dpre[.., 3d:7d]
-      RUN(gemm_dgrad(w.dy, d, bs1, wt.proj_out.w, 5 * d, w.dattn, d, bs1, B, S, (int)d, (int)d, B2F_EPI_BIAS, nullptr, 0, 0, st));
-      RUN(gemm_dgrad(w.dy, d, bs1, wt.proj_out.w + d, 5 * d, w.dpre + 3 * d, 7 * d, bs7, B, S, (int)(4 * d), (int)d,
-                     B2F_EPI_DGELU, w.pre + 3 * d, 7 * d, bs7, st));
-      RUN(attn_delta(w.cat, 5 * d, w.dattn, d, w.delta, w.lse, B, H, S, (int)S_pad, st));
-      RUN(attention_bwd(w.qkv, 3 * d, w.qkv + d, 3 * d, w.pre + 2 * d, 7 * d, w.dattn, d, w.lse, w.delta, S_pad, w.dpre, 7 * d,
-                        w.dpre + d, 7 * d, w.dpre + 2 * d, 7 * d, B, H, S, g.head_dim, scale, st));
+      RUN(b2f_gemm_dgrad(w.dy, d, bs1, wt.proj_out.w, 5 * d, w.dattn, d, bs1, B, S, (int)d, (int)d, B2F_EPI_BIAS, nullptr, 0, 0, st));
+      RUN(b2f_gemm_dgrad(w.dy, d, bs1, wt.proj_out.w + d, 5 * d, w.dpre + 3 * d, 7 * d, bs7, B, S, (int)(4 * d), (int)d,
+                         B2F_EPI_DGELU, w.pre + 3 * d, 7 * d, bs7, st));
+      RUN(b2f_attn_delta(w.cat, 5 * d, w.dattn, d, w.delta, w.lse, B, H, S, (int)S_pad, st));
+      RUN(b2f_attention_bwd(w.qkv, 3 * d, w.qkv + d, 3 * d, w.pre + 2 * d, 7 * d, w.dattn, d, w.lse, w.delta, S_pad, w.dpre, 7 * d,
+                            w.dpre + d, 7 * d, w.dpre + 2 * d, 7 * d, B, H, S, g.head_dim, scale, st));
       {
         Grad gq = find_grad(c, pn + "attn.norm_q.weight", g.head_dim, &rc);
         Grad gk = find_grad(c, pn + "attn.norm_k.weight", g.head_dim, &rc);
         if (rc) return rc;
         const bool want = gq.p || gk.p;
-        RUN(rmsnorm_rope_bwd(w.dpre, w.dpre + d, 7 * d, bs7, w.pre, w.pre + d, 7 * d, bs7, nullptr, nullptr, wt.norm_q,
-                             wt.norm_k, c->rope_cos, c->rope_sin, want ? w.partial : nullptr, B, S, H, 0, eps, st));
+        RUN(b2f_rmsnorm_rope_bwd(w.dpre, w.dpre + d, 7 * d, bs7, w.pre, w.pre + d, 7 * d, bs7, nullptr, nullptr, wt.norm_q,
+                                 wt.norm_k, c->rope_cos, c->rope_sin, want ? w.partial : nullptr, B, S, H, 0, eps, st));
         if (want) {
-          RUN(col_reduce(w.partial, (int)((BS + 7) / 8), 512, w.red, 512, 1, 0, st));
-          if (gq.p) RUN(col_reduce(w.red + 256, 1, 128, gq.p, 128, 1, acc0, st));
-          if (gk.p) RUN(col_reduce(w.red + 384, 1, 128, gk.p, 128, 1, acc0, st));
+          RUN(b2f_col_reduce(w.partial, (int)((BS + 7) / 8), 512, w.red, 512, 1, 0, st));
+          if (gq.p) RUN(b2f_col_reduce(w.red + 256, 1, 128, gq.p, 128, 1, acc0, st));
+          if (gk.p) RUN(b2f_col_reduce(w.red + 384, 1, 128, gk.p, 128, 1, acc0, st));
         }
       }
       {
         Grad gw = find_grad(c, pn + "attn.qkv.weight", 3 * d * d, &rc);
         Grad gb = find_grad(c, pn + "attn.qkv.bias", 3 * d, &rc);
         if (rc) return rc;
-        if (gw.p) RUN(gemm_wgrad(w.dpre, 7 * d, bs7, w.xn, d, bs1, gw.p, d, B, S, (int)(3 * d), (int)d, acc0, st));
+        if (gw.p) RUN(b2f_gemm_wgrad(w.dpre, 7 * d, bs7, w.xn, d, bs1, gw.p, d, B, S, (int)(3 * d), (int)d, acc0, st));
         if (gb.p) RUN(bias_grad(w.dpre, 7 * d, bs7, S, (int)(3 * d), gb.p));
       }
-      RUN(gemm_dgrad(w.dpre, 7 * d, bs7, wt.qkv_mlp.w, d, w.dxn, d, bs1, B, S, (int)d, (int)(7 * d), B2F_EPI_BIAS, nullptr, 0,
-                     0, st));
-      RUN(ln_modulate_bwd(hin, d, bs1, w.dxn, d, bs1, ms + d, nullptr, mod_ld, w.dh, d, bs1, w.dh, d, bs1, w.partial, B, S,
-                          (int)d, eps, 0, 0, st));
-      RUN(col_reduce(w.partial, nlch, (int)(2 * d), w.red, 2 * d, B, 0, st));
+      RUN(b2f_gemm_dgrad(w.dpre, 7 * d, bs7, wt.qkv_mlp.w, d, w.dxn, d, bs1, B, S, (int)d, (int)(7 * d), B2F_EPI_BIAS, nullptr, 0,
+                         0, st));
+      RUN(b2f_ln_modulate_bwd(hin, d, bs1, w.dxn, d, bs1, ms + d, nullptr, mod_ld, w.dh, d, bs1, w.dh, d, bs1, w.partial, B, S,
+                              (int)d, eps, 0, 0, st));
+      RUN(b2f_col_reduce(w.partial, nlch, (int)(2 * d), w.red, 2 * d, B, 0, st));
       RUN(cuda_err(cudaMemcpy2DAsync(w.dmod + d, 3 * d * 4, w.red, 2 * d * 4, d * 4, B, cudaMemcpyDeviceToDevice, st),
                    "dscale copy"));
       RUN(cuda_err(cudaMemcpy2DAsync(w.dmod, 3 * d * 4, w.red + d, 2 * d * 4, d * 4, B, cudaMemcpyDeviceToDevice, st),
@@ -441,8 +397,8 @@ int b2f_flux_train_backward(b2f_flux* h, const void* dout, const void* mod, int6
 
   // ---------------------------------------------------------------- head: gradient w.r.t. encoder_hidden_states
   if (d_enc && first_block == 0)
-    RUN(gemm_dgrad(w.dh, d, bs1, c->context_embedder.w, g.joint_dim, d_enc, g.joint_dim, (int64_t)S_txt * g.joint_dim, B,
-                   S_txt, g.joint_dim, (int)d, B2F_EPI_BIAS, nullptr, 0, 0, st));
+    RUN(b2f_gemm_dgrad(w.dh, d, bs1, c->context_embedder.w, g.joint_dim, d_enc, g.joint_dim, (int64_t)S_txt * g.joint_dim, B,
+                       S_txt, g.joint_dim, (int)d, B2F_EPI_BIAS, nullptr, 0, 0, st));
 #undef RUN
   return B2F_OK;
 }

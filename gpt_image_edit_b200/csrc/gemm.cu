@@ -18,14 +18,11 @@
 // Replaces: torch.nn.functional.linear → cuBLASLt (diffusers FluxTransformer2DModel linears,
 // reference call site univa/utils/flux_pipeline.py:1067; SURVEY.md §2b row 1).
 #include <algorithm>
-#include <atomic>
 #include <cstdlib>
 
 #include "gemm_sm90.cuh"
 
 namespace b2f {
-
-extern std::atomic<uint64_t> g_launch_count;
 
 namespace {
 
@@ -591,8 +588,7 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cu
     prof_end_tagged(KC_GEMM, stream, 2.0 * p.batch * (double)p.M * p.N * kk,
                     2.0 * ((double)p.batch * p.M * kk + (double)p.N * kk + (double)p.batch * p.M * p.N), tag_);
   }
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("gemm_bf16_kernel");
+  B2F_LAUNCHED("gemm_bf16_kernel", 1);
   return B2F_OK;
 }
 
@@ -714,10 +710,11 @@ static int gemm_bf16_impl(const void* A, int64_t lda, int64_t a_bs, const void* 
   return launch_gemm<0, true>(tmA, tmB, p, stream, lp);
 }
 
-int gemm_bf16(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
-              const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N,
-              int K, int epilogue, const void* resid, int64_t ldr, int64_t resid_bs, const void* gate,
-              int64_t gate_ld, cudaStream_t stream) {
+extern "C" int b2f_gemm_bf16(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias,
+                             void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epilogue,
+                             const void* resid, int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld,
+                             b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (epilogue == B2F_EPI_QKV_NORM_ROPE) return B2F_ERR_INVALID;  // needs the extended entry point
   return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, N, K, epilogue, resid, ldr,
                         resid_bs, gate, gate_ld, nullptr, stream);
@@ -727,9 +724,10 @@ int gemm_bf16(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t l
 // backward-data GEMM of every linear layer on the training path (reference train_denoiser.py:1172,
 // accelerator.backward -> autograd of F.linear).  Epilogues: B2F_EPI_BIAS (plain store), B2F_EPI_DGELU /
 // B2F_EPI_DSILU (times act'(u), u = `resid` [batch, M, N]), B2F_EPI_RESID (accumulate into another gradient).
-int gemm_dgrad(const void* dY, int64_t ldy, int64_t dy_bs, const void* W, int64_t ldw, void* dX, int64_t ldx,
-               int64_t dx_bs, int batch, int M, int N, int K, int epilogue, const void* aux, int64_t ld_aux,
-               int64_t aux_bs, cudaStream_t stream) {
+extern "C" int b2f_gemm_dgrad(const void* dY, int64_t ldy, int64_t dy_bs, const void* W, int64_t ldw, void* dX,
+                              int64_t ldx, int64_t dx_bs, int batch, int M, int N, int K, int epilogue, const void* aux,
+                              int64_t ld_aux, int64_t aux_bs, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (batch <= 0 || M <= 0 || N <= 0 || K <= 0 || !dY || !W || !dX) return B2F_ERR_INVALID;
   if ((K & 7) || (N & 7) || (ldy & 7) || (ldw & 7) || (ldx & 7) || (dy_bs & 7) || (dx_bs & 7)) return B2F_ERR_ALIGN;
@@ -763,8 +761,10 @@ int gemm_dgrad(const void* dY, int64_t ldy, int64_t dy_bs, const void* W, int64_
 // dW[M, N] (+)= sum_b dY[b, :, M]^T . X[b, :, N]  (fp32 output, contraction over the `rows` tokens of every batch
 // item): the backward-weight GEMM of the trainable projections (reference train_denoiser.py:71-119 names them).
 // dY: [batch, rows, >= M] view, X: [batch, rows, >= N] view (token pitches ldy / ldx, batch pitches in elements).
-int gemm_wgrad(const void* dY, int64_t ldy, int64_t dy_bs, const void* X, int64_t ldx, int64_t x_bs, float* dW,
-               int64_t ldw, int batch, int rows, int M, int N, int accumulate, cudaStream_t stream) {
+extern "C" int b2f_gemm_wgrad(const void* dY, int64_t ldy, int64_t dy_bs, const void* X, int64_t ldx, int64_t x_bs,
+                              float* dW, int64_t ldw, int batch, int rows, int M, int N, int accumulate,
+                              b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (batch <= 0 || rows <= 0 || M <= 0 || N <= 0 || !dY || !X || !dW) return B2F_ERR_INVALID;
   if ((M & 7) || (N & 7) || (ldy & 7) || (ldx & 7) || (dy_bs & 7) || (x_bs & 7) || (ldw & 3)) return B2F_ERR_ALIGN;
@@ -791,11 +791,12 @@ int gemm_wgrad(const void* dY, int64_t ldy, int64_t dy_bs, const void* X, int64_
   return launch_gemm<2>(tmA, tmB, p, stream);
 }
 
-int gemm_qkv_norm_rope(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
-                       const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M,
-                       int d_model, int K, const void* nw_q, const void* nw_k, const float* cos,
-                       const float* sin, int rope_row0, float eps, int n_extra, void* out_extra,
-                       int64_t ld_extra, int64_t bs_extra, int epi_extra, cudaStream_t stream) {
+extern "C" int b2f_gemm_qkv_norm_rope(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
+                                      const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M,
+                                      int d_model, int K, const void* nw_q, const void* nw_k, const float* cos,
+                                      const float* sin, int rope_row0, float eps, int n_extra, void* out_extra,
+                                      int64_t ld_extra, int64_t bs_extra, int epi_extra, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   QkvExtra qx{nw_q, nw_k, cos, sin, rope_row0, d_model, eps, n_extra, epi_extra, out_extra, ld_extra, bs_extra};
   return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, 3 * d_model + n_extra, K,
                         B2F_EPI_QKV_NORM_ROPE, nullptr, 0, 0, nullptr, 0, &qx, stream);
@@ -803,22 +804,26 @@ int gemm_qkv_norm_rope(const void* A, int64_t lda, int64_t a_bs, const void* W, 
 
 // ---------------------------------------------------------------------------------------------------- LoRA
 // out = epi(A W^T + T Bcat^T + bias): the forward GEMM with r_pad / 64 extra k-blocks per tile (LoraExt).
-int gemm_bf16_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias, void* out,
-                   int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epilogue, const void* resid,
-                   int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld, const void* T, int64_t ldt,
-                   int64_t t_bs, const void* Bc, int64_t ldbc, int r_pad, cudaStream_t stream) {
+extern "C" int b2f_gemm_bf16_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
+                                  const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N,
+                                  int K, int epilogue, const void* resid, int64_t ldr, int64_t resid_bs,
+                                  const void* gate, int64_t gate_ld, const void* T, int64_t ldt, int64_t t_bs,
+                                  const void* Bc, int64_t ldbc, int r_pad, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (epilogue == B2F_EPI_QKV_NORM_ROPE || r_pad <= 0) return B2F_ERR_INVALID;
   const LoraExt lx{T, ldt, t_bs, Bc, ldbc, r_pad, nullptr, 1.f};
   return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, N, K, epilogue, resid, ldr,
                         resid_bs, gate, gate_ld, nullptr, stream, &lx);
 }
 
-int gemm_qkv_norm_rope_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, const void* bias,
-                            void* out, int64_t ldc, int64_t out_bs, int batch, int M, int d_model, int K,
-                            const void* nw_q, const void* nw_k, const float* cos, const float* sin, int rope_row0,
-                            float eps, int n_extra, void* out_extra, int64_t ld_extra, int64_t bs_extra,
-                            int epi_extra, const void* T, int64_t ldt, int64_t t_bs, const void* Bc, int64_t ldbc,
-                            int r_pad, cudaStream_t stream) {
+extern "C" int b2f_gemm_qkv_norm_rope_lora(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
+                                           const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M,
+                                           int d_model, int K, const void* nw_q, const void* nw_k, const float* cos,
+                                           const float* sin, int rope_row0, float eps, int n_extra, void* out_extra,
+                                           int64_t ld_extra, int64_t bs_extra, int epi_extra, const void* T,
+                                           int64_t ldt, int64_t t_bs, const void* Bc, int64_t ldbc, int r_pad,
+                                           b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (r_pad <= 0) return B2F_ERR_INVALID;
   QkvExtra qx{nw_q, nw_k, cos, sin, rope_row0, d_model, eps, n_extra, epi_extra, out_extra, ld_extra, bs_extra};
   const LoraExt lx{T, ldt, t_bs, Bc, ldbc, r_pad, nullptr, 1.f};
@@ -827,9 +832,10 @@ int gemm_qkv_norm_rope_lora(const void* A, int64_t lda, int64_t a_bs, const void
 }
 
 // LoRA down projection: out[batch, M, N] = bf16((A W^T)[., n] * fp32(colscale[n] * cs_mul)), W = Acat [N, K].
-int gemm_colscale(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, void* out, int64_t ldc,
-                  int64_t out_bs, int batch, int M, int N, int K, const float* colscale, float cs_mul,
-                  cudaStream_t stream) {
+extern "C" int b2f_gemm_colscale(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw, void* out,
+                                 int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, const float* colscale,
+                                 float cs_mul, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!colscale) return B2F_ERR_INVALID;
   const LoraExt lx{nullptr, 0, 0, nullptr, 0, 0, colscale, cs_mul};
   return gemm_bf16_impl(A, lda, a_bs, W, ldw, nullptr, out, ldc, out_bs, batch, M, N, K, B2F_EPI_BIAS, nullptr, 0, 0,

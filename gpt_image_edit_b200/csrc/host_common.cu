@@ -1,4 +1,5 @@
-// Device facts + TMA tensor-map encoding (driver entry point fetched at run time).
+// Library-wide entry points (error strings, version, device facts, launch count, profiler) and TMA
+// tensor-map encoding (driver entry point fetched at run time).
 #include "host_common.h"
 
 #include <cstring>
@@ -12,6 +13,41 @@
 namespace b2f {
 
 std::atomic<uint64_t> g_launch_count{0};
+
+extern "C" uint64_t b2f_launch_count(void) { return g_launch_count.load(); }
+
+extern "C" const char* b2f_strerror(int code) {
+  switch (code) {
+    case B2F_OK: return "ok";
+    case B2F_ERR_INVALID: return "invalid argument or shape";
+    case B2F_ERR_CUDA: return "CUDA error (see stderr)";
+    case B2F_ERR_UNSUPPORTED: return "unsupported shape or mode";
+    case B2F_ERR_ALIGN: return "pointer or pitch not 16-byte aligned";
+    case B2F_ERR_NODEVICE: return "no sm_90 device";
+    case B2F_ERR_WORKSPACE: return "workspace too small";
+    default: return "unknown error";
+  }
+}
+
+extern "C" int b2f_version(void) { return 2; }
+
+extern "C" int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin) {
+  int n = 0;
+  if (cudaGetDeviceCount(&n) != cudaSuccess || n == 0) {
+    cudaGetLastError();
+    return B2F_ERR_NODEVICE;
+  }
+  int dev = 0, v = 0;
+  cudaGetDevice(&dev);
+  if (num_sms) cudaDeviceGetAttribute(num_sms, cudaDevAttrMultiProcessorCount, dev);
+  if (cc_major) cudaDeviceGetAttribute(cc_major, cudaDevAttrComputeCapabilityMajor, dev);
+  if (cc_minor) cudaDeviceGetAttribute(cc_minor, cudaDevAttrComputeCapabilityMinor, dev);
+  if (smem_optin) {
+    cudaDeviceGetAttribute(&v, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev);
+    *smem_optin = (size_t)v;
+  }
+  return B2F_OK;
+}
 
 const DeviceInfo& device_info() {
   static DeviceInfo info;
@@ -84,9 +120,9 @@ void prof_end_tagged(int kc, cudaStream_t s, double flops, double bytes, const c
   sh.recs.push_back(g_prof.recs[kc].back());     // the event pair is shared with the class list (freed there)
   sh.flops += flops;
 }
-void prof_set(bool on) { g_prof.enabled = on; }
-// "tag\tlaunches\tms\tTFLOP/s\n" per shape since the last call; must be called BEFORE prof_collect (which recycles the events)
-int prof_shapes(char* buf, int cap) {
+extern "C" void b2f_prof_enable(int on) { g_prof.enabled = on != 0; }
+// "tag\tlaunches\tms\tTFLOP/s\n" per shape since the last call; call BEFORE b2f_prof_collect (which recycles the events)
+extern "C" int b2f_prof_shapes(char* buf, int cap) {
   std::lock_guard<std::mutex> lk(g_prof.mu);
   std::string out;
   for (auto& kv : g_prof.shapes) {
@@ -107,7 +143,7 @@ int prof_shapes(char* buf, int cap) {
   memcpy(buf, out.c_str(), out.size() + 1);
   return (int)out.size();
 }
-int prof_collect(int kc, double* ms, int64_t* launches, double* flops, double* bytes) {
+extern "C" int b2f_prof_collect(int kc, double* ms, int64_t* launches, double* flops, double* bytes) {
   if (kc < 0 || kc >= KC_COUNT) return B2F_ERR_INVALID;
   std::lock_guard<std::mutex> lk(g_prof.mu);
   double total = 0;

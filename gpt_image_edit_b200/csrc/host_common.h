@@ -1,8 +1,10 @@
-// Host-side helpers shared by the launchers: error codes, TMA tensor-map encoding through the
-// driver entry point (no -lcuda link, so the library loads on a box without a driver).
+// Host-side helpers shared by the launchers: error codes, launch counting, TMA tensor-map encoding through
+// the driver entry point (no -lcuda link, so the library loads on a box without a driver).  Every launcher
+// is itself the extern "C" b2f_* entry point that include/b2f.h declares.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <atomic>
 #include <cstdint>
 #include <cstdio>
 
@@ -45,10 +47,15 @@ inline int cuda_err(cudaError_t e, const char* what) {
   return B2F_ERR_CUDA;
 }
 
-#define B2F_CHECK_LAUNCH(name)                              \
-  do {                                                      \
-    cudaError_t _e = cudaGetLastError();                    \
-    if (_e != cudaSuccess) return b2f::cuda_err(_e, name);  \
+// Kernels launched since load (b2f_launch_count).
+extern std::atomic<uint64_t> g_launch_count;
+
+// After enqueueing n kernels: count them, and return B2F_ERR_CUDA from the launcher if a launch failed.
+#define B2F_LAUNCHED(name, n)                                           \
+  do {                                                                  \
+    b2f::g_launch_count.fetch_add((n), std::memory_order_relaxed);      \
+    cudaError_t _e = cudaGetLastError();                                \
+    if (_e != cudaSuccess) return b2f::cuda_err(_e, name);              \
   } while (0)
 
 }  // namespace b2f

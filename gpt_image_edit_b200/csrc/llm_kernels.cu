@@ -2,14 +2,10 @@
 // They restate the torch-eager chains of transformers' Qwen2_5_VL modules (SURVEY.md Appendix B;
 // reference call site univa/models/qwen2p5vl/modeling_univa_qwen2p5vl.py:373-399, 481-492) with the
 // same bf16 rounding points.
-#include <atomic>
-
 #include "host_common.h"
 #include "ptx.cuh"
 
 namespace b2f {
-
-extern std::atomic<uint64_t> g_launch_count;
 
 namespace {
 
@@ -221,8 +217,9 @@ __global__ void __launch_bounds__(256) embed_kernel(const __nv_bfloat16* tok, lo
 
 }  // namespace
 
-int rmsnorm(const void* x, int64_t ldx, const void* w, void* y, int64_t ldy, int64_t rows, int D,
-            float eps, cudaStream_t stream) {
+extern "C" int b2f_rmsnorm(const void* x, int64_t ldx, const void* w, void* y, int64_t ldy, int64_t rows, int D,
+                           float eps, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!x || !w || !y || rows <= 0) return B2F_ERR_INVALID;
   if (D <= 0 || (D & 255) || D > 5120) return B2F_ERR_UNSUPPORTED;
@@ -237,38 +234,38 @@ int rmsnorm(const void* x, int64_t ldx, const void* w, void* y, int64_t ldy, int
     rmsnorm_kernel<14><<<grid, 128, 0, stream>>>(X, ldx, W, Y, ldy, rows, D, eps);
   else
     rmsnorm_kernel<20><<<grid, 128, 0, stream>>>(X, ldx, W, Y, ldy, rows, D, eps);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("rmsnorm_kernel");
+  B2F_LAUNCHED("rmsnorm_kernel", 1);
   return B2F_OK;
 }
 
-int rope_half(void* x, int64_t ld, int heads, int head_pitch, const float* cos, const float* sin,
-              int rot, int64_t tokens, int fp32_math, cudaStream_t stream) {
+extern "C" int b2f_rope_half(void* x, int64_t ld, int heads, int head_pitch, const float* cos, const float* sin,
+                             int rot, int64_t tokens, int fp32_math, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!x || !cos || !sin || heads <= 0 || tokens <= 0 || rot <= 0 || (rot & 1) || rot > head_pitch)
     return B2F_ERR_INVALID;
   const long long total = tokens * heads;
   rope_half_kernel<<<(unsigned)((total + 7) / 8), 256, 0, stream>>>(
       static_cast<__nv_bfloat16*>(x), ld, heads, head_pitch, cos, sin, rot, tokens, fp32_math);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("rope_half_kernel");
+  B2F_LAUNCHED("rope_half_kernel", 1);
   return B2F_OK;
 }
 
-int swiglu(const void* gu, int64_t ld, void* out, int64_t ldo, int64_t rows, int I,
-           cudaStream_t stream) {
+extern "C" int b2f_swiglu(const void* gu, int64_t ld, void* out, int64_t ldo, int64_t rows, int I,
+                          b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!gu || !out || rows <= 0 || I <= 0 || (I & 7) || (ld & 7) || (ldo & 7)) return B2F_ERR_INVALID;
   const long long n = rows * (I >> 3);
   swiglu_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(
       static_cast<const __nv_bfloat16*>(gu), ld, static_cast<__nv_bfloat16*>(out), ldo, rows, I);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("swiglu_kernel");
+  B2F_LAUNCHED("swiglu_kernel", 1);
   return B2F_OK;
 }
 
-int move_rows(const void* src, int64_t ld_src, void* dst, int64_t ld_dst, const int64_t* idx, int64_t n,
-              int D, int scatter, cudaStream_t stream) {
+extern "C" int b2f_move_rows(const void* src, int64_t ld_src, void* dst, int64_t ld_dst, const int64_t* idx, int64_t n,
+                             int D, int scatter, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!src || !dst || !idx || n <= 0 || D <= 0 || (D & 7) || (ld_src & 7) || (ld_dst & 7))
     return B2F_ERR_INVALID;
@@ -276,24 +273,25 @@ int move_rows(const void* src, int64_t ld_src, void* dst, int64_t ld_dst, const 
   move_rows_kernel<<<(unsigned)((tot + 255) / 256), 256, 0, stream>>>(
       static_cast<const __nv_bfloat16*>(src), ld_src, static_cast<__nv_bfloat16*>(dst), ld_dst,
       reinterpret_cast<const long long*>(idx), n, D, scatter);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("move_rows_kernel");
+  B2F_LAUNCHED("move_rows_kernel", 1);
   return B2F_OK;
 }
 
-int geglu(const void* gu, int64_t ld, void* out, int64_t ldo, int64_t rows, int I, cudaStream_t stream) {
+extern "C" int b2f_geglu(const void* gu, int64_t ld, void* out, int64_t ldo, int64_t rows, int I,
+                         b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!gu || !out || rows <= 0 || I <= 0 || (I & 7) || (ld & 7) || (ldo & 7)) return B2F_ERR_INVALID;
   const long long n = rows * (I >> 3);
   geglu_kernel<<<(unsigned)((n + 255) / 256), 256, 0, stream>>>(
       static_cast<const __nv_bfloat16*>(gu), ld, static_cast<__nv_bfloat16*>(out), ldo, rows, I);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("geglu_kernel");
+  B2F_LAUNCHED("geglu_kernel", 1);
   return B2F_OK;
 }
 
-int layernorm(const void* x, int64_t ldx, const void* w, const void* b, void* y, int64_t ldy,
-              int64_t rows, int D, float eps, cudaStream_t stream) {
+extern "C" int b2f_layernorm(const void* x, int64_t ldx, const void* w, const void* b, void* y, int64_t ldy,
+                             int64_t rows, int D, float eps, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!x || !w || !b || !y || rows <= 0) return B2F_ERR_INVALID;
   if (D <= 0 || (D & 255) || D > 5120) return B2F_ERR_UNSUPPORTED;
@@ -307,13 +305,13 @@ int layernorm(const void* x, int64_t ldx, const void* w, const void* b, void* y,
     layernorm_kernel<5><<<grid, 128, 0, stream>>>(X, ldx, W, Bv, Y, ldy, rows, D, eps);
   else
     layernorm_kernel<20><<<grid, 128, 0, stream>>>(X, ldx, W, Bv, Y, ldy, rows, D, eps);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("layernorm_kernel");
+  B2F_LAUNCHED("layernorm_kernel", 1);
   return B2F_OK;
 }
 
-int embed(const void* tok, int64_t ld_tok, const int64_t* ids, const void* pos, int64_t ld_pos, int period,
-          void* out, int64_t ldo, int64_t n, int D, cudaStream_t stream) {
+extern "C" int b2f_embed(const void* tok, int64_t ld_tok, const int64_t* ids, const void* pos, int64_t ld_pos,
+                         int period, void* out, int64_t ldo, int64_t n, int D, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!tok || !ids || !out || n <= 0 || D <= 0 || (D & 7) || (ld_tok & 7) || (ldo & 7)) return B2F_ERR_INVALID;
   if (pos && (period <= 0 || (ld_pos & 7))) return B2F_ERR_INVALID;
@@ -322,8 +320,7 @@ int embed(const void* tok, int64_t ld_tok, const int64_t* ids, const void* pos, 
       static_cast<const __nv_bfloat16*>(tok), ld_tok, reinterpret_cast<const long long*>(ids),
       static_cast<const __nv_bfloat16*>(pos), ld_pos, period > 0 ? period : 1,
       static_cast<__nv_bfloat16*>(out), ldo, n, D);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("embed_kernel");
+  B2F_LAUNCHED("embed_kernel", 1);
   return B2F_OK;
 }
 

@@ -62,8 +62,9 @@ __global__ void __launch_bounds__(256) lora_fuse_kernel(uint16_t* W, int64_t ldw
 
 }  // namespace
 
-int lora_fuse(void* W, int64_t ldw, int rows, int cols, const void* Bc, int64_t ldb, const void* A, int64_t lda,
-              const float* colscale, float cs_mul, int r, cudaStream_t stream) {
+extern "C" int b2f_lora_fuse(void* W, int64_t ldw, int rows, int cols, const void* Bc, int64_t ldb, const void* A,
+                             int64_t lda, const float* colscale, float cs_mul, int r, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!W || !Bc || !A || !colscale || rows <= 0 || cols <= 0 || r <= 0 || ldw < cols || lda < cols || ldb < r)
     return B2F_ERR_INVALID;
@@ -72,7 +73,7 @@ int lora_fuse(void* W, int64_t ldw, int rows, int cols, const void* Bc, int64_t 
   lora_fuse_kernel<<<grid, 256, 0, stream>>>(static_cast<uint16_t*>(W), ldw, rows, cols,
                                              static_cast<const uint16_t*>(Bc), ldb, static_cast<const uint16_t*>(A),
                                              lda, colscale, cs_mul, r);
-  B2F_CHECK_LAUNCH("lora_fuse_kernel");
+  B2F_LAUNCHED("lora_fuse_kernel", 1);
   return B2F_OK;
 }
 

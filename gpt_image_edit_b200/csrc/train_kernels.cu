@@ -7,14 +7,10 @@
 // arithmetic is fp32, parameter gradients and every reduction over tokens are fp32.  Column reductions over tokens
 // (bias / gate / scale / shift / RMSNorm-weight gradients) are two-stage and deterministic: each block writes a
 // partial row into a caller-provided fp32 scratch, `col_reduce` sums the partial rows in a fixed order.
-#include <atomic>
-
 #include "host_common.h"
 #include "ptx.cuh"
 
 namespace b2f {
-
-extern std::atomic<uint64_t> g_launch_count;
 
 namespace {
 
@@ -663,17 +659,13 @@ inline bool al16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) =
 
 }  // namespace
 
-#define B2F_TRAIN_LAUNCHED(name)                           \
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);  \
-  B2F_CHECK_LAUNCH(name);                                  \
-  return B2F_OK
+extern "C" int b2f_train_chunks(int rows) { return (rows + CHUNK_ROWS - 1) / CHUNK_ROWS; }
+extern "C" int b2f_train_ln_chunks(int rows) { return (rows + CHUNK_LN - 1) / CHUNK_LN; }
 
-int train_chunks(int rows) { return (rows + CHUNK_ROWS - 1) / CHUNK_ROWS; }
-int train_ln_chunks(int rows) { return (rows + CHUNK_LN - 1) / CHUNK_LN; }
-
-int gate_resid_fwd(const void* x, int64_t ldx, int64_t x_bs, const void* y, int64_t ldy, int64_t y_bs, const void* gate,
-                   const void* gate_b, int64_t gate_ld, void* out, int64_t ldo, int64_t o_bs, int batch, int rows, int D,
-                   int split_row, cudaStream_t st) {
+extern "C" int b2f_gate_resid_fwd(const void* x, int64_t ldx, int64_t x_bs, const void* y, int64_t ldy, int64_t y_bs,
+                                  const void* gate, const void* gate_b, int64_t gate_ld, void* out, int64_t ldo,
+                                  int64_t o_bs, int batch, int rows, int D, int split_row, b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!x || !y || !gate || !out || batch <= 0 || rows <= 0 || D <= 0 || (D & 7)) return B2F_ERR_INVALID;
   if (split_row > 0 && !gate_b) return B2F_ERR_INVALID;
   if ((ldx | x_bs | ldy | y_bs | ldo | o_bs | gate_ld) & 7) return B2F_ERR_ALIGN;
@@ -686,17 +678,20 @@ int gate_resid_fwd(const void* x, int64_t ldx, int64_t x_bs, const void* y, int6
   p.out = static_cast<__nv_bfloat16*>(out);
   p.ldx = ldx; p.x_bs = x_bs; p.ldy = ldy; p.y_bs = y_bs; p.ldo = ldo; p.o_bs = o_bs; p.gate_ld = gate_ld;
   p.batch = batch; p.rows = rows; p.D = D; p.split_row = split_row;
-  dim3 grid(train_chunks(rows), (D + 1023) / 1024, batch);
+  dim3 grid(b2f_train_chunks(rows), (D + 1023) / 1024, batch);
   prof_begin(KC_OTHER, st);
   gate_resid_fwd_kernel<<<grid, 128, 0, st>>>(p);
   prof_end(KC_OTHER, st, 0, 6.0 * batch * rows * D);
-  B2F_TRAIN_LAUNCHED("gate_resid_fwd_kernel");
+  B2F_LAUNCHED("gate_resid_fwd_kernel", 1);
+  return B2F_OK;
 }
 
-// partial: fp32 scratch of batch * train_chunks(rows) * D floats (may be null: no column sums)
-int gate_bwd(const void* dout, int64_t ldd, int64_t d_bs, const void* y, int64_t ldy, int64_t y_bs, const void* gate,
-             const void* gate_b, int64_t gate_ld, void* dy, int64_t ldo, int64_t o_bs, float* partial, int batch,
-             int rows, int D, int split_row, int part_row0, cudaStream_t st) {
+// partial: fp32 scratch of batch * b2f_train_chunks(rows) * D floats (may be null: no column sums)
+extern "C" int b2f_gate_bwd(const void* dout, int64_t ldd, int64_t d_bs, const void* y, int64_t ldy, int64_t y_bs,
+                            const void* gate, const void* gate_b, int64_t gate_ld, void* dy, int64_t ldo, int64_t o_bs,
+                            float* partial, int batch, int rows, int D, int split_row, int part_row0,
+                            b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!dout || batch <= 0 || rows <= 0 || D <= 0 || (D & 7)) return B2F_ERR_INVALID;
   if (dy && !gate) return B2F_ERR_INVALID;
   if (gate && split_row > 0 && !gate_b) return B2F_ERR_INVALID;
@@ -711,26 +706,31 @@ int gate_bwd(const void* dout, int64_t ldd, int64_t d_bs, const void* y, int64_t
   p.partial = partial;
   p.ldx = ldd; p.x_bs = d_bs; p.ldy = ldy; p.y_bs = y_bs; p.ldo = ldo; p.o_bs = o_bs; p.gate_ld = gate_ld;
   p.batch = batch; p.rows = rows; p.D = D; p.split_row = split_row; p.part_row0 = part_row0;
-  dim3 grid(train_chunks(rows), (D + 1023) / 1024, batch);
+  dim3 grid(b2f_train_chunks(rows), (D + 1023) / 1024, batch);
   prof_begin(KC_OTHER, st);
   gate_bwd_kernel<<<grid, 128, 0, st>>>(p);
   prof_end(KC_OTHER, st, 0, (2.0 + (y ? 2.0 : 0.0) + (dy ? 2.0 : 0.0)) * batch * rows * D);
-  B2F_TRAIN_LAUNCHED("gate_bwd_kernel");
+  B2F_LAUNCHED("gate_bwd_kernel", 1);
+  return B2F_OK;
 }
 
-int col_reduce(const float* partial, int nchunks, int D, float* out, int64_t out_ld, int batch, int accumulate,
-               cudaStream_t st) {
+extern "C" int b2f_col_reduce(const float* partial, int nchunks, int D, float* out, int64_t out_ld, int batch,
+                              int accumulate, b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!partial || !out || nchunks <= 0 || D <= 0 || batch <= 0) return B2F_ERR_INVALID;
   dim3 grid((D + 255) / 256, batch);
   col_reduce_kernel<<<grid, 256, 0, st>>>(partial, nchunks, D, out, out_ld, accumulate);
-  B2F_TRAIN_LAUNCHED("col_reduce_kernel");
+  B2F_LAUNCHED("col_reduce_kernel", 1);
+  return B2F_OK;
 }
 
-// partial: batch * train_ln_chunks(rows) * 2 * D floats (dscale | dshift per chunk), or null
-int ln_modulate_bwd(const void* x, int64_t ldx, int64_t x_bs, const void* dy, int64_t ldy, int64_t dy_bs,
-                    const void* scale, const void* scale_b, int64_t mod_ld, const void* dres_in, int64_t ldr, int64_t r_bs,
-                    void* dres_out, int64_t ldo, int64_t o_bs, float* partial, int batch, int rows, int D, float eps,
-                    int split_row, int part_row0, cudaStream_t st) {
+// partial: batch * b2f_train_ln_chunks(rows) * 2 * D floats (dscale | dshift per chunk), or null
+extern "C" int b2f_ln_modulate_bwd(const void* x, int64_t ldx, int64_t x_bs, const void* dy, int64_t ldy, int64_t dy_bs,
+                                   const void* scale, const void* scale_b, int64_t mod_ld, const void* dres_in,
+                                   int64_t ldr, int64_t r_bs, void* dres_out, int64_t ldo, int64_t o_bs, float* partial,
+                                   int batch, int rows, int D, float eps, int split_row, int part_row0,
+                                   b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!x || !dy || !scale || !dres_out || batch <= 0 || rows <= 0 || D <= 0 || (D & 7)) return B2F_ERR_INVALID;
   if (split_row > 0 && !scale_b) return B2F_ERR_INVALID;
   if ((ldx | x_bs | ldy | dy_bs | ldr | r_bs | ldo | o_bs | mod_ld) & 7) return B2F_ERR_ALIGN;
@@ -747,16 +747,19 @@ int ln_modulate_bwd(const void* x, int64_t ldx, int64_t x_bs, const void* dy, in
   p.ldx = ldx; p.x_bs = x_bs; p.ldy = ldy; p.dy_bs = dy_bs; p.ldr = ldr; p.r_bs = r_bs; p.ldo = ldo; p.o_bs = o_bs;
   p.mod_ld = mod_ld;
   p.batch = batch; p.rows = rows; p.D = D; p.split_row = split_row; p.part_row0 = part_row0; p.eps = eps;
-  dim3 grid(train_ln_chunks(rows), batch);
+  dim3 grid(b2f_train_ln_chunks(rows), batch);
   prof_begin(KC_LNMOD, st);
   ln_modulate_bwd_kernel<<<grid, 256, 0, st>>>(p);
   prof_end(KC_LNMOD, st, 0, (dres_in ? 8.0 : 6.0) * batch * rows * D);
-  B2F_TRAIN_LAUNCHED("ln_modulate_bwd_kernel");
+  B2F_LAUNCHED("ln_modulate_bwd_kernel", 1);
+  return B2F_OK;
 }
 
-int rmsnorm_rope_out(const void* xq, const void* xk, int64_t ldx, int64_t x_bs, void* oq, void* ok, int64_t ldo,
-                     int64_t o_bs, const void* wq_a, const void* wk_a, const void* wq_b, const void* wk_b,
-                     const float* cos, const float* sin, int batch, int S, int H, int n_a, float eps, cudaStream_t st) {
+extern "C" int b2f_rmsnorm_rope_out(const void* xq, const void* xk, int64_t ldx, int64_t x_bs, void* oq, void* ok,
+                                    int64_t ldo, int64_t o_bs, const void* wq_a, const void* wk_a, const void* wq_b,
+                                    const void* wk_b, const float* cos, const float* sin, int batch, int S, int H,
+                                    int n_a, float eps, b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!xq || !xk || !oq || !ok || !wq_b || !wk_b || !cos || !sin || batch <= 0 || S <= 0 || H <= 0) return B2F_ERR_INVALID;
   if (n_a > 0 && (!wq_a || !wk_a)) return B2F_ERR_INVALID;
   if ((ldx | x_bs | ldo | o_bs) & 7) return B2F_ERR_ALIGN;
@@ -775,13 +778,16 @@ int rmsnorm_rope_out(const void* xq, const void* xk, int64_t ldx, int64_t x_bs, 
   prof_begin(KC_NORMROPE, st);
   rmsnorm_rope_out_kernel<<<(unsigned)((tokens + 7) / 8), 256, 0, st>>>(p);
   prof_end(KC_NORMROPE, st, 0, 8.0 * tokens * H * 128);
-  B2F_TRAIN_LAUNCHED("rmsnorm_rope_out_kernel");
+  B2F_LAUNCHED("rmsnorm_rope_out_kernel", 1);
+  return B2F_OK;
 }
 
 // partial: ((batch*S + 7) / 8) * 512 floats, or null.  dq/dk are updated in place.
-int rmsnorm_rope_bwd(void* dq, void* dk, int64_t ld, int64_t bs, const void* xq, const void* xk, int64_t ldx, int64_t x_bs,
-                     const void* wq_a, const void* wk_a, const void* wq_b, const void* wk_b, const float* cos,
-                     const float* sin, float* partial, int batch, int S, int H, int n_a, float eps, cudaStream_t st) {
+extern "C" int b2f_rmsnorm_rope_bwd(void* dq, void* dk, int64_t ld, int64_t bs, const void* xq, const void* xk,
+                                    int64_t ldx, int64_t x_bs, const void* wq_a, const void* wk_a, const void* wq_b,
+                                    const void* wk_b, const float* cos, const float* sin, float* partial, int batch,
+                                    int S, int H, int n_a, float eps, b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!dq || !dk || !xq || !xk || !wq_b || !wk_b || !cos || !sin || batch <= 0 || S <= 0 || H <= 0) return B2F_ERR_INVALID;
   if (n_a > 0 && (!wq_a || !wk_a)) return B2F_ERR_INVALID;
   if ((ld | bs | ldx | x_bs) & 7) return B2F_ERR_ALIGN;
@@ -800,32 +806,39 @@ int rmsnorm_rope_bwd(void* dq, void* dk, int64_t ld, int64_t bs, const void* xq,
   prof_begin(KC_NORMROPE, st);
   rmsnorm_rope_bwd_kernel<<<(unsigned)((tokens + 7) / 8), 256, 0, st>>>(p);
   prof_end(KC_NORMROPE, st, 0, 12.0 * tokens * H * 128);
-  B2F_TRAIN_LAUNCHED("rmsnorm_rope_bwd_kernel");
+  B2F_LAUNCHED("rmsnorm_rope_bwd_kernel", 1);
+  return B2F_OK;
 }
 
-int gelu_rows(const void* x, int64_t ldx, void* y, int64_t ldy, int64_t rows, int D, cudaStream_t st) {
+extern "C" int b2f_gelu_rows(const void* x, int64_t ldx, void* y, int64_t ldy, int64_t rows, int D,
+                             b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!x || !y || rows <= 0 || D <= 0 || (D & 7) || (ldx & 7) || (ldy & 7)) return B2F_ERR_INVALID;
   const long long n = rows * (D / 8);
   prof_begin(KC_OTHER, st);
   gelu_rows_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(static_cast<const __nv_bfloat16*>(x), ldx,
                                                                static_cast<__nv_bfloat16*>(y), ldy, rows, D);
   prof_end(KC_OTHER, st, 0, 4.0 * rows * D);
-  B2F_TRAIN_LAUNCHED("gelu_rows_kernel");
+  B2F_LAUNCHED("gelu_rows_kernel", 1);
+  return B2F_OK;
 }
 
-int outer_acc(const float* dmod, int64_t dmod_ld, const void* act, int64_t act_ld, float* dW, int64_t ldw, int B, int N,
-              int K, int accumulate, cudaStream_t st) {
+extern "C" int b2f_outer_acc(const float* dmod, int64_t dmod_ld, const void* act, int64_t act_ld, float* dW,
+                             int64_t ldw, int B, int N, int K, int accumulate, b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!dmod || !act || !dW || B <= 0 || N <= 0 || K <= 0 || (K & 3) || (ldw & 3) || (act_ld & 3)) return B2F_ERR_INVALID;
   dim3 grid((K / 4 + 255) / 256, N);
   prof_begin(KC_OTHER, st);
   outer_acc_kernel<<<grid, 256, 0, st>>>(dmod, dmod_ld, static_cast<const __nv_bfloat16*>(act), act_ld, dW, ldw, B, N, K,
                                         accumulate);
   prof_end(KC_OTHER, st, 0, (accumulate ? 8.0 : 4.0) * N * K);
-  B2F_TRAIN_LAUNCHED("outer_acc_kernel");
+  B2F_LAUNCHED("outer_acc_kernel", 1);
+  return B2F_OK;
 }
 
-int attn_delta(const void* o, int64_t ldo, const void* dout, int64_t lddo, float* delta, float* lse, int B, int H, int S,
-               int S_pad, cudaStream_t st) {
+extern "C" int b2f_attn_delta(const void* o, int64_t ldo, const void* dout, int64_t lddo, float* delta, float* lse,
+                              int B, int H, int S, int S_pad, b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!o || !dout || !delta || !lse || B <= 0 || H <= 0 || S <= 0 || S_pad < S || (ldo & 7) || (lddo & 7)) return B2F_ERR_INVALID;
   const long long threads = (long long)B * H * S_pad * 16;
   prof_begin(KC_OTHER, st);
@@ -833,43 +846,52 @@ int attn_delta(const void* o, int64_t ldo, const void* dout, int64_t lddo, float
                                                                       static_cast<const __nv_bfloat16*>(dout), lddo, delta,
                                                                       lse, B, H, S, S_pad);
   prof_end(KC_OTHER, st, 0, 4.0 * B * H * S * 128);
-  B2F_TRAIN_LAUNCHED("attn_delta_kernel");
+  B2F_LAUNCHED("attn_delta_kernel", 1);
+  return B2F_OK;
 }
 
 // loss_out: device scalar; ws: >= 1024 floats of scratch
-int mse_loss(const void* pred, const float* target, const float* w, void* dpred, float* loss_out, float* ws, int64_t n,
-             float grad_scale, cudaStream_t st) {
+extern "C" int b2f_mse_loss(const void* pred, const float* target, const float* w, void* dpred, float* loss_out,
+                            float* ws, int64_t n, float grad_scale, b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!pred || !target || !loss_out || !ws || n <= 0) return B2F_ERR_INVALID;
   const int blocks = int(n / 256 < 1 ? 1 : (n / 256 > 1024 ? 1024 : n / 256));
   mse_loss_kernel<<<blocks, 256, 0, st>>>(static_cast<const __nv_bfloat16*>(pred), target, w,
                                           static_cast<__nv_bfloat16*>(dpred), ws, n, grad_scale / float(n),
                                           1.0f / float(n));
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("mse_loss_kernel");
+  B2F_LAUNCHED("mse_loss_kernel", 1);
   // loss = sum of the per-block partial means
   col_reduce_kernel<<<dim3(1, 1), 256, 0, st>>>(ws, blocks, 1, loss_out, 1, 0);
-  B2F_TRAIN_LAUNCHED("col_reduce_kernel");
+  B2F_LAUNCHED("col_reduce_kernel", 1);
+  return B2F_OK;
 }
 
 // sumsq_out (+)= sum(g^2);  ws: >= 1024 floats
-int grad_sumsq(const float* g, int64_t n, float* sumsq_out, float* ws, int accumulate, cudaStream_t st) {
+extern "C" int b2f_grad_sumsq(const float* g, int64_t n, float* sumsq_out, float* ws, int accumulate,
+                              b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!g || !sumsq_out || !ws || n <= 0) return B2F_ERR_INVALID;
   const int blocks = int(n / 1024 < 1 ? 1 : (n / 1024 > 1024 ? 1024 : n / 1024));
   sumsq_kernel<<<blocks, 256, 0, st>>>(g, n, ws);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("sumsq_kernel");
+  B2F_LAUNCHED("sumsq_kernel", 1);
   col_reduce_kernel<<<dim3(1, 1), 256, 0, st>>>(ws, blocks, 1, sumsq_out, 1, accumulate);
-  B2F_TRAIN_LAUNCHED("col_reduce_kernel");
+  B2F_LAUNCHED("col_reduce_kernel", 1);
+  return B2F_OK;
 }
 
-int clip_coef(const float* sumsq, float max_norm, float pre_scale, float* coef, float* norm_out, cudaStream_t st) {
+extern "C" int b2f_clip_coef(const float* sumsq, float max_norm, float pre_scale, float* coef, float* norm_out,
+                             b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!sumsq || !coef) return B2F_ERR_INVALID;
   clip_coef_kernel<<<1, 1, 0, st>>>(sumsq, max_norm, pre_scale, coef, norm_out);
-  B2F_TRAIN_LAUNCHED("clip_coef_kernel");
+  B2F_LAUNCHED("clip_coef_kernel", 1);
+  return B2F_OK;
 }
 
-int adamw_step(float* p32, float* m, float* v, const float* g, void* p16, int64_t n, float lr, float beta1, float beta2,
-               float eps, float wd, int step, const float* gscale, cudaStream_t st) {
+extern "C" int b2f_adamw_step(float* p32, float* m, float* v, const float* g, void* p16, int64_t n, float lr,
+                              float beta1, float beta2, float eps, float wd, int step, const float* gscale,
+                              b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!p32 || !m || !v || !g || n <= 0 || step <= 0) return B2F_ERR_INVALID;
   AdamParams a{};
   a.p32 = p32; a.m = m; a.v = v; a.g = g; a.p16 = static_cast<__nv_bfloat16*>(p16); a.n = n;
@@ -881,23 +903,29 @@ int adamw_step(float* p32, float* m, float* v, const float* g, void* p16, int64_
   prof_begin(KC_OTHER, st);
   adamw_kernel<<<(unsigned)(blocks > 148 * 16 ? 148 * 16 : blocks), 256, 0, st>>>(a);
   prof_end(KC_OTHER, st, 0, 30.0 * n);
-  B2F_TRAIN_LAUNCHED("adamw_kernel");
+  B2F_LAUNCHED("adamw_kernel", 1);
+  return B2F_OK;
 }
 
-int blend_bf16(const void* a, const void* b, float wa, float wb, void* out, int64_t n, cudaStream_t st) {
+extern "C" int b2f_blend_bf16(const void* a, const void* b, float wa, float wb, void* out, int64_t n,
+                              b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!a || !b || !out || n <= 0 || (n & 7)) return B2F_ERR_INVALID;
   if (!al16(a) || !al16(b) || !al16(out)) return B2F_ERR_ALIGN;
   blend_kernel<<<(unsigned)((n / 8 + 255) / 256), 256, 0, st>>>(static_cast<const __nv_bfloat16*>(a),
                                                              static_cast<const __nv_bfloat16*>(b), wa, wb,
                                                              static_cast<__nv_bfloat16*>(out), n / 8);
-  B2F_TRAIN_LAUNCHED("blend_kernel");
+  B2F_LAUNCHED("blend_kernel", 1);
+  return B2F_OK;
 }
 
-int cast_bf16_f32(const void* src, void* dst, int64_t n, int to_f32, cudaStream_t st) {
+extern "C" int b2f_cast_bf16_f32(const void* src, void* dst, int64_t n, int to_f32, b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   if (!src || !dst || n <= 0) return B2F_ERR_INVALID;
   const long long blocks = (n + 255) / 256;
   cast_kernel<<<(unsigned)(blocks > 148 * 16 ? 148 * 16 : blocks), 256, 0, st>>>(src, dst, n, to_f32);
-  B2F_TRAIN_LAUNCHED("cast_kernel");
+  B2F_LAUNCHED("cast_kernel", 1);
+  return B2F_OK;
 }
 
 }  // namespace b2f

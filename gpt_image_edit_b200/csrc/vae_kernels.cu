@@ -2,14 +2,10 @@
 //   GroupNorm(32 groups, eps, affine) [+ SiLU]  — statistics pass + apply pass
 //   nearest 2x upsample, NCHW -> NHWC channel-padded import, row softmax and a bf16 transpose
 //   (the last two serve the single-head dh=512 mid-block attention, run as GEMMs).
-#include <atomic>
-
 #include "host_common.h"
 #include "ptx.cuh"
 
 namespace b2f {
-
-extern std::atomic<uint64_t> g_launch_count;
 
 namespace {
 
@@ -246,8 +242,10 @@ __global__ void __launch_bounds__(256) transpose_kernel(const __nv_bfloat16* in,
 
 }  // namespace
 
-int groupnorm_silu(const void* x, const void* gamma, const void* beta, void* y, double* stats_ws,
-                   int N, long long P, int C, float eps, int silu, cudaStream_t stream) {
+extern "C" int b2f_groupnorm_silu(const void* x, const void* gamma, const void* beta, void* y, void* stats_ws_, int N,
+                                  int64_t P, int C, float eps, int silu, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  double* stats_ws = static_cast<double*>(stats_ws_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!x || !gamma || !beta || !y || !stats_ws || N <= 0 || P <= 0) return B2F_ERR_INVALID;
   if (C % 32 || C % 8 || C > 2048 || (GN_THREADS % (C / 8)) != 0) return B2F_ERR_UNSUPPORTED;
@@ -263,12 +261,12 @@ int groupnorm_silu(const void* x, const void* gamma, const void* beta, void* y, 
                                           static_cast<const __nv_bfloat16*>(beta),
                                           static_cast<__nv_bfloat16*>(y), P, C, eps, silu);
   prof_end(KC_OTHER, stream, 0.0, 6.0 * N * (double)P * C);
-  g_launch_count.fetch_add(2, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("groupnorm kernels");
+  B2F_LAUNCHED("groupnorm kernels", 2);
   return B2F_OK;
 }
 
-int upsample2x(const void* in, void* out, int N, int H, int W, int C, cudaStream_t stream) {
+extern "C" int b2f_upsample2x(const void* in, void* out, int N, int H, int W, int C, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!in || !out || N <= 0 || H <= 0 || W <= 0 || C <= 0 || (C & 7)) return B2F_ERR_INVALID;
   const long long total = (long long)N * 4 * H * W * (C / 8);
@@ -276,13 +274,13 @@ int upsample2x(const void* in, void* out, int N, int H, int W, int C, cudaStream
   upsample2x_kernel<<<(unsigned)((total + 255) / 256), 256, 0, stream>>>(
       static_cast<const uint4*>(in), static_cast<uint4*>(out), N, H, W, C / 8);
   prof_end(KC_OTHER, stream, 0.0, 2.0 * N * (double)H * W * C * 5.0);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("upsample2x_kernel");
+  B2F_LAUNCHED("upsample2x_kernel", 1);
   return B2F_OK;
 }
 
-int nchw_to_nhwc_pad(const void* in, int in_is_f32, void* out, int N, int C, int H, int W, int Cpad,
-                     cudaStream_t stream) {
+extern "C" int b2f_nchw_to_nhwc_pad(const void* in, int in_is_f32, void* out, int N, int C, int H, int W, int Cpad,
+                                    b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!in || !out || N <= 0 || C <= 0 || H <= 0 || W <= 0 || Cpad < C || (Cpad & 7)) return B2F_ERR_INVALID;
   const long long total = (long long)N * H * W * (Cpad / 8);
@@ -296,31 +294,30 @@ int nchw_to_nhwc_pad(const void* in, int in_is_f32, void* out, int N, int C, int
   else
     nchw_to_nhwc_pad_kernel<__nv_bfloat16><<<grid, 256, 0, stream>>>(
         static_cast<const __nv_bfloat16*>(in), static_cast<__nv_bfloat16*>(out), N, C, H, W, Cpad);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("nchw_to_nhwc_pad_kernel");
+  B2F_LAUNCHED("nchw_to_nhwc_pad_kernel", 1);
   return B2F_OK;
 }
 
-int softmax_rows(void* s, int64_t ld, int rows, int L, float scale, cudaStream_t stream) {
+extern "C" int b2f_softmax_rows(void* s, int64_t ld, int rows, int L, float scale, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!s || rows <= 0 || L <= 0 || (L & 7) || (ld & 7)) return B2F_ERR_INVALID;
   prof_begin(KC_OTHER, stream);
   softmax_rows_kernel<<<rows, 256, 0, stream>>>(static_cast<__nv_bfloat16*>(s), ld, L, scale);
   prof_end(KC_OTHER, stream, 0.0, 4.0 * (double)rows * L);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("softmax_rows_kernel");
+  B2F_LAUNCHED("softmax_rows_kernel", 1);
   return B2F_OK;
 }
 
-int transpose_bf16(const void* in, int64_t ld_in, void* out, int64_t ld_out, int R, int Cc,
-                   cudaStream_t stream) {
+extern "C" int b2f_transpose_bf16(const void* in, int64_t ld_in, void* out, int64_t ld_out, int R, int Cc,
+                                  b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!in || !out || R <= 0 || Cc <= 0) return B2F_ERR_INVALID;
   dim3 grid((Cc + 31) / 32, (R + 31) / 32);
   transpose_kernel<<<grid, 256, 0, stream>>>(static_cast<const __nv_bfloat16*>(in), ld_in,
                                              static_cast<__nv_bfloat16*>(out), ld_out, R, Cc);
-  g_launch_count.fetch_add(1, std::memory_order_relaxed);
-  B2F_CHECK_LAUNCH("transpose_kernel");
+  B2F_LAUNCHED("transpose_kernel", 1);
   return B2F_OK;
 }
 

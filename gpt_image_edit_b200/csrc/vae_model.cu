@@ -13,21 +13,6 @@
 
 namespace b2f {
 
-int gemm_bf16(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
-              const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N,
-              int K, int epilogue, const void* resid, int64_t ldr, int64_t resid_bs, const void* gate,
-              int64_t gate_ld, cudaStream_t stream);
-int conv3x3(const void* in, const void* w, const void* bias, void* out, const void* resid, int N,
-            int Hin, int Win, int Cin, int Cout, int stride, int out_nchw, cudaStream_t stream);
-int groupnorm_silu(const void* x, const void* gamma, const void* beta, void* y, double* stats_ws,
-                   int N, long long P, int C, float eps, int silu, cudaStream_t stream);
-int upsample2x(const void* in, void* out, int N, int H, int W, int C, cudaStream_t stream);
-int nchw_to_nhwc_pad(const void* in, int in_is_f32, void* out, int N, int C, int H, int W, int Cpad,
-                     cudaStream_t stream);
-int softmax_rows(void* s, int64_t ld, int rows, int L, float scale, cudaStream_t stream);
-int transpose_bf16(const void* in, int64_t ld_in, void* out, int64_t ld_out, int R, int Cc,
-                   cudaStream_t stream);
-
 typedef uint16_t bf16_t;
 
 struct VaeCtx {
@@ -60,12 +45,12 @@ struct VaeRun {
   }
   void gn(const std::string& name, const bf16_t* x, bf16_t* y, long long P, int C, int silu) {
     if (rc) return;
-    run(groupnorm_silu(x, w(name + ".weight"), w(name + ".bias"), y, stats, N, P, C, 1e-6f, silu, st));
+    run(b2f_groupnorm_silu(x, w(name + ".weight"), w(name + ".bias"), y, stats, N, P, C, 1e-6f, silu, st));
   }
   void conv(const std::string& name, const bf16_t* in, bf16_t* out, const bf16_t* resid, int H, int W,
             int Cin, int Cout, int stride = 1, int nchw = 0) {
     if (rc) return;
-    run(conv3x3(in, w(name + ".weight"), w(name + ".bias"), out, resid, N, H, W, Cin, Cout, stride, nchw, st));
+    run(b2f_conv3x3(in, w(name + ".weight"), w(name + ".bias"), out, resid, N, H, W, Cin, Cout, stride, nchw, st));
   }
   // ResnetBlock2D in place on X: X[N,H,W,Cin] -> X[N,H,W,Cout]
   void resnet(const std::string& name, int H, int W, int Cin, int Cout) {
@@ -75,8 +60,8 @@ struct VaeRun {
     gn(name + ".norm2", B, A, P, Cout, 1);
     if (Cin != Cout) {
       if (rc) return;
-      run(gemm_bf16(X, Cin, 0, w(name + ".conv_shortcut.weight"), Cin, w(name + ".conv_shortcut.bias"), B,
-                    Cout, 0, 1, (int)(N * P), Cout, Cin, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
+      run(b2f_gemm_bf16(X, Cin, 0, w(name + ".conv_shortcut.weight"), Cin, w(name + ".conv_shortcut.bias"), B,
+                        Cout, 0, 1, (int)(N * P), Cout, Cin, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
       conv(name + ".conv2", A, X, B, H, W, Cout, Cout);
     } else {
       conv(name + ".conv2", A, X, X, H, W, Cout, Cout);
@@ -98,15 +83,15 @@ struct VaeRun {
     for (int n = 0; n < N && !rc; ++n) {
       bf16_t* xa = A + (long long)n * P * C;
       bf16_t* xx = X + (long long)n * P * C;
-      run(gemm_bf16(xa, C, 0, wqkv, C, bqkv, qkv, 3 * C, 0, 1, (int)P, 3 * C, C, B2F_EPI_BIAS, nullptr, 0, 0,
-                    nullptr, 0, st));
-      run(gemm_bf16(qkv, 3 * C, 0, qkv + C, 3 * C, nullptr, S, P, 0, 1, (int)P, (int)P, C, B2F_EPI_BIAS,
-                    nullptr, 0, 0, nullptr, 0, st));
-      run(softmax_rows(S, P, (int)P, (int)P, scale, st));
-      run(transpose_bf16(qkv + 2 * C, 3 * C, vT, P, (int)P, C, st));
-      run(gemm_bf16(S, P, 0, vT, P, nullptr, xa, C, 0, 1, (int)P, C, (int)P, B2F_EPI_BIAS, nullptr, 0, 0,
-                    nullptr, 0, st));
-      run(gemm_bf16(xa, C, 0, wo, C, bo, xx, C, 0, 1, (int)P, C, C, B2F_EPI_RESID, xx, C, 0, nullptr, 0, st));
+      run(b2f_gemm_bf16(xa, C, 0, wqkv, C, bqkv, qkv, 3 * C, 0, 1, (int)P, 3 * C, C, B2F_EPI_BIAS, nullptr, 0, 0,
+                        nullptr, 0, st));
+      run(b2f_gemm_bf16(qkv, 3 * C, 0, qkv + C, 3 * C, nullptr, S, P, 0, 1, (int)P, (int)P, C, B2F_EPI_BIAS,
+                        nullptr, 0, 0, nullptr, 0, st));
+      run(b2f_softmax_rows(S, P, (int)P, (int)P, scale, st));
+      run(b2f_transpose_bf16(qkv + 2 * C, 3 * C, vT, P, (int)P, C, st));
+      run(b2f_gemm_bf16(S, P, 0, vT, P, nullptr, xa, C, 0, 1, (int)P, C, (int)P, B2F_EPI_BIAS, nullptr, 0, 0,
+                        nullptr, 0, st));
+      run(b2f_gemm_bf16(xa, C, 0, wo, C, bo, xx, C, 0, 1, (int)P, C, C, B2F_EPI_RESID, xx, C, 0, nullptr, 0, st));
     }
   }
   void mid(const std::string& name, int H, int W, int C) {
@@ -200,7 +185,7 @@ int b2f_vae_encode(b2f_vae* h, const void* image_nchw, int image_is_f32, int N, 
   int rc = vae_setup(c, &r, N, H, W, ws, ws_bytes, st);
   if (rc) return rc;
   const b2f_vae_cfg& g = c->cfg;
-  r.run(nchw_to_nhwc_pad(image_nchw, image_is_f32, r.A, N, g.in_channels, H, W, 64, st));
+  r.run(b2f_nchw_to_nhwc_pad(image_nchw, image_is_f32, r.A, N, g.in_channels, H, W, 64, st));
   r.conv("encoder.conv_in", r.A, r.X, nullptr, H, W, 64, g.block_out[0]);
   int ch = g.block_out[0], hh = H, ww = W;
   for (int i = 0; i < 4; ++i) {
@@ -234,7 +219,7 @@ static int vae_decode_impl(b2f_vae* h, const void* z_nchw, int N, int h_lat, int
   int rc = vae_setup(c, &r, N, H, W, ws, ws_bytes, st);
   if (rc) return rc;
   const b2f_vae_cfg& g = c->cfg;
-  r.run(nchw_to_nhwc_pad(z_nchw, 0, r.A, N, g.latent_channels, h_lat, w_lat, 64, st));
+  r.run(b2f_nchw_to_nhwc_pad(z_nchw, 0, r.A, N, g.latent_channels, h_lat, w_lat, 64, st));
   int ch = g.block_out[3], hh = h_lat, ww = w_lat;
   r.conv("decoder.conv_in", r.A, r.X, nullptr, hh, ww, 64, ch);
   r.mid("decoder.mid_block", hh, ww, ch);
@@ -245,7 +230,7 @@ static int vae_decode_impl(b2f_vae* h, const void* z_nchw, int N, int h_lat, int
       ch = co;
     }
     if (i != 3) {
-      r.run(upsample2x(r.X, r.A, N, hh, ww, ch, st));
+      r.run(b2f_upsample2x(r.X, r.A, N, hh, ww, ch, st));
       hh *= 2;
       ww *= 2;
       r.conv("decoder.up_blocks." + std::to_string(i) + ".upsamplers.0.conv", r.A, r.X, nullptr, hh, ww, ch, ch);

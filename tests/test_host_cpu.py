@@ -8,6 +8,10 @@ import torch
 
 
 def test_library_loads_and_exports_every_declared_symbol():
+    """libb2f.so exports exactly the functions include/b2f.h declares, and every declaration has a ctypes binding."""
+    import shutil
+    import subprocess
+
     from gpt_image_edit_b200 import _lib
 
     declared = _lib.declared_symbols()
@@ -15,6 +19,11 @@ def test_library_loads_and_exports_every_declared_symbol():
     for name in declared:
         assert hasattr(_lib.lib, name), f"libb2f.so does not export {name}"
     assert set(declared) == set(_lib._SIGNATURES), "ctypes signatures out of sync with include/b2f.h"
+    if shutil.which("nm") is None:
+        pytest.skip("binutils nm not installed")
+    out = subprocess.run(["nm", "-D", "--defined-only", str(_lib.LIB_PATH)], capture_output=True, text=True, check=True)
+    exported = {line.split()[-1] for line in out.stdout.splitlines() if line.strip()}
+    assert exported == set(declared), (sorted(exported - set(declared)), sorted(set(declared) - exported))
     assert _lib.lib.b2f_version() >= 1
     assert _lib.lib.b2f_strerror(-5).decode() == "no sm_90 device"
 

@@ -143,12 +143,15 @@ def test_lora_gemm_qkv_norm_rope(extra):
 
 def test_lora_fuse_kernel():
     """W' = bf16(W + sum_k fp32(B_k s_k) A_k): within one bf16 rounding of the fp64 merge."""
-    from gpt_image_edit_b200 import ops
+    from gpt_image_edit_b200 import _lib, ops
     g = _g(400)
     w = _bf(300, 200, g=g, scale=0.05)
     acat, bcat, cs = _adapters(200, 300, (16, 5), (1.0, -2.0), g)
     w2 = w.clone()
-    ops.lora_fuse_(w2, bcat[:, :21].contiguous(), acat[:21].contiguous(), cs[:21].contiguous(), cs_mul=0.5)
+    b_, a_, c_ = bcat[:, :21].contiguous(), acat[:21].contiguous(), cs[:21].contiguous()
+    n0 = _lib.launch_count()
+    ops.lora_fuse_(w2, b_, a_, c_, cs_mul=0.5)
+    assert _lib.launch_count() - n0 == 1, "a fuse is one kernel launch and b2f_launch_count counts it"
     ref = R.d64(w) + R.d64(bcat[:, :21]) @ (R.d64(acat[:21]) * (cs[:21] * 0.5).double()[:, None])
     d = R.ulp_diff(w2, ref, R.acc_floor(21, R.d64(bcat[:, :21]).abs() @ R.d64(acat[:21]).abs()))
     assert d.max().item() <= 1.0, d.max().item()
