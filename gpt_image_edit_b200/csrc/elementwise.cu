@@ -53,13 +53,37 @@ struct LnModParams {
   int split_row;
   const __nv_bfloat16* scale_b;
   const __nv_bfloat16* shift_b;
+  // FP8 output (b2f_ln_modulate_fp8): `out` holds e4m3 bytes (pitches in bytes), one fp32 scale per row
+  float* row_scale;
+  long long row_scale_bs;
 };
+
+__device__ __forceinline__ float warp_max(float v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
+  return v;
+}
+// amax of 8 packed bf16 values (exact: |x| of a bf16 value is a bf16 value)
+__device__ __forceinline__ float amax8(const uint4 q, float m) {
+  const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    m = fmax3(m, fabsf(__uint_as_float(w[j] << 16)), fabsf(__uint_as_float(w[j] & 0xffff0000u)));
+  return m;
+}
+// The row rule of include/b2f.h: (scale, inverse) of a row whose amax is `amax`; an all-zero row gets (1, 0).
+__device__ __forceinline__ void row_scale_of(float amax, float& s, float& inv) {
+  s = amax > 0.f ? __fdiv_rn(amax, 448.0f) : 1.0f;
+  inv = amax > 0.f ? __fdiv_rn(448.0f, amax) : 0.0f;
+}
 
 // One warp per row, rows taken grid-stride.  The row stays PACKED in registers (MAXC uint4 per lane, 48 registers
 // for D = 3072) and is unpacked again in each of the three passes (sum, centred sum of squares, output): with the
 // 96-float copy the kernel ran at 16 warps per SM and 2.5 TB/s in the denoising loop; packed it fits 6 blocks of
 // 4 warps per SM, i.e. twice the bytes in flight.
-template <int MAXC>
+// FP8 = true (b2f_ln_modulate_fp8): the modulated bf16 row replaces the input row in registers, then one warp amax and
+// the row rule write e4m3 bytes and the row's scale instead of the bf16 row.
+template <int MAXC, bool FP8 = false>
 __global__ void __launch_bounds__(128, 6) ln_modulate_kernel(const LnModParams p) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long total = (long long)p.batch * p.rows;
@@ -127,9 +151,64 @@ __global__ void __launch_bounds__(128, 6) ln_modulate_kernel(const LnModParams p
           const __nv_bfloat162 r2 = __hadd2_rn(z, *reinterpret_cast<const __nv_bfloat162*>(&h[j]));      // bf16(z + shift)
           o[j] = *reinterpret_cast<const uint32_t*>(&r2);
         }
-        *reinterpret_cast<uint4*>(orow + c * 256 + lane * 8) = make_uint4(o[0], o[1], o[2], o[3]);
+        if constexpr (FP8)
+          q[c] = make_uint4(o[0], o[1], o[2], o[3]);
+        else
+          *reinterpret_cast<uint4*>(orow + c * 256 + lane * 8) = make_uint4(o[0], o[1], o[2], o[3]);
       }
     }
+    if constexpr (FP8) {
+      float m = 0.f;
+#pragma unroll
+      for (int c = 0; c < MAXC; ++c)
+        if (c < nchunk) m = amax8(q[c], m);
+      float s, inv;
+      row_scale_of(warp_max(m), s, inv);
+      uint8_t* orow8 = reinterpret_cast<uint8_t*>(p.out) + b * p.out_batch_stride + r * p.ldo;
+#pragma unroll
+      for (int c = 0; c < MAXC; ++c) {
+        if (c < nchunk) {
+          float v[8];
+          unpack8(q[c], v);
+          *reinterpret_cast<uint2*>(orow8 + c * 256 + lane * 8) = inv > 0.f ? quant_e4m3x8(v, inv) : make_uint2(0, 0);
+        }
+      }
+      if (lane == 0) p.row_scale[b * p.row_scale_bs + r] = s;
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// Row quantization to e4m3 (include/b2f.h, b2f_quant_fp8_rows): one warp per row of K bf16 values (K % 16 == 0), 8
+// values per lane and step.  The first pass takes the amax, the second re-reads the row (from L1 / L2) and converts.
+struct QuantParams {
+  const __nv_bfloat16* x;
+  long long ldx, x_bs;
+  uint8_t* q;
+  long long ldq, q_bs;
+  float* scale;
+  long long scale_bs;
+  int batch, rows, K;
+};
+
+__global__ void __launch_bounds__(256) quant_fp8_rows_kernel(const QuantParams p) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long long total = (long long)p.batch * p.rows;
+  for (long long grow = (long long)blockIdx.x * 8 + warp; grow < total; grow += (long long)gridDim.x * 8) {
+    const int b = int(grow / p.rows);
+    const int r = int(grow - (long long)b * p.rows);
+    const __nv_bfloat16* xr = p.x + b * p.x_bs + r * p.ldx;
+    float m = 0.f;
+    for (int k = lane * 8; k < p.K; k += 256) m = amax8(*reinterpret_cast<const uint4*>(xr + k), m);
+    float s, inv;
+    row_scale_of(warp_max(m), s, inv);
+    uint8_t* qr = p.q + b * p.q_bs + r * p.ldq;
+    for (int k = lane * 8; k < p.K; k += 256) {
+      float v[8];
+      unpack8(*reinterpret_cast<const uint4*>(xr + k), v);
+      *reinterpret_cast<uint2*>(qr + k) = inv > 0.f ? quant_e4m3x8(v, inv) : make_uint2(0, 0);   // +0, not -0 * 0
+    }
+    if (lane == 0) p.scale[b * p.scale_bs + r] = s;
   }
 }
 
@@ -352,7 +431,8 @@ extern "C" int b2f_ln_modulate(const void* x, int64_t ldx, int64_t x_batch_strid
   LnModParams p{static_cast<const __nv_bfloat16*>(x), ldx, x_batch_stride,
                 static_cast<const __nv_bfloat16*>(scale), static_cast<const __nv_bfloat16*>(shift),
                 mod_ld, static_cast<__nv_bfloat16*>(out), ldo, out_batch_stride, batch, rows, D, eps,
-                split_row, static_cast<const __nv_bfloat16*>(scale_b), static_cast<const __nv_bfloat16*>(shift_b)};
+                split_row, static_cast<const __nv_bfloat16*>(scale_b), static_cast<const __nv_bfloat16*>(shift_b),
+                nullptr, 0};
   if (split_row > 0 && (!scale_b || !shift_b)) return B2F_ERR_INVALID;
   const long long total = (long long)batch * rows;
   // grid-stride rows: at most 12 four-row blocks per SM (two generations of the 6 resident ones)
@@ -371,6 +451,61 @@ extern "C" int b2f_ln_modulate(const void* x, int64_t ldx, int64_t x_batch_strid
   else
     ln_modulate_kernel<LN_MAXC><<<grid, 128, 0, stream>>>(p);
   B2F_LAUNCHED("ln_modulate_kernel", 1);
+  return B2F_OK;
+}
+
+extern "C" int b2f_ln_modulate_fp8(const void* x, int64_t ldx, int64_t x_batch_stride, const void* scale,
+                                   const void* shift, int64_t mod_ld, void* out, int64_t ldo, int64_t out_batch_stride,
+                                   float* row_scale, int64_t row_scale_batch_stride, int batch, int rows, int D,
+                                   float eps, int split_row, const void* scale_b, const void* shift_b,
+                                   b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!device_info().ok) return B2F_ERR_NODEVICE;
+  if (!x || !scale || !shift || !out || !row_scale || batch <= 0 || rows <= 0) return B2F_ERR_INVALID;
+  if (D <= 0 || (D & 255) || D > 3072) return B2F_ERR_UNSUPPORTED;   // the 20-chunk row (D > 3072) would spill
+  if ((ldx & 7) || (ldo & 15) || (mod_ld & 7) || (x_batch_stride & 7) || (out_batch_stride & 15) ||
+      (reinterpret_cast<uintptr_t>(out) & 15) || (reinterpret_cast<uintptr_t>(row_scale) & 3))
+    return B2F_ERR_ALIGN;
+  if (split_row > 0 && (!scale_b || !shift_b)) return B2F_ERR_INVALID;
+  LnModParams p{static_cast<const __nv_bfloat16*>(x), ldx, x_batch_stride,
+                static_cast<const __nv_bfloat16*>(scale), static_cast<const __nv_bfloat16*>(shift),
+                mod_ld, static_cast<__nv_bfloat16*>(out), ldo, out_batch_stride, batch, rows, D, eps,
+                split_row, static_cast<const __nv_bfloat16*>(scale_b), static_cast<const __nv_bfloat16*>(shift_b),
+                row_scale, row_scale_batch_stride};
+  const long long total = (long long)batch * rows;
+  const long long want = (total + 3) / 4;
+  const long long cap = (long long)device_info().num_sms * 12;
+  const unsigned grid = (unsigned)(want < cap ? want : cap);
+  prof_begin(KC_LNMOD, stream);
+  if (D <= 1024)
+    ln_modulate_kernel<4, true><<<grid, 128, 0, stream>>>(p);
+  else
+    ln_modulate_kernel<12, true><<<grid, 128, 0, stream>>>(p);
+  prof_end(KC_LNMOD, stream, 0.0, 3.0 * (double)total * D + 4.0 * total);
+  B2F_LAUNCHED("ln_modulate_kernel<fp8>", 1);
+  return B2F_OK;
+}
+
+extern "C" int b2f_quant_fp8_rows(const void* x, int64_t ldx, int64_t x_batch_stride, void* q, int64_t ldq,
+                                  int64_t q_batch_stride, float* scale, int64_t scale_batch_stride, int batch, int rows,
+                                  int K, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!device_info().ok) return B2F_ERR_NODEVICE;
+  if (!x || !q || !scale || batch <= 0 || rows <= 0 || K <= 0) return B2F_ERR_INVALID;
+  if ((K & 15) || (ldx & 7) || (x_batch_stride & 7) || (ldq & 15) || (q_batch_stride & 15) ||
+      ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(q)) & 15) ||
+      (reinterpret_cast<uintptr_t>(scale) & 3))
+    return B2F_ERR_ALIGN;
+  QuantParams p{static_cast<const __nv_bfloat16*>(x), ldx, x_batch_stride, static_cast<uint8_t*>(q), ldq,
+                q_batch_stride, scale, scale_batch_stride, batch, rows, K};
+  const long long total = (long long)batch * rows;
+  const long long want = (total + 7) / 8;
+  const long long cap = (long long)device_info().num_sms * 16;
+  const unsigned grid = (unsigned)(want < cap ? want : cap);
+  prof_begin(KC_OTHER, stream);
+  quant_fp8_rows_kernel<<<grid, 256, 0, stream>>>(p);
+  prof_end(KC_OTHER, stream, 0.0, 3.0 * (double)total * K + 4.0 * total);
+  B2F_LAUNCHED("quant_fp8_rows_kernel", 1);
   return B2F_OK;
 }
 

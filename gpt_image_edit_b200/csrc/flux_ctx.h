@@ -21,6 +21,9 @@ struct Lin {
   const bf16_t* w = nullptr;
   const bf16_t* b = nullptr;
   LoraBind lora;
+  // FP8 copy of w (b2f_flux_bind_fp8; block linears only): e4m3 [out, in] and fp32 per-channel scales [out]
+  const uint8_t* w8 = nullptr;
+  const float* ws = nullptr;
 };
 // LoRA of one AdaLN linear: rows [row0, row0 + rows) of the fused adaln weight
 struct AdalnLora {
@@ -55,6 +58,8 @@ struct FluxCtx {
   float lora_scale = 1.f;
   int lora_count = 0;
   int lora_rmax() const;
+  // b2f_flux_set_fp8: the block linears of b2f_flux_forward run in FP8
+  bool fp8 = false;
   // fp32 gradient buffers of the trainable tensors, bound by name (flux_train.cu); an unbound name is frozen
   std::map<std::string, std::pair<float*, int64_t>> grads;
 };

@@ -95,13 +95,26 @@ static int adaln_rmax(const FluxCtx* c) {
   return r;
 }
 
+// The e4m3 rows and per-token scales standing in for a block linear's bf16 input A while FP8 is on (b2f_flux_set_fp8).
+struct Q8 {
+  const uint8_t* a;
+  int64_t lda, a_bs;
+  const float* s;
+  int64_t s_bs;
+};
+
 // A linear layer of the forward with its unfused LoRA, if one is bound:
 //   T = bf16(colscale * cs_mul * (A Acat^T))  into tb [batch, M, r_pad]    (gemm_colscale)
 //   out = epi(A W^T + T Bcat^T + bias)                                      (gemm_bf16_lora: r_pad / 64 more k-blocks)
-// Without one it is exactly the plain gemm_bf16 launch.
+// Without one it is exactly the plain gemm_bf16 launch.  With q8 (FP8 on; no adapter can be bound then) it is the FP8
+// launch on (q8, w8).
 static int lin_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_t lda, int64_t a_bs, int64_t ldw,
                    void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epi, const void* resid,
-                   int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld, cudaStream_t st) {
+                   int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld, cudaStream_t st,
+                   const Q8* q8 = nullptr) {
+  if (q8)
+    return b2f_gemm_fp8(q8->a, q8->lda, q8->a_bs, q8->s, q8->s_bs, l.w8, K, l.ws, l.b, out, ldc, out_bs, batch, M, N, K,
+                        epi, resid, ldr, resid_bs, gate, gate_ld, st);
   if (!l.lora.A)
     return b2f_gemm_bf16(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, N, K, epi, resid, ldr, resid_bs, gate,
                          gate_ld, st);
@@ -115,7 +128,12 @@ static int lin_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_
 static int qkv_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_t lda, int64_t a_bs, int64_t ldw,
                    void* out, int64_t ldc, int64_t out_bs, int batch, int M, int d_model, int K, const void* nw_q,
                    const void* nw_k, const float* cos, const float* sin, int rope_row0, float eps, int n_extra,
-                   void* out_extra, int64_t ld_extra, int64_t bs_extra, int epi_extra, cudaStream_t st) {
+                   void* out_extra, int64_t ld_extra, int64_t bs_extra, int epi_extra, cudaStream_t st,
+                   const Q8* q8 = nullptr) {
+  if (q8)
+    return b2f_gemm_qkv_norm_rope_fp8(q8->a, q8->lda, q8->a_bs, q8->s, q8->s_bs, l.w8, K, l.ws, l.b, out, ldc, out_bs,
+                                      batch, M, d_model, K, nw_q, nw_k, cos, sin, rope_row0, eps, n_extra, out_extra,
+                                      ld_extra, bs_extra, epi_extra, st);
   if (!l.lora.A)
     return b2f_gemm_qkv_norm_rope(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, d_model, K, nw_q, nw_k, cos,
                                   sin, rope_row0, eps, n_extra, out_extra, ld_extra, bs_extra, epi_extra, st);
@@ -126,6 +144,16 @@ static int qkv_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_
   return b2f_gemm_qkv_norm_rope_lora(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, d_model, K, nw_q, nw_k, cos,
                                      sin, rope_row0, eps, n_extra, out_extra, ld_extra, bs_extra, epi_extra, tb, r, t_bs,
                                      l.lora.Bc, r, r, st);
+}
+
+// The ten FP8-capable linears of each block (b2f_flux_bind_fp8): every linear of for_each_linear inside a block that is
+// not an AdaLN linear.
+template <class F>
+static void for_each_block_linear(FluxCtx* c, F&& f) {
+  for_each_linear(c, [&](const std::string& name, Lin* l, int64_t, int64_t out_f, int64_t in_f) {
+    if (l && (name.rfind("transformer_blocks.", 0) == 0 || name.rfind("single_transformer_blocks.", 0) == 0))
+      f(name, l, out_f, in_f);
+  });
 }
 
 int FluxCtx::lora_rmax() const {
@@ -229,11 +257,12 @@ int b2f_flux_finalize(b2f_flux* h) {
   }
 #undef EL
 #undef EW
-  // (re)binding weights drops every LoRA binding
+  // (re)binding weights drops every LoRA binding (the FP8 ones went with the reassigned block weights)
   for_each_linear(c, [](const std::string&, Lin* l, int64_t, int64_t, int64_t) {
     if (l) l->lora = LoraBind();
   });
   c->adaln_lora.clear();
+  c->fp8 = false;
   c->finalized = true;
   return B2F_OK;
 }
@@ -252,8 +281,10 @@ size_t b2f_flux_workspace_bytes(const b2f_flux* h, int B, int S_img, int S_txt) 
   const FluxCtx* c = reinterpret_cast<const FluxCtx*>(h);
   if (!c || B <= 0 || S_img <= 0 || S_txt < 0) return 0;
   const size_t S = (size_t)S_img + S_txt;
-  // h[d] + xn[d] + qkv[3d] + cat[5d] per token, bf16; with unfused LoRA adapters bound, T[r_pad] per token
-  return (size_t)B * S * ((size_t)c->d * 10 + (size_t)c->lora_rmax()) * 2 + 1024;
+  // h[d] + xn[d] + qkv[3d] + cat[5d] per token, bf16; with unfused LoRA adapters bound, T[r_pad] per token; with FP8
+  // on, e4m3 q8[5d] and an fp32 scale per token
+  const size_t fp8 = c->fp8 ? (size_t)B * S * ((size_t)c->d * 5 + 4) + 256 : 0;
+  return (size_t)B * S * ((size_t)c->d * 10 + (size_t)c->lora_rmax()) * 2 + 1024 + fp8;
 }
 
 size_t b2f_flux_temb_workspace_bytes(const b2f_flux* h, int rows) {
@@ -359,6 +390,10 @@ int b2f_flux_bind_lora(b2f_flux* h, const char* target, const void* Acat, const 
   FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
   if (!c || !c->finalized || !target) return B2F_ERR_INVALID;
   const bool unbind = Acat == nullptr;
+  if (!unbind && c->fp8) {
+    fprintf(stderr, "[b2f] flux_bind_lora: FP8 is on; fuse the adapter or switch FP8 off first\n");
+    return B2F_ERR_UNSUPPORTED;
+  }
   if (!unbind) {
     if (!Bcat || !colscale || r_pad <= 0 || r_pad % 64) return B2F_ERR_INVALID;
     if ((reinterpret_cast<uintptr_t>(Acat) | reinterpret_cast<uintptr_t>(Bcat) |
@@ -413,6 +448,57 @@ int b2f_flux_set_lora_scale(b2f_flux* h, float scale) {
   return B2F_OK;
 }
 
+int b2f_flux_bind_fp8(b2f_flux* h, const char* name, const void* w8, const float* w_scale, int64_t numel) {
+  FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
+  if (!c || !c->finalized || !name) return B2F_ERR_INVALID;
+  if (w8 && !w_scale) return B2F_ERR_INVALID;
+  if ((reinterpret_cast<uintptr_t>(w8) | reinterpret_cast<uintptr_t>(w_scale)) & 15) return B2F_ERR_ALIGN;
+  if (!w8 && c->fp8) {
+    fprintf(stderr, "[b2f] flux_bind_fp8: cannot unbind '%s' while FP8 is on\n", name);
+    return B2F_ERR_INVALID;
+  }
+  const std::string key(name);
+  int rc = B2F_ERR_INVALID;
+  bool found = false;
+  for_each_block_linear(c, [&](const std::string& n, Lin* l, int64_t out_f, int64_t in_f) {
+    if (found || n != key) return;
+    found = true;
+    if (w8 && numel != out_f * in_f) {
+      fprintf(stderr, "[b2f] flux_bind_fp8: '%s' has %lld elements, expected %lld\n", name, (long long)numel,
+              (long long)(out_f * in_f));
+      return;
+    }
+    l->w8 = static_cast<const uint8_t*>(w8);
+    l->ws = w8 ? w_scale : nullptr;
+    rc = B2F_OK;
+  });
+  if (!found) fprintf(stderr, "[b2f] flux_bind_fp8: no block linear named '%s'\n", name);
+  return rc;
+}
+
+int b2f_flux_set_fp8(b2f_flux* h, int on) {
+  FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
+  if (!c || !c->finalized) return B2F_ERR_INVALID;
+  if (!on) {
+    c->fp8 = false;
+    return B2F_OK;
+  }
+  if (c->lora_rmax() > 0) {
+    fprintf(stderr, "[b2f] flux_set_fp8: unfused LoRA adapters are bound; fuse or unbind them first\n");
+    return B2F_ERR_UNSUPPORTED;
+  }
+  int rc = B2F_OK;
+  for_each_block_linear(c, [&](const std::string& n, Lin* l, int64_t, int64_t) {
+    if (!rc && !l->w8) {
+      fprintf(stderr, "[b2f] flux_set_fp8: no FP8 weight bound for '%s'\n", n.c_str());
+      rc = B2F_ERR_INVALID;
+    }
+  });
+  if (rc) return rc;
+  c->fp8 = true;
+  return B2F_OK;
+}
+
 int b2f_flux_lora_rank(const b2f_flux* h) {
   const FluxCtx* c = reinterpret_cast<const FluxCtx*>(h);
   return c && c->finalized ? c->lora_rmax() : 0;
@@ -447,6 +533,20 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
   bf16_t* qkv = xn + BS * d;       // [B,S,3d]
   bf16_t* cat = qkv + BS * 3 * d;  // [B,S,5d]
   bf16_t* tb = cat + BS * 5 * d;   // LoRA T [B,S,r_pad] (only with adapters bound)
+  // FP8 on: e4m3 rows q8 [B,S,5d] (pitch 5d bytes) and their scales qs [B,S], rewritten before each block linear
+  uint8_t* q8 = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tb + BS * c->lora_rmax()) + 255) &
+                                           ~uintptr_t(255));
+  float* qs = reinterpret_cast<float*>(q8 + BS * 5 * d);
+  const bool f8 = c->fp8;
+  const int64_t q8_bs = (int64_t)S * 5 * d;
+  const Q8 q_txt{q8, 5 * d, q8_bs, qs, S};
+  const Q8 q_img{q8 + (int64_t)S_txt * 5 * d, 5 * d, q8_bs, qs + S_txt, S};
+  const Q8* qt = f8 ? &q_txt : nullptr;   // the text rows (a single block: all rows) of q8
+  const Q8* qi = f8 ? &q_img : nullptr;
+  // (K columns of cat from column c0) -> q8 over all S rows
+  auto quant_cat = [&](int64_t c0, int K) {
+    return b2f_quant_fp8_rows(cat + c0, 5 * d, (int64_t)S * 5 * d, q8, 5 * d, q8_bs, qs, S, B, S, K, st);
+  };
   const float ls = c->lora_scale;
   const int64_t h_bs = (int64_t)S * d, qkv_bs = (int64_t)S * 3 * d, cat_bs = (int64_t)S * 5 * d;
   bf16_t* h_img = hb + (int64_t)S_txt * d;
@@ -480,45 +580,64 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
       const bf16_t* mi = modp + (int64_t)blk * 12 * d;
       const bf16_t* mt = mi + 6 * d;
       // both streams in one launch over the joint buffer: text rows use the context modulation
-      RUN(b2f_ln_modulate(hb, d, h_bs, mt + d, mt, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt, mi + d, mi, st));
+      if (f8) {
+        RUN(b2f_ln_modulate_fp8(hb, d, h_bs, mt + d, mt, mod_ld, q8, 5 * d, q8_bs, qs, S, B, S, (int)d, eps, S_txt,
+                                mi + d, mi, st));
+      } else {
+        RUN(b2f_ln_modulate(hb, d, h_bs, mt + d, mt, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt, mi + d, mi, st));
+      }
       // QKV projections with per-head RMSNorm + RoPE fused into the GEMM epilogue; both streams write
       // straight into the joint [txt; img] qkv buffer
       RUN(qkv_fwd(w.qkv, tb, ls, xn_img, d, h_bs, d, qkv_img, 3 * d, qkv_bs, B, S_img, (int)d,
-                             (int)d, w.norm_q, w.norm_k, c->rope_cos, c->rope_sin, S_txt, eps, 0, nullptr, 0, 0, 0, st));
+                             (int)d, w.norm_q, w.norm_k, c->rope_cos, c->rope_sin, S_txt, eps, 0, nullptr, 0, 0, 0, st,
+                             qi));
       RUN(qkv_fwd(w.add_qkv, tb, ls, xn_txt, d, h_bs, d, qkv_txt, 3 * d, qkv_bs, B, S_txt,
                              (int)d, (int)d, w.norm_added_q, w.norm_added_k, c->rope_cos, c->rope_sin, 0, eps, 0,
-                             nullptr, 0, 0, 0, st));
+                             nullptr, 0, 0, 0, st, qt));
       RUN(b2f_attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S,
                             g.head_dim, scale, 0, st));
+      if (f8) RUN(quant_cat(0, (int)d));
       RUN(lin_fwd(w.to_out, tb, ls, cat_img, 5 * d, cat_bs, d, h_img, d, h_bs, B, S_img,
-                    (int)d, (int)d, B2F_EPI_GATE_RESID, h_img, d, h_bs, mi + 2 * d, mod_ld, st));
+                    (int)d, (int)d, B2F_EPI_GATE_RESID, h_img, d, h_bs, mi + 2 * d, mod_ld, st, qi));
       RUN(lin_fwd(w.to_add_out, tb, ls, cat_txt, 5 * d, cat_bs, d, h_txt, d, h_bs, B,
-                    S_txt, (int)d, (int)d, B2F_EPI_GATE_RESID, h_txt, d, h_bs, mt + 2 * d, mod_ld, st));
-      RUN(b2f_ln_modulate(hb, d, h_bs, mt + 4 * d, mt + 3 * d, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt,
-                          mi + 4 * d, mi + 3 * d, st));
+                    S_txt, (int)d, (int)d, B2F_EPI_GATE_RESID, h_txt, d, h_bs, mt + 2 * d, mod_ld, st, qt));
+      if (f8) {
+        RUN(b2f_ln_modulate_fp8(hb, d, h_bs, mt + 4 * d, mt + 3 * d, mod_ld, q8, 5 * d, q8_bs, qs, S, B, S, (int)d, eps,
+                                S_txt, mi + 4 * d, mi + 3 * d, st));
+      } else {
+        RUN(b2f_ln_modulate(hb, d, h_bs, mt + 4 * d, mt + 3 * d, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt,
+                            mi + 4 * d, mi + 3 * d, st));
+      }
       RUN(lin_fwd(w.ff1, tb, ls, xn_img, d, h_bs, d, cat_img + d, 5 * d, cat_bs, B, S_img,
-                    (int)(4 * d), (int)d, B2F_EPI_GELU_TANH, nullptr, 0, 0, nullptr, 0, st));
+                    (int)(4 * d), (int)d, B2F_EPI_GELU_TANH, nullptr, 0, 0, nullptr, 0, st, qi));
       RUN(lin_fwd(w.ffc1, tb, ls, xn_txt, d, h_bs, d, cat_txt + d, 5 * d, cat_bs, B, S_txt,
-                    (int)(4 * d), (int)d, B2F_EPI_GELU_TANH, nullptr, 0, 0, nullptr, 0, st));
+                    (int)(4 * d), (int)d, B2F_EPI_GELU_TANH, nullptr, 0, 0, nullptr, 0, st, qt));
+      if (f8) RUN(quant_cat(d, (int)(4 * d)));
       RUN(lin_fwd(w.ff2, tb, ls, cat_img + d, 5 * d, cat_bs, 4 * d, h_img, d, h_bs, B, S_img,
-                    (int)d, (int)(4 * d), B2F_EPI_GATE_RESID, h_img, d, h_bs, mi + 5 * d, mod_ld, st));
+                    (int)d, (int)(4 * d), B2F_EPI_GATE_RESID, h_img, d, h_bs, mi + 5 * d, mod_ld, st, qi));
       RUN(lin_fwd(w.ffc2, tb, ls, cat_txt + d, 5 * d, cat_bs, 4 * d, h_txt, d, h_bs, B, S_txt,
-                    (int)d, (int)(4 * d), B2F_EPI_GATE_RESID, h_txt, d, h_bs, mt + 5 * d, mod_ld, st));
+                    (int)d, (int)(4 * d), B2F_EPI_GATE_RESID, h_txt, d, h_bs, mt + 5 * d, mod_ld, st, qt));
     } else {
       const int si = blk - g.num_double;
       const SingleW& w = c->sgl[si];
       // mod columns: [shift, scale, gate]
       const bf16_t* ms = modp + (int64_t)g.num_double * 12 * d + (int64_t)si * 3 * d;
-      RUN(b2f_ln_modulate(hb, d, h_bs, ms + d, ms, mod_ld, xn, d, h_bs, B, S, (int)d, eps, 0, nullptr, nullptr, st));
+      if (f8) {
+        RUN(b2f_ln_modulate_fp8(hb, d, h_bs, ms + d, ms, mod_ld, q8, 5 * d, q8_bs, qs, S, B, S, (int)d, eps, 0, nullptr,
+                                nullptr, st));
+      } else {
+        RUN(b2f_ln_modulate(hb, d, h_bs, ms + d, ms, mod_ld, xn, d, h_bs, B, S, (int)d, eps, 0, nullptr, nullptr, st));
+      }
       // ONE launch for [to_q;to_k;to_v;proj_mlp] (N = 7d): Q/K get RMSNorm+RoPE, V passes through into
       // qkv, the MLP columns are GELU'd straight into cat[:, :, d:5d]
       RUN(qkv_fwd(w.qkv_mlp, tb, ls, xn, d, h_bs, d, qkv, 3 * d, qkv_bs, B, S, (int)d, (int)d,
                              w.norm_q, w.norm_k, c->rope_cos, c->rope_sin, 0, eps, (int)(4 * d), cat + d, 5 * d,
-                             cat_bs, B2F_EPI_GELU_TANH, st));
+                             cat_bs, B2F_EPI_GELU_TANH, st, qt));
       RUN(b2f_attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S,
                             g.head_dim, scale, 0, st));
+      if (f8) RUN(quant_cat(0, (int)(5 * d)));
       RUN(lin_fwd(w.proj_out, tb, ls, cat, 5 * d, cat_bs, 5 * d, hb, d, h_bs, B, S, (int)d,
-                    (int)(5 * d), B2F_EPI_GATE_RESID, hb, d, h_bs, ms + 2 * d, mod_ld, st));
+                    (int)(5 * d), B2F_EPI_GATE_RESID, hb, d, h_bs, ms + 2 * d, mod_ld, st, qt));
     }
   }
 

@@ -129,6 +129,10 @@ int b2f_flux_train_forward(b2f_flux* h, const void* hidden, const void* enc, con
     fprintf(stderr, "[b2f] flux_train_forward: unfused LoRA adapters are bound\n");
     return B2F_ERR_UNSUPPORTED;
   }
+  if (c->fp8) {   // training runs the bf16 weights: switch FP8 off first
+    fprintf(stderr, "[b2f] flux_train_forward: FP8 is on\n");
+    return B2F_ERR_UNSUPPORTED;
+  }
   if (ws_bytes < b2f_flux_train_workspace_bytes(h, B, S_img, S_txt)) return B2F_ERR_WORKSPACE;
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   const size_t infer = b2f_flux_workspace_bytes(h, B, S_img, S_txt);
@@ -158,6 +162,10 @@ int b2f_flux_train_backward(b2f_flux* h, const void* dout, const void* mod, int6
   if (!c || !c->finalized || !mod || !silu_temb || !ws || B <= 0 || S_img <= 0 || S_txt <= 0)
     return B2F_ERR_INVALID;
   if (n_out_rows <= 0 || n_out_rows > S_img) return B2F_ERR_INVALID;
+  if (c->fp8) {
+    fprintf(stderr, "[b2f] flux_train_backward: FP8 is on\n");
+    return B2F_ERR_UNSUPPORTED;
+  }
   if (ws_bytes < b2f_flux_train_workspace_bytes(h, B, S_img, S_txt)) return B2F_ERR_WORKSPACE;
   const int S = S_img + S_txt;
   if (!c->rope_cos || c->rope_S != S) return B2F_ERR_INVALID;

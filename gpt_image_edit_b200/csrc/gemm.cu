@@ -7,6 +7,7 @@
 //                                           two m64n128k16 per k16 step, 128 fp32 accumulators per thread
 //                                           (setmaxnreg.inc to 232); named barriers make them take turns on the main
 //                                           loop, so one runs its MMAs while the other runs its epilogue
+//   FP8 mode              e4m3 A and W (per-token / per-channel fp32 scales), m64n128k32 e4m3 wgmma; see Fp8Params
 //   epilogue              x = bf16(acc + bias) from registers → the consumer's own bf16 staging tile →
 //                         act/gate/resid → global with 16-byte accesses, 16 threads per row; a fused QKV head runs one
 //                         thread per row; the fp32 wgrad output goes straight from registers
@@ -270,11 +271,27 @@ struct LoraParams<true> {
   float cs_mul;
 };
 
-template <int MODE, bool LORA = false>
+// FP8 mode (FP8 = true, MODE 0 only, not with LORA): A and W are e4m3 with one fp32 scale per row of A (a_scale, per
+// token) and per row of W (w_scale, per output channel).  A k-block is still 128 bytes of K, now 128 elements, so the
+// ring, the swizzle and the 32-byte descriptor step are unchanged; each k32 step is one m64n128k32 e4m3 wgmma.  The
+// staged value is x = bf16(fmaf(acc, fp32(a_scale[m] * w_scale[n]), bias[n])) (bf16(acc * scale) without a bias), and
+// every epilogue runs from x as in the bf16 kernel.  FP8 = false has an empty parameter and compiles to the plain kernel.
+template <bool FP8>
+struct Fp8Params {};
+template <>
+struct Fp8Params<true> {
+  const float* a_scale;
+  long long a_scale_bs;
+  const float* w_scale;
+};
+
+template <int MODE, bool LORA = false, bool FP8 = false>
 __global__ void __launch_bounds__(THREADS, 1)
 gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-                 const GemmParams p, const __grid_constant__ LoraParams<LORA> lx) {
+                 const GemmParams p, const __grid_constant__ LoraParams<LORA> lx,
+                 const __grid_constant__ Fp8Params<FP8> fx) {
   constexpr int TA = MODE == 2, TB = MODE >= 1;
+  constexpr int KB_ELEMS = FP8 ? BLOCK_K * 2 : BLOCK_K;   // elements of K per 128-byte k-block
   extern __shared__ uint8_t smem_raw[];
   uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(ring + STAGES * STAGE_BYTES + 2 * STAGING_BYTES);
@@ -299,7 +316,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 
   const int num_tiles = p.num_m_blocks * p.num_n_blocks;
   const int n_local = (num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;   // this CTA's tiles
-  const int num_kb = MODE == 2 ? p.kbatch * p.kb_per_batch : (p.K + BLOCK_K - 1) / BLOCK_K;
+  const int num_kb = MODE == 2 ? p.kbatch * p.kb_per_batch : (p.K + KB_ELEMS - 1) / KB_ELEMS;
   int num_kb_all = num_kb;   // k-blocks per tile, the LoRA ones last
   if constexpr (LORA) num_kb_all += lx.num_kb2;
 
@@ -329,7 +346,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           } else {
             const CUtensorMap* mapA = &tmA;
             const CUtensorMap* mapB = &tmB;
-            int kc = kb * BLOCK_K;
+            int kc = kb * KB_ELEMS;
             if constexpr (LORA) {
               if (kb >= num_kb) {   // the LoRA k-blocks: (T, Bcat) in place of (A, W)
                 mapA = &lx.tmT;
@@ -395,8 +412,13 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 #pragma unroll
       for (int k = 0; k < BLOCK_K / 16; ++k) {
         const uint64_t ka = soff + uint64_t((k * A_KSTEP) >> 4), kb16 = soff + uint64_t((k * B_KSTEP) >> 4);
-        wgmma_m64n128_ss<TA, TB>(acc0, da0 + ka, db0 + kb16, 1u);
-        wgmma_m64n128_ss<TA, TB>(acc1, da1 + ka, db0 + kb16, 1u);
+        if constexpr (FP8) {
+          wgmma_m64n128k32_e4m3_ss(acc0, da0 + ka, db0 + kb16, 1u);
+          wgmma_m64n128k32_e4m3_ss(acc1, da1 + ka, db0 + kb16, 1u);
+        } else {
+          wgmma_m64n128_ss<TA, TB>(acc0, da0 + ka, db0 + kb16, 1u);
+          wgmma_m64n128_ss<TA, TB>(acc1, da1 + ka, db0 + kb16, 1u);
+        }
       }
       wgmma_commit();
       wgmma_wait<1>();   // the previous stage's MMAs are complete: hand it back to the producer
@@ -455,6 +477,16 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     }
     // x = bf16(acc + bias) into this consumer's staging tile, once its previous tile's epilogue is done reading it
     named_bar_sync(BAR_EPI + c, 128);
+    float sa[2][2];   // FP8: the token scales of this thread's rows 64 h + r_lo + 8 rr (0 past M)
+    if constexpr (FP8) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          const long long row = (long long)mb * BLOCK_M + 64 * h + r_lo + 8 * rr;
+          sa[h][rr] = row < p.M ? __ldg(fx.a_scale + bb * fx.a_scale_bs + row) : 0.f;
+        }
+    }
 #pragma unroll
     for (int j = 0; j < BLOCK_N / 8; ++j) {
       const int col = 8 * j + 2 * (lane & 3);
@@ -469,27 +501,51 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           cs2.y *= lx.cs_mul;
         }
       }
+      if constexpr (FP8) {
+        const float2 ws2 = n < p.N ? __ldg(reinterpret_cast<const float2*>(fx.w_scale + n)) : make_float2(0.f, 0.f);
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const float* a = h ? acc1 : acc0;
-        float x0 = a[4 * j], x1 = a[4 * j + 1], x2 = a[4 * j + 2], x3 = a[4 * j + 3];
-        if (has_bias) {
-          x0 += b2.x;
-          x1 += b2.y;
-          x2 += b2.x;
-          x3 += b2.y;
-        }
-        if constexpr (LORA) {
-          if (lx.colscale) {
-            x0 *= cs2.x;
-            x1 *= cs2.y;
-            x2 *= cs2.x;
-            x3 *= cs2.y;
+        for (int h = 0; h < 2; ++h) {
+          const float* a = h ? acc1 : acc0;
+          const float s0 = sa[h][0] * ws2.x, s1 = sa[h][0] * ws2.y, s2 = sa[h][1] * ws2.x, s3 = sa[h][1] * ws2.y;
+          float x0, x1, x2, x3;
+          if (has_bias) {
+            x0 = fmaf(a[4 * j], s0, b2.x);
+            x1 = fmaf(a[4 * j + 1], s1, b2.y);
+            x2 = fmaf(a[4 * j + 2], s2, b2.x);
+            x3 = fmaf(a[4 * j + 3], s3, b2.y);
+          } else {
+            x0 = a[4 * j] * s0;
+            x1 = a[4 * j + 1] * s1;
+            x2 = a[4 * j + 2] * s2;
+            x3 = a[4 * j + 3] * s3;
           }
+          uint8_t* s0p = stg + (64 * h + r_lo) * SROW + col * 2;
+          *reinterpret_cast<uint32_t*>(s0p) = pack_bf16x2(x0, x1);
+          *reinterpret_cast<uint32_t*>(s0p + 8 * SROW) = pack_bf16x2(x2, x3);
         }
-        uint8_t* s0 = stg + (64 * h + r_lo) * SROW + col * 2;
-        *reinterpret_cast<uint32_t*>(s0) = pack_bf16x2(x0, x1);
-        *reinterpret_cast<uint32_t*>(s0 + 8 * SROW) = pack_bf16x2(x2, x3);
+      } else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float* a = h ? acc1 : acc0;
+          float x0 = a[4 * j], x1 = a[4 * j + 1], x2 = a[4 * j + 2], x3 = a[4 * j + 3];
+          if (has_bias) {
+            x0 += b2.x;
+            x1 += b2.y;
+            x2 += b2.x;
+            x3 += b2.y;
+          }
+          if constexpr (LORA) {
+            if (lx.colscale) {
+              x0 *= cs2.x;
+              x1 *= cs2.y;
+              x2 *= cs2.x;
+              x3 *= cs2.y;
+            }
+          }
+          uint8_t* s0 = stg + (64 * h + r_lo) * SROW + col * 2;
+          *reinterpret_cast<uint32_t*>(s0) = pack_bf16x2(x0, x1);
+          *reinterpret_cast<uint32_t*>(s0 + 8 * SROW) = pack_bf16x2(x2, x3);
+        }
       }
     }
     named_bar_sync(BAR_EPI + c, 128);
@@ -552,13 +608,14 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 }
 
-template <int MODE, bool LORA = false>
+template <int MODE, bool LORA = false, bool FP8 = false>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream,
-                const LoraParams<LORA>& lx = LoraParams<LORA>{}) {
+                const LoraParams<LORA>& lx = LoraParams<LORA>{}, const Fp8Params<FP8>& fx = Fp8Params<FP8>{}) {
   static_assert(!LORA || MODE == 0, "the LoRA K-extension is forward-only");
+  static_assert(!FP8 || (MODE == 0 && !LORA), "FP8 is a mode of the plain forward GEMM");
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<MODE, LORA>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<MODE, LORA, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          PP_SMEM_BYTES);
     if (e != cudaSuccess) return cuda_err(e, "gemm smem attribute");
     attr_set = true;
@@ -577,16 +634,19 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cu
   }
   const double kk = MODE == 2 ? (double)p.kbatch * p.K : (double)p.K + k_ext;
   prof_begin(KC_GEMM, stream);
-  gemm_bf16_kernel<MODE, LORA><<<grid, THREADS, PP_SMEM_BYTES, stream>>>(tmA, tmB, p, lx);
+  gemm_bf16_kernel<MODE, LORA, FP8><<<grid, THREADS, PP_SMEM_BYTES, stream>>>(tmA, tmB, p, lx, fx);
   {
     char tag_[96];
-    if (LORA)
+    const double ab = FP8 ? 1.0 : 2.0;   // bytes per A / W element
+    if (FP8)
+      snprintf(tag_, sizeof tag_, "gemm fp8 %dx%dx%d b%d e%d", p.M, p.N, p.K, p.batch, p.epi);
+    else if (LORA)
       snprintf(tag_, sizeof tag_, "gemm lora %dx%dx%d+%d b%d e%d%s", p.M, p.N, p.K, k_ext, p.batch, p.epi,
                down ? " down" : "");
     else
       snprintf(tag_, sizeof tag_, "gemm m%d %dx%dx%d b%d e%d", MODE, p.M, p.N, (int)kk, p.batch, p.epi);
     prof_end_tagged(KC_GEMM, stream, 2.0 * p.batch * (double)p.M * p.N * kk,
-                    2.0 * ((double)p.batch * p.M * kk + (double)p.N * kk + (double)p.batch * p.M * p.N), tag_);
+                    ab * ((double)p.batch * p.M * kk + (double)p.N * kk) + 2.0 * (double)p.batch * p.M * p.N, tag_);
   }
   B2F_LAUNCHED("gemm_bf16_kernel", 1);
   return B2F_OK;
@@ -602,6 +662,14 @@ struct QkvExtra {
   int n_extra, epi_extra;   // optional second output block of n_extra columns
   void* out_extra;
   int64_t ld_extra, bs_extra;
+};
+
+// FP8 operands of one forward launch: A and W are e4m3, a_scale fp32 [batch, M] (batch pitch a_scale_bs), w_scale
+// fp32 [N].
+struct Fp8Ext {
+  const float* a_scale;
+  int64_t a_scale_bs;
+  const float* w_scale;
 };
 
 // LoRA operands of one forward launch (see LoraParams): T [batch, M, r_pad] (row pitch ldt, batch pitch t_bs) and
@@ -620,11 +688,18 @@ struct LoraExt {
 static int gemm_bf16_impl(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
               const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N,
               int K, int epilogue, const void* resid, int64_t ldr, int64_t resid_bs, const void* gate,
-              int64_t gate_ld, const QkvExtra* qx, cudaStream_t stream, const LoraExt* lx = nullptr) {
+              int64_t gate_ld, const QkvExtra* qx, cudaStream_t stream, const LoraExt* lx = nullptr,
+              const Fp8Ext* fx = nullptr) {
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (batch <= 0 || M <= 0 || N <= 0 || K <= 0 || !A || !W || !out) return B2F_ERR_INVALID;
   if ((K & 7) || (N & 7) || (lda & 7) || (ldw & 7) || (ldc & 7) || (a_bs & 7) || (out_bs & 7))
     return B2F_ERR_ALIGN;
+  if (fx) {   // byte operands: TMA needs 16-byte pitches
+    if (lx || !fx->a_scale || !fx->w_scale) return B2F_ERR_INVALID;
+    if ((K & 15) || (lda & 15) || (ldw & 15) || (a_bs & 15) || (reinterpret_cast<uintptr_t>(fx->w_scale) & 15) ||
+        (reinterpret_cast<uintptr_t>(fx->a_scale) & 3))
+      return B2F_ERR_ALIGN;
+  }
   if ((reinterpret_cast<uintptr_t>(A) | reinterpret_cast<uintptr_t>(W) |
        reinterpret_cast<uintptr_t>(out) | reinterpret_cast<uintptr_t>(bias) |
        reinterpret_cast<uintptr_t>(resid) | reinterpret_cast<uintptr_t>(gate)) & 15)
@@ -679,8 +754,21 @@ static int gemm_bf16_impl(const void* A, int64_t lda, int64_t a_bs, const void* 
   }
 
   CUtensorMap tmA, tmB;
-  int rc = make_tmap_3d_rows(&tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)batch, (uint64_t)lda,
-                             batch > 1 ? (uint64_t)a_bs : (uint64_t)M * lda);
+  int rc;
+  if (fx) {
+    rc = make_tmap_u8_rows(&tmA, A, 3, (uint64_t)K, (uint64_t)M, (uint64_t)batch, (uint64_t)lda,
+                           batch > 1 ? (uint64_t)a_bs : (uint64_t)M * lda);
+    if (rc != B2F_OK) return rc;
+    rc = make_tmap_u8_rows(&tmB, W, 2, (uint64_t)K, (uint64_t)N, 1, (uint64_t)ldw, 0);
+    if (rc != B2F_OK) return rc;
+    Fp8Params<true> fp;
+    fp.a_scale = fx->a_scale;
+    fp.a_scale_bs = fx->a_scale_bs;
+    fp.w_scale = fx->w_scale;
+    return launch_gemm<0, false, true>(tmA, tmB, p, stream, LoraParams<false>{}, fp);
+  }
+  rc = make_tmap_3d_rows(&tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)batch, (uint64_t)lda,
+                         batch > 1 ? (uint64_t)a_bs : (uint64_t)M * lda);
   if (rc != B2F_OK) return rc;
   rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, BLOCK_N, BLOCK_K);
   if (rc != B2F_OK) return rc;
@@ -800,6 +888,32 @@ extern "C" int b2f_gemm_qkv_norm_rope(const void* A, int64_t lda, int64_t a_bs, 
   QkvExtra qx{nw_q, nw_k, cos, sin, rope_row0, d_model, eps, n_extra, epi_extra, out_extra, ld_extra, bs_extra};
   return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, 3 * d_model + n_extra, K,
                         B2F_EPI_QKV_NORM_ROPE, nullptr, 0, 0, nullptr, 0, &qx, stream);
+}
+
+// ---------------------------------------------------------------------------------------------------- FP8
+// b2f_gemm_bf16 / b2f_gemm_qkv_norm_rope with e4m3 operands and per-token / per-channel fp32 scales (Fp8Params).
+extern "C" int b2f_gemm_fp8(const void* A, int64_t lda, int64_t a_bs, const float* a_scale, int64_t a_scale_bs,
+                            const void* W, int64_t ldw, const float* w_scale, const void* bias, void* out, int64_t ldc,
+                            int64_t out_bs, int batch, int M, int N, int K, int epilogue, const void* resid, int64_t ldr,
+                            int64_t resid_bs, const void* gate, int64_t gate_ld, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (epilogue == B2F_EPI_QKV_NORM_ROPE) return B2F_ERR_INVALID;
+  const Fp8Ext fx{a_scale, a_scale_bs, w_scale};
+  return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, N, K, epilogue, resid, ldr,
+                        resid_bs, gate, gate_ld, nullptr, stream, nullptr, &fx);
+}
+
+extern "C" int b2f_gemm_qkv_norm_rope_fp8(const void* A, int64_t lda, int64_t a_bs, const float* a_scale,
+                                          int64_t a_scale_bs, const void* W, int64_t ldw, const float* w_scale,
+                                          const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M,
+                                          int d_model, int K, const void* nw_q, const void* nw_k, const float* cos,
+                                          const float* sin, int rope_row0, float eps, int n_extra, void* out_extra,
+                                          int64_t ld_extra, int64_t bs_extra, int epi_extra, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  QkvExtra qx{nw_q, nw_k, cos, sin, rope_row0, d_model, eps, n_extra, epi_extra, out_extra, ld_extra, bs_extra};
+  const Fp8Ext fx{a_scale, a_scale_bs, w_scale};
+  return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, 3 * d_model + n_extra, K,
+                        B2F_EPI_QKV_NORM_ROPE, nullptr, 0, 0, nullptr, 0, &qx, stream, nullptr, &fx);
 }
 
 // ---------------------------------------------------------------------------------------------------- LoRA

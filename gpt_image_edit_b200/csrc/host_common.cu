@@ -29,7 +29,7 @@ extern "C" const char* b2f_strerror(int code) {
   }
 }
 
-extern "C" int b2f_version(void) { return 2; }
+extern "C" int b2f_version(void) { return 3; }
 
 extern "C" int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin) {
   int n = 0;
@@ -218,6 +218,25 @@ int make_tmap_3d_rows(CUtensorMap* out, const void* gptr, uint64_t width, uint64
                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {
     fprintf(stderr, "[b2f] cuTensorMapEncodeTiled(3d) failed: %d\n", int(r));
+    return B2F_ERR_CUDA;
+  }
+  return B2F_OK;
+}
+
+int make_tmap_u8_rows(CUtensorMap* out, const void* gptr, int rank, uint64_t width, uint64_t rows, uint64_t batch,
+                      uint64_t ld_bytes, uint64_t batch_stride_bytes) {
+  EncodeTiledFn fn = get_encode_fn();
+  if (!fn) return B2F_ERR_CUDA;
+  if (rank != 2 && rank != 3) return B2F_ERR_INVALID;
+  cuuint64_t dims[3] = {width, rows, batch};
+  cuuint64_t strides[2] = {ld_bytes, batch_stride_bytes};
+  cuuint32_t box[3] = {128, 128, 1};
+  cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_UINT8, rank, const_cast<void*>(gptr), dims, strides, box, estr,
+                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r != CUDA_SUCCESS) {
+    fprintf(stderr, "[b2f] cuTensorMapEncodeTiled(u8 %dd) failed: %d\n", rank, int(r));
     return B2F_ERR_CUDA;
   }
   return B2F_OK;

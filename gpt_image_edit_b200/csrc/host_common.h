@@ -27,6 +27,10 @@ int make_tmap_2d_bf16(CUtensorMap* out, const void* gptr, uint64_t rows, uint64_
 // out-of-range rows are zero-filled per batch item.
 int make_tmap_3d_rows(CUtensorMap* out, const void* gptr, uint64_t width, uint64_t rows,
                       uint64_t batch, uint64_t ld_elems, uint64_t batch_stride_elems, uint32_t box_rows = 128);
+// Byte-element (e4m3) tensor map over [rows, width] (rank 2) or [batch, rows, width] (rank 3), pitches in bytes, box
+// [1,] 128 rows x 128 bytes, SWIZZLE_128B: the same shared-memory layout as a [128][64] bf16 box.
+int make_tmap_u8_rows(CUtensorMap* out, const void* gptr, int rank, uint64_t width, uint64_t rows, uint64_t batch,
+                      uint64_t ld_bytes, uint64_t batch_stride_bytes);
 // 4-D bf16 tensor map for NHWC activations: global [n, h, w, c], box [1, box_h, box_w, box_c].
 // `stride` (1 or 2) is the traversal stride in h and w: the box still delivers box_h x box_w pixels.
 int make_tmap_4d_bf16(CUtensorMap* out, const void* gptr, uint64_t n, uint64_t h, uint64_t w,

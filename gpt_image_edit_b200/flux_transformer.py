@@ -76,6 +76,18 @@ def _plain_linears(cfg: FluxTransformerConfig):
     return out
 
 
+def _fp8_linears(cfg: FluxTransformerConfig):
+    """bound names of the block linears that run in FP8 once enable_fp8() is called (b2f_flux_bind_fp8)."""
+    out = []
+    for i in range(cfg.num_layers):
+        p = f"transformer_blocks.{i}."
+        out += [p + n for n in ("attn.qkv", "attn.add_qkv", "attn.to_out.0", "attn.to_add_out", "ff.net.0.proj",
+                                "ff.net.2", "ff_context.net.0.proj", "ff_context.net.2")]
+    for i in range(cfg.num_single_layers):
+        out += [f"single_transformer_blocks.{i}.qkv_mlp", f"single_transformer_blocks.{i}.proj_out"]
+    return out
+
+
 def _norm_weights(cfg: FluxTransformerConfig):
     out = []
     for i in range(cfg.num_layers):
@@ -132,6 +144,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         self._rope = None
         self._schedule = None
         self.gradient_checkpointing = False
+        self._fp8 = None   # bound name -> (e4m3 weight, fp32 scales) while FP8 is enabled
         self._lora_init()
 
     def __del__(self):
@@ -163,6 +176,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
                     if tuple(sd[k].shape) != tuple(v.shape):
                         raise RuntimeError(f"{k}: shape {tuple(sd[k].shape)} != {tuple(v.shape)}")
                     v.copy_(sd[k])
+        self._fp8_requantize()
         return SimpleNamespace(missing_keys=missing, unexpected_keys=unexpected)
 
     @torch.no_grad()
@@ -181,6 +195,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
                 for o in range(0, flat.numel(), step):
                     n = min(step, flat.numel() - o)
                     flat[o:o + n] = (torch.randn(n, device=self.device, generator=g) * s_).to(torch.bfloat16)
+        self._fp8_requantize()
         return self
 
     def named_parameters_diffusers(self):
@@ -196,6 +211,56 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
             if isinstance(a, torch.dtype) and a != torch.bfloat16:
                 raise _lib.B2FError("B200FluxTransformer2DModel computes in bfloat16 only")
         return self
+
+    # ------------------------------------------------------------------ FP8
+    @property
+    def fp8_enabled(self) -> bool:
+        return self._fp8 is not None
+
+    @torch.no_grad()
+    def enable_fp8(self):
+        """Run the ten linears of every transformer block in FP8 (e4m3 operands on the FP8 tensor cores, per-token
+        activation scales, per-output-channel weight scales; include/b2f.h).  Adds an e4m3 copy of those weights
+        (912 d^2 bytes: 8.6 GB at FLUX size) and quantizes it on the device.  The bf16 weights stay the master copy:
+        state_dict(), fuse_lora and training keep seeing them, and load_state_dict / randomize_ / fuse_lora /
+        unfuse_lora re-quantize.  Unfused LoRA adapters must be fused first."""
+        if self._fp8 is not None:
+            return self
+        if self._lora_bound:
+            raise _lib.B2FError("enable_fp8: unfused LoRA adapters are active; fuse_lora() them first")
+        fp8 = OrderedDict()
+        for name in _fp8_linears(self.config):
+            w = self._store[name + ".weight"]
+            fp8[name] = (torch.empty(w.shape, device=w.device, dtype=torch.float8_e4m3fn),
+                         torch.empty(w.shape[0], device=w.device, dtype=torch.float32))
+        self._fp8 = fp8
+        self._fp8_requantize()
+        for name, (w8, ws) in fp8.items():
+            check(_lib.lib.b2f_flux_bind_fp8(self._h, name.encode(), ptr(w8), ptr(ws), w8.numel()),
+                  f"b2f_flux_bind_fp8 {name}")
+        check(_lib.lib.b2f_flux_set_fp8(self._h, 1), "b2f_flux_set_fp8")
+        return self
+
+    def disable_fp8(self):
+        """Back to the bf16 block linears; the FP8 weight copies are released."""
+        if self._fp8 is None:
+            return self
+        check(_lib.lib.b2f_flux_set_fp8(self._h, 0), "b2f_flux_set_fp8")
+        for name in self._fp8:
+            check(_lib.lib.b2f_flux_bind_fp8(self._h, name.encode(), None, None, 0), f"b2f_flux_bind_fp8 {name}")
+        self._fp8 = None
+        self._lora_rebind()   # adapters loaded while FP8 was on act unfused again
+        return self
+
+    @torch.no_grad()
+    def _fp8_requantize(self):
+        """FP8 copies <- the row rule (b2f_quant_fp8_rows) of the current bf16 weights, in place."""
+        if getattr(self, "_fp8", None) is None:
+            return
+        for name, (w8, ws) in self._fp8.items():
+            w = self._store[name + ".weight"]
+            check(_lib.lib.b2f_quant_fp8_rows(ptr(w), w.stride(0), 0, ptr(w8), w8.stride(0), 0, ptr(ws), 0, 1,
+                                              w.shape[0], w.shape[1], stream_ptr()), f"b2f_quant_fp8_rows {name}")
 
     # ------------------------------------------------------------------ helpers
     def _workspace(self, nbytes: int, tag) -> torch.Tensor:
@@ -279,6 +344,9 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
                 img_ids=None, txt_ids=None, guidance=None, joint_attention_kwargs=None, return_dict=True,
                 **unused):
         cfg = self.config
+        if self._fp8 is not None and self._lora_bound:
+            raise _lib.B2FError("FP8 is enabled and LoRA adapters are active unfused: fuse_lora() them first "
+                                "(or disable_fp8())")
         jak = dict(joint_attention_kwargs or {})
         if jak.get("attention_mask") is not None:
             raise _lib.B2FError("attention_mask (mixed-size training batches) is not implemented in libb2f")
@@ -323,7 +391,8 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
     def debug_buffers(self, B: int, S_img: int, S_txt: int) -> SimpleNamespace:
         """Views of the whole forward workspace in b2f_flux_forward's layout (text rows first): h and xn [B, S, d],
         qkv [B, S, 3d], cat [B, S, 5d].  After a partial-range forward they hold what the last block left (stage-level
-        parity tests read them); the views are only for reading."""
+        parity tests read them); the views are only for reading.  With FP8 enabled the blocks quantize their
+        LayerNorm outputs straight to e4m3 and do not write xn."""
         ws = self._ws["fwd"]
         off = (-ws.data_ptr()) % 256
         S, d = S_img + S_txt, self.inner_dim

@@ -326,7 +326,8 @@ class FluxLoraMixin:
         from . import _lib
         _lib.check(_lib.lib.b2f_flux_clear_lora(self._h), "b2f_flux_clear_lora")
         self._lora_bound = self._lora_concat(self._lora_unfused_set(), pad=True)
-        for t, (A, B, cs) in self._lora_bound.items():
+        # with FP8 enabled the engine takes no unfused adapter: the forward refuses until they are fused or FP8 is off
+        for t, (A, B, cs) in ({} if getattr(self, "_fp8", None) is not None else self._lora_bound).items():
             _lib.check(_lib.lib.b2f_flux_bind_lora(self._h, t.encode(), A.data_ptr(), B.data_ptr(), cs.data_ptr(),
                                                    int(A.shape[0])), f"b2f_flux_bind_lora {t}")
         self._lora_version += 1
@@ -427,6 +428,7 @@ class FluxLoraMixin:
                                               B.stride(0), A.data_ptr(), A.stride(0), cs.data_ptr(), float(lora_scale),
                                               int(A.shape[0]), _lib.stream_ptr()), f"b2f_lora_fuse {t}")
         self._lora_fused.update(names)
+        self._fp8_requantize()
         self._lora_rebind()
 
     @torch.no_grad()
@@ -436,4 +438,5 @@ class FluxLoraMixin:
             self._lora_weight(t).copy_(saved)
         self._lora_saved.clear()
         self._lora_fused.clear()
+        self._fp8_requantize()
         self._lora_rebind()

@@ -371,3 +371,143 @@ def lora_fuse_(weight, bcat, acat, colscale, *, cs_mul: float = 1.0) -> torch.Te
                                  bcat.stride(0), ptr(acat), acat.stride(0), ptr(colscale), float(cs_mul), acat.shape[0],
                                  stream_ptr()), "b2f_lora_fuse")
     return weight
+
+
+# ---------------------------------------------------------------------------------------------------- FP8 (e4m3)
+FP8 = torch.float8_e4m3fn
+
+
+def _shape(t: torch.Tensor, name: str, want) -> None:
+    if tuple(t.shape) != tuple(want):
+        raise _lib.B2FError(f"{name}: expected shape {tuple(want)}, got {tuple(t.shape)}")
+
+
+def _scales(s: torch.Tensor, name: str, B: int, rows: int) -> torch.Tensor:
+    """a per-row fp32 scale vector as [B, rows] (any batch pitch, unit row pitch); [rows] when B == 1."""
+    _req(s, name, torch.float32)
+    s2 = s if s.dim() == 2 else s.unsqueeze(0)
+    _shape(s2, name, (B, rows))
+    return s2
+
+
+def quant_fp8_rows(x, *, out=None, scale=None):
+    """(q, scale): the FP8 row rule of include/b2f.h (b2f_quant_fp8_rows) on every row of x [rows, K] or [B, rows, K]
+    (any pitches): q e4m3 like x, scale fp32 [rows] / [B, rows]."""
+    _req(x, "x")
+    x3 = _as3(x)
+    B, rows, K = x3.shape
+    if out is None:
+        out = torch.empty(x.shape, device=x.device, dtype=FP8)
+    if scale is None:
+        scale = torch.empty(x.shape[:-1], device=x.device, dtype=torch.float32)
+    _req(out, "out", FP8)
+    q3, s2 = _as3(out), _scales(scale, "scale", B, rows)
+    _shape(q3, "out", (B, rows, K))
+    check(_lib.lib.b2f_quant_fp8_rows(ptr(x3), x3.stride(1), x3.stride(0), ptr(q3), q3.stride(1), q3.stride(0), ptr(s2),
+                                      s2.stride(0), B, rows, K, stream_ptr()), "b2f_quant_fp8_rows")
+    return out, scale
+
+
+def ln_modulate_fp8(x, scale, shift, *, out=None, row_scale=None, eps: float = 1e-6, split_row: int = 0, scale_b=None,
+                    shift_b=None):
+    """(q, row_scale): ln_modulate's bf16 result quantized by the FP8 row rule (b2f_ln_modulate_fp8)."""
+    _req(x, "x")
+    _req(scale, "scale")
+    _req(shift, "shift")
+    x3 = _as3(x)
+    B, rows, D = x3.shape
+    if out is None:
+        out = torch.empty(x.shape, device=x.device, dtype=FP8)
+    if row_scale is None:
+        row_scale = torch.empty(x.shape[:-1], device=x.device, dtype=torch.float32)
+    _req(out, "out", FP8)
+    o3, s2 = _as3(out), _scales(row_scale, "row_scale", B, rows)
+    _shape(o3, "out", (B, rows, D))
+    if scale.dim() != 2 or shift.stride(0) != scale.stride(0):
+        raise _lib.B2FError("scale/shift must be [B,D] views with equal pitch")
+    for t, n in ((scale, "scale"), (shift, "shift"), (scale_b, "scale_b"), (shift_b, "shift_b")):
+        if t is not None:
+            _shape(t, n, (B, D))
+    check(_lib.lib.b2f_ln_modulate_fp8(ptr(x3), x3.stride(1), x3.stride(0), ptr(scale), ptr(shift), scale.stride(0),
+                                       ptr(o3), o3.stride(1), o3.stride(0), ptr(s2), s2.stride(0), B, rows, D, eps,
+                                       split_row, ptr(scale_b), ptr(shift_b), stream_ptr()), "b2f_ln_modulate_fp8")
+    return out, row_scale
+
+
+def _fp8_weight_checks(wq, w_scale, bias, N, K):
+    _shape(wq, "wq", (N, K))
+    _shape(w_scale, "w_scale", (N,))
+    if bias is not None:
+        _req(bias, "bias")
+        _shape(bias, "bias", (N,))
+
+
+def linear_fp8(xq, x_scale, wq, w_scale, bias=None, *, epilogue: int = EPI_BIAS, out=None, resid=None,
+               gate=None) -> torch.Tensor:
+    """out = epilogue(fp32(x_scale[m] * w_scale[n]) * (xq @ wq^T) + bias) via b2f_gemm_fp8.  xq e4m3 [M,K] / [B,M,K],
+    x_scale fp32 [M] / [B,M], wq e4m3 [N,K], w_scale fp32 [N]."""
+    _req(xq, "xq", FP8)
+    _req(wq, "wq", FP8)
+    _req(w_scale, "w_scale", torch.float32)
+    x3 = _as3(xq)
+    B, M, K = x3.shape
+    s2 = _scales(x_scale, "x_scale", B, M)
+    N = wq.shape[0]
+    _fp8_weight_checks(wq, w_scale, bias, N, K)
+    if out is None:
+        out = torch.empty((*xq.shape[:-1], N), device=xq.device, dtype=torch.bfloat16)
+    _req(out, "out")
+    o3 = _as3(out)
+    _shape(o3, "out", (B, M, N))
+    ldr = rbs = gld = 0
+    if epilogue in (EPI_GATE_RESID, EPI_RESID):
+        _req(resid, "resid")
+        r3 = _as3(resid)
+        _shape(r3, "resid", (B, M, N))
+        ldr, rbs = r3.stride(1), r3.stride(0)
+        if epilogue == EPI_GATE_RESID:
+            _req(gate, "gate")
+            _shape(gate, "gate", (B, N) if gate.dim() == 2 else (N,))
+            gld = gate.stride(0) if gate.dim() == 2 else 0
+    check(_lib.lib.b2f_gemm_fp8(ptr(x3), x3.stride(1), x3.stride(0), ptr(s2), s2.stride(0), ptr(wq), wq.stride(0),
+                                ptr(w_scale), ptr(bias), ptr(o3), o3.stride(1), o3.stride(0), B, M, N, K, epilogue,
+                                ptr(resid), ldr, rbs, ptr(gate), gld, stream_ptr()), "b2f_gemm_fp8")
+    return out
+
+
+def linear_qkv_norm_rope_fp8(xq, x_scale, wq, w_scale, bias, nq, nk, cos, sin, *, rope_row0: int = 0, out=None,
+                             eps: float = 1e-6, out_extra=None, epi_extra: int = EPI_BIAS):
+    """linear_qkv_norm_rope with the FP8 operands of linear_fp8 (b2f_gemm_qkv_norm_rope_fp8)."""
+    _req(xq, "xq", FP8)
+    _req(wq, "wq", FP8)
+    _req(w_scale, "w_scale", torch.float32)
+    _req(cos, "cos", torch.float32)
+    _req(sin, "sin", torch.float32)
+    x3 = _as3(xq)
+    B, M, K = x3.shape
+    s2 = _scales(x_scale, "x_scale", B, M)
+    n_extra = 0 if out_extra is None else out_extra.shape[-1]
+    N = wq.shape[0] - n_extra
+    _fp8_weight_checks(wq, w_scale, bias, N + n_extra, K)
+    _shape(nq, "nq", (128,))
+    _shape(nk, "nk", (128,))
+    if cos.dim() != 2 or cos.shape[0] < rope_row0 + M or cos.shape[1] != 128 or cos.shape != sin.shape:
+        raise _lib.B2FError(f"cos/sin: expected [>= {rope_row0 + M}, 128] tables, got {tuple(cos.shape)} / "
+                            f"{tuple(sin.shape)}")
+    if out is None:
+        out = torch.empty((*xq.shape[:-1], N), device=xq.device, dtype=torch.bfloat16)
+    _req(out, "out")
+    o3 = _as3(out)
+    _shape(o3, "out", (B, M, N))
+    e3 = None
+    if out_extra is not None:
+        _req(out_extra, "out_extra")
+        e3 = _as3(out_extra)
+        _shape(e3, "out_extra", (B, M, n_extra))
+    check(_lib.lib.b2f_gemm_qkv_norm_rope_fp8(ptr(x3), x3.stride(1), x3.stride(0), ptr(s2), s2.stride(0), ptr(wq),
+                                              wq.stride(0), ptr(w_scale), ptr(bias), ptr(o3), o3.stride(1), o3.stride(0),
+                                              B, M, N // 3, K, ptr(nq), ptr(nk), ptr(cos), ptr(sin), rope_row0, eps,
+                                              n_extra, ptr(e3), 0 if e3 is None else e3.stride(1),
+                                              0 if e3 is None else e3.stride(0), epi_extra, stream_ptr()),
+          "b2f_gemm_qkv_norm_rope_fp8")
+    return out

@@ -300,6 +300,9 @@ class FluxTrainGraph:
         if getattr(self.den, "lora_unfused_active", lambda: False)():
             raise _lib.B2FError("the denoiser has unfused LoRA adapters active and the training backward does not see them: "
                            "fuse_lora() or disable / unload them first")
+        if getattr(self.den, "fp8_enabled", False):
+            raise _lib.B2FError("the denoiser runs its block linears in FP8 and training uses the bf16 weights: "
+                                "disable_fp8() first")
         self.proj = getattr(model.denoise_tower, "denoise_projector", None)
         self.params = params
         self.on_block_done = on_block_done          # callback(bucket) after a block's gradients are complete

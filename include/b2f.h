@@ -33,7 +33,7 @@ extern "C" {
 typedef void* b2f_stream_t; /* cudaStream_t */
 
 const char* b2f_strerror(int code);
-/* ABI version; bumped on any signature change or addition (2: LoRA entry points). */
+/* ABI version; bumped on any signature change or addition (2: LoRA entry points, 3: FP8 entry points). */
 int b2f_version(void);
 /* Device facts the host needs for grid sizing / reporting. Returns B2F_ERR_NODEVICE without GPU. */
 int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin);
@@ -151,6 +151,45 @@ int b2f_lora_fuse(void* W, int64_t ldw, int rows, int cols, const void* Bcat, in
                   int64_t lda, const float* colscale, float cs_mul, int r, b2f_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
+ * FP8 (e4m3) linear layers: per-token activation scales and per-output-channel weight scales (the scheme torchao calls
+ * float8 dynamic activation / float8 weight, per row), computed by the FP8 tensor cores (wgmma ...e4m3.e4m3, fp32
+ * accumulators).
+ *
+ * Row rule.  A bf16 row x[0..K) (a token's activations, or one output channel of a weight) becomes e4m3 bytes q and one
+ * fp32 scale s:
+ *   amax = max |x_i| (fp32, exact);
+ *   amax == 0:  s = 1, every q_i = 0 (+0);
+ *   otherwise   inv = 448.0f / amax, s = amax / 448.0f (IEEE fp32 divisions, round to nearest),
+ *               q_i = e4m3(x_i * inv): one fp32 multiply, then round to nearest even saturating to +-448
+ *               (cvt.rn.satfinite.e4m3x2.f32).
+ * So x_i ~ s * q_i.  The CPU equivalent is (x.float() * inv).clamp(-448, 448).to(torch.float8_e4m3fn).
+ *
+ * GEMM.  acc[m, n] = sum_k qa[m, k] qw[n, k] in fp32 on the tensor cores; the staged value is
+ *   x = bf16(fmaf(acc, fp32(sa[m] * sw[n]), bias[n]))      (bf16(acc * fp32(sa[m] * sw[n])) without a bias),
+ * and from x on every epilogue is exactly b2f_gemm_bf16's / b2f_gemm_qkv_norm_rope's.  The tensor cores' fp32
+ * accumulation of e4m3 products is not IEEE fp32 accumulation: tests/test_fp8_gpu.py states the measured allowance.
+ */
+/* x [batch, rows, K] bf16 (pitches in elements) -> q [batch, rows, K] e4m3 (pitches in bytes) and scale fp32
+ * [batch, rows] (batch pitch scale_batch_stride).  K % 16 == 0; ldq, q_batch_stride multiples of 16. */
+int b2f_quant_fp8_rows(const void* x, int64_t ldx, int64_t x_batch_stride, void* q, int64_t ldq, int64_t q_batch_stride,
+                       float* scale, int64_t scale_batch_stride, int batch, int rows, int K, b2f_stream_t stream);
+/* b2f_gemm_bf16 (every forward epilogue) with A [batch, M, K] e4m3 (pitches in bytes) scaled by a_scale fp32 [batch, M]
+ * (batch pitch a_scale_batch_stride) and W [N, K] e4m3 scaled by w_scale fp32 [N] (16-byte aligned).  K, lda, ldw and
+ * a_batch_stride are multiples of 16 (TMA). */
+int b2f_gemm_fp8(const void* A, int64_t lda, int64_t a_batch_stride, const float* a_scale,
+                 int64_t a_scale_batch_stride, const void* W, int64_t ldw, const float* w_scale, const void* bias,
+                 void* out, int64_t ldc, int64_t out_batch_stride, int batch, int M, int N, int K, int epilogue,
+                 const void* resid, int64_t ldr, int64_t resid_batch_stride, const void* gate, int64_t gate_ld,
+                 b2f_stream_t stream);
+/* b2f_gemm_qkv_norm_rope (including the n_extra second output block) with the operands of b2f_gemm_fp8. */
+int b2f_gemm_qkv_norm_rope_fp8(const void* A, int64_t lda, int64_t a_batch_stride, const float* a_scale,
+                               int64_t a_scale_batch_stride, const void* W, int64_t ldw, const float* w_scale,
+                               const void* bias, void* out, int64_t ldc, int64_t out_batch_stride, int batch, int M,
+                               int d_model, int K, const void* nw_q, const void* nw_k, const float* cos,
+                               const float* sin, int rope_row0, float eps, int n_extra, void* out_extra,
+                               int64_t ld_extra, int64_t extra_batch_stride, int epi_extra, b2f_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
  * AdaLN modulate (HBM-bound): out = LayerNorm(x; eps, no affine) * (1 + scale[b]) + shift[b].
  * Replaces nn.LayerNorm + the broadcast multiply/add of diffusers AdaLayerNormZero /
  * AdaLayerNormZeroSingle / AdaLayerNormContinuous and the norm2 modulate inside
@@ -163,6 +202,14 @@ int b2f_ln_modulate(const void* x, int64_t ldx, int64_t x_batch_stride, const vo
                     const void* shift, int64_t mod_ld, void* out, int64_t ldo,
                     int64_t out_batch_stride, int batch, int rows, int D, float eps, int split_row,
                     const void* scale_b, const void* shift_b, b2f_stream_t stream);
+/* b2f_ln_modulate whose bf16 result row goes through the FP8 row rule (b2f_quant_fp8_rows) instead of being stored: out
+ * receives e4m3 bytes (pitches in bytes, multiples of 16) and row_scale fp32 [batch, rows] (batch pitch
+ * row_scale_batch_stride) the row scales.  Bit-identical to b2f_ln_modulate followed by b2f_quant_fp8_rows.
+ * D % 256 == 0, D <= 3072. */
+int b2f_ln_modulate_fp8(const void* x, int64_t ldx, int64_t x_batch_stride, const void* scale, const void* shift,
+                        int64_t mod_ld, void* out, int64_t ldo, int64_t out_batch_stride, float* row_scale,
+                        int64_t row_scale_batch_stride, int batch, int rows, int D, float eps, int split_row,
+                        const void* scale_b, const void* shift_b, b2f_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Per-head RMSNorm + interleaved-pair RoPE, in place on the Q and K blocks of a fused QKV buffer
@@ -332,6 +379,20 @@ int b2f_flux_forward(b2f_flux* ctx, const void* hidden, const void* enc, const v
                      int64_t mod_ld, void* out, int B, int S_img, int S_txt, int n_out_rows,
                      void* ws, size_t ws_bytes, int first_block, int last_block,
                      b2f_stream_t stream);
+/* FP8 block linears (see b2f_gemm_fp8).  b2f_flux_bind_fp8 binds the e4m3 copy w8 [out, in] of one block linear and its
+ * fp32 per-channel scales w_scale [out] (borrowed; made by b2f_quant_fp8_rows from the bf16 weight) under the linear's
+ * bound name (transformer_blocks.{i}.attn.qkv / attn.add_qkv / attn.to_out.0 / attn.to_add_out / ff.net.0.proj /
+ * ff.net.2 / ff_context.net.0.proj / ff_context.net.2, single_transformer_blocks.{i}.qkv_mlp / proj_out); numel =
+ * out * in; w8 == NULL unbinds.  b2f_flux_set_fp8(ctx, 1) makes b2f_flux_forward run those ten linears per block in FP8:
+ * it requires every one to be bound and no LoRA adapter to be bound (b2f_flux_bind_lora is refused while FP8 is on;
+ * fuse adapters first).  Every other linear (embedders, AdaLN, norm_out / proj_out) and attention stay bf16.  The
+ * inputs are quantized per token: the block's modulated LayerNorms by b2f_ln_modulate_fp8, the attention output
+ * (input of to_out / to_add_out), the MLP activations (ff.net.2 / ff_context.net.2) and the single block's [attn | mlp]
+ * (proj_out) by one b2f_quant_fp8_rows launch each over all tokens.  While FP8 is on b2f_flux_workspace_bytes adds an
+ * e4m3 [B, S, 5d] buffer and an fp32 [B, S] scale vector, the blocks leave the workspace's xn rows unwritten, and the
+ * training entry points refuse.  b2f_flux_finalize drops the FP8 bindings and switches FP8 off. */
+int b2f_flux_bind_fp8(b2f_flux* ctx, const char* name, const void* w8, const float* w_scale, int64_t numel);
+int b2f_flux_set_fp8(b2f_flux* ctx, int on);
 
 /* ------------------------------------------------------------------------------------------
  * Kernels of the Qwen2.5-VL conditioning prefill (transformers Qwen2_5_VL*, SURVEY.md Appendix B;

@@ -259,6 +259,8 @@ def main(args):
     device = torch.device("cuda")
     model, task_head, processor = load_main_model_and_processor(args.model_path, device, args.synthetic, args.small)
     pipe, tokenizers, text_encoders = load_pipe(model.denoise_tower.denoiser, args.flux_path, device, args.synthetic, args.small)
+    if getattr(args, "fp8", False):
+        pipe.transformer.enable_fp8()
     session = ChatSession(args, model, task_head, pipe, processor, tokenizers, text_encoders, device)
 
     if args.prompt is not None or args.image is not None:       # one non-interactive turn
@@ -296,6 +298,8 @@ def build_parser():
     p.add_argument("--max_new_tokens", type=int, default=128, help="text-reply branch (reference: 128)")
     p.add_argument("--force_text_reply", action="store_true", help="with --synthetic: route the turn to the text-reply "
                    "branch (the synthetic task head otherwise always chooses 'generate image')")
+    p.add_argument("--fp8", action="store_true", help="run the denoiser's block linears in FP8 (e4m3 tensor cores, "
+                   "per-token / per-channel scales; adds an 8.6 GB e4m3 copy of those weights)")
     p.add_argument("--prompt", type=str, default=None)
     p.add_argument("--image", type=str, default=None)
     p.add_argument("--output", type=str, default="output.png")
