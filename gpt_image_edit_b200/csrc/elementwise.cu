@@ -63,19 +63,6 @@ __device__ __forceinline__ float warp_max(float v) {
   for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
   return v;
 }
-// amax of 8 packed bf16 values (exact: |x| of a bf16 value is a bf16 value)
-__device__ __forceinline__ float amax8(const uint4 q, float m) {
-  const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j)
-    m = fmax3(m, fabsf(__uint_as_float(w[j] << 16)), fabsf(__uint_as_float(w[j] & 0xffff0000u)));
-  return m;
-}
-// The row rule of include/b2f.h: (scale, inverse) of a row whose amax is `amax`; an all-zero row gets (1, 0).
-__device__ __forceinline__ void row_scale_of(float amax, float& s, float& inv) {
-  s = amax > 0.f ? __fdiv_rn(amax, 448.0f) : 1.0f;
-  inv = amax > 0.f ? __fdiv_rn(448.0f, amax) : 0.0f;
-}
 
 // One warp per row, rows taken grid-stride.  The row stays PACKED in registers (MAXC uint4 per lane, 48 registers
 // for D = 3072) and is unpacked again in each of the three passes (sum, centred sum of squares, output): with the

@@ -60,6 +60,8 @@ struct FluxCtx {
   int lora_rmax() const;
   // b2f_flux_set_fp8: the block linears of b2f_flux_forward run in FP8
   bool fp8 = false;
+  // b2f_flux_set_fp8_attention: the blocks' attention runs in FP8 (b2f_attn_quant_fp8 + b2f_attention_fp8)
+  bool fp8_attn = false;
   // fp32 gradient buffers of the trainable tensors, bound by name (flux_train.cu); an unbound name is frozen
   std::map<std::string, std::pair<float*, int64_t>> grads;
 };

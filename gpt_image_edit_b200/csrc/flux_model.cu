@@ -263,6 +263,7 @@ int b2f_flux_finalize(b2f_flux* h) {
   });
   c->adaln_lora.clear();
   c->fp8 = false;
+  c->fp8_attn = false;
   c->finalized = true;
   return B2F_OK;
 }
@@ -282,9 +283,11 @@ size_t b2f_flux_workspace_bytes(const b2f_flux* h, int B, int S_img, int S_txt) 
   if (!c || B <= 0 || S_img <= 0 || S_txt < 0) return 0;
   const size_t S = (size_t)S_img + S_txt;
   // h[d] + xn[d] + qkv[3d] + cat[5d] per token, bf16; with unfused LoRA adapters bound, T[r_pad] per token; with FP8
-  // on, e4m3 q8[5d] and an fp32 scale per token
+  // on, e4m3 q8[5d] and an fp32 scale per token; with FP8 attention on, the buffers of b2f_attn_quant_fp8
   const size_t fp8 = c->fp8 ? (size_t)B * S * ((size_t)c->d * 5 + 4) + 256 : 0;
-  return (size_t)B * S * ((size_t)c->d * 10 + (size_t)c->lora_rmax()) * 2 + 1024 + fp8;
+  const size_t S_pad = (S + 127) / 128 * 128, H = (size_t)c->cfg.num_heads;
+  const size_t fa = c->fp8_attn ? (size_t)B * c->d * (2 * S + S_pad) + (size_t)B * (2 * H + c->d) * 4 + 256 : 0;
+  return (size_t)B * S * ((size_t)c->d * 10 + (size_t)c->lora_rmax()) * 2 + 1024 + fp8 + fa;
 }
 
 size_t b2f_flux_temb_workspace_bytes(const b2f_flux* h, int rows) {
@@ -499,6 +502,14 @@ int b2f_flux_set_fp8(b2f_flux* h, int on) {
   return B2F_OK;
 }
 
+int b2f_flux_set_fp8_attention(b2f_flux* h, int on) {
+  FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
+  if (!c || !c->finalized) return B2F_ERR_INVALID;
+  if (on && c->cfg.head_dim != 128) return B2F_ERR_UNSUPPORTED;
+  c->fp8_attn = on != 0;
+  return B2F_OK;
+}
+
 int b2f_flux_lora_rank(const b2f_flux* h) {
   const FluxCtx* c = reinterpret_cast<const FluxCtx*>(h);
   return c && c->finalized ? c->lora_rmax() : 0;
@@ -547,6 +558,25 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
   auto quant_cat = [&](int64_t c0, int K) {
     return b2f_quant_fp8_rows(cat + c0, 5 * d, (int64_t)S * 5 * d, q8, 5 * d, q8_bs, qs, S, B, S, K, st);
   };
+  // FP8 attention on: q8 / k8 [B,S,d], v8t [B,H,128,S_pad] e4m3 and their scales sq / sk [B,H], sv [B,d] fp32
+  const int64_t S_pad = ((int64_t)S + 127) / 128 * 128;
+  uint8_t* aq8 = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(f8 ? reinterpret_cast<uint8_t*>(qs + BS) : q8) +
+                                             255) & ~uintptr_t(255));
+  uint8_t* ak8 = aq8 + BS * d;
+  uint8_t* av8 = ak8 + BS * d;
+  float* asq = reinterpret_cast<float*>(av8 + (int64_t)B * d * S_pad);
+  float* ask = asq + (int64_t)B * H;
+  float* asv = ask + (int64_t)B * H;
+  // joint attention of the qkv buffer into cat[:, :, :d]
+  auto attention = [&]() {
+    if (!c->fp8_attn)
+      return b2f_attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S, g.head_dim,
+                               scale, 0, st);
+    const int r = b2f_attn_quant_fp8(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, aq8, ak8, asq, ask, av8, asv, B, H,
+                                     S, g.head_dim, st);
+    if (r) return r;
+    return b2f_attention_fp8(aq8, ak8, asq, ask, av8, asv, cat, 5 * d, B, H, S, g.head_dim, scale, 0, st);
+  };
   const float ls = c->lora_scale;
   const int64_t h_bs = (int64_t)S * d, qkv_bs = (int64_t)S * 3 * d, cat_bs = (int64_t)S * 5 * d;
   bf16_t* h_img = hb + (int64_t)S_txt * d;
@@ -594,8 +624,7 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
       RUN(qkv_fwd(w.add_qkv, tb, ls, xn_txt, d, h_bs, d, qkv_txt, 3 * d, qkv_bs, B, S_txt,
                              (int)d, (int)d, w.norm_added_q, w.norm_added_k, c->rope_cos, c->rope_sin, 0, eps, 0,
                              nullptr, 0, 0, 0, st, qt));
-      RUN(b2f_attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S,
-                            g.head_dim, scale, 0, st));
+      RUN(attention());
       if (f8) RUN(quant_cat(0, (int)d));
       RUN(lin_fwd(w.to_out, tb, ls, cat_img, 5 * d, cat_bs, d, h_img, d, h_bs, B, S_img,
                     (int)d, (int)d, B2F_EPI_GATE_RESID, h_img, d, h_bs, mi + 2 * d, mod_ld, st, qi));
@@ -633,8 +662,7 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
       RUN(qkv_fwd(w.qkv_mlp, tb, ls, xn, d, h_bs, d, qkv, 3 * d, qkv_bs, B, S, (int)d, (int)d,
                              w.norm_q, w.norm_k, c->rope_cos, c->rope_sin, 0, eps, (int)(4 * d), cat + d, 5 * d,
                              cat_bs, B2F_EPI_GELU_TANH, st, qt));
-      RUN(b2f_attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S,
-                            g.head_dim, scale, 0, st));
+      RUN(attention());
       if (f8) RUN(quant_cat(0, (int)(5 * d)));
       RUN(lin_fwd(w.proj_out, tb, ls, cat, 5 * d, cat_bs, 5 * d, hb, d, h_bs, B, S, (int)d,
                     (int)(5 * d), B2F_EPI_GATE_RESID, hb, d, h_bs, ms + 2 * d, mod_ld, st, qt));

@@ -129,7 +129,7 @@ int b2f_flux_train_forward(b2f_flux* h, const void* hidden, const void* enc, con
     fprintf(stderr, "[b2f] flux_train_forward: unfused LoRA adapters are bound\n");
     return B2F_ERR_UNSUPPORTED;
   }
-  if (c->fp8) {   // training runs the bf16 weights: switch FP8 off first
+  if (c->fp8 || c->fp8_attn) {   // training runs the bf16 weights and attention: switch FP8 off first
     fprintf(stderr, "[b2f] flux_train_forward: FP8 is on\n");
     return B2F_ERR_UNSUPPORTED;
   }
@@ -162,7 +162,7 @@ int b2f_flux_train_backward(b2f_flux* h, const void* dout, const void* mod, int6
   if (!c || !c->finalized || !mod || !silu_temb || !ws || B <= 0 || S_img <= 0 || S_txt <= 0)
     return B2F_ERR_INVALID;
   if (n_out_rows <= 0 || n_out_rows > S_img) return B2F_ERR_INVALID;
-  if (c->fp8) {
+  if (c->fp8 || c->fp8_attn) {
     fprintf(stderr, "[b2f] flux_train_backward: FP8 is on\n");
     return B2F_ERR_UNSUPPORTED;
   }

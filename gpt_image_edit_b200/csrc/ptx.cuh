@@ -170,6 +170,18 @@ __device__ __forceinline__ void wgmma_m64n128k32_e4m3_ss(float (&d)[64], uint64_
       : "l"(desc_a), "l"(desc_b), "r"(scale_d));
 }
 
+// The same with A from registers: a[0..3] hold 4 e4m3 bytes each (lowest byte first), a[0] = A[g][4t..4t+3],
+// a[1] = A[g+8][4t..4t+3], a[2] = A[g][16+4t..16+4t+3], a[3] = A[g+8][16+4t..16+4t+3] for row g = 16 w + l / 4 and
+// t = l % 4 (PTX ISA, wgmma register fragment of an 8-bit A, m64nNk32).
+__device__ __forceinline__ void wgmma_m64n128k32_e4m3_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t desc_b,
+                                                         uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k32.f32.e4m3.e4m3 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d));
+}
+
 // ------------------------------------------------------------------ FP8 (e4m3) conversion
 // Two fp32 values -> two e4m3 bytes (lo in bits 0-7), round to nearest even, saturating to +-448 (NaN stays NaN).
 __device__ __forceinline__ uint16_t cvt_e4m3x2(float lo, float hi) {
@@ -217,6 +229,21 @@ __device__ __forceinline__ void fadd2(float& d0, float& d1, float a0, float a1, 
 __device__ __forceinline__ void fmul2(float& d0, float& d1, float a0, float a1, float b0, float b1) {
   d0 = __fmul_rn(a0, b0);
   d1 = __fmul_rn(a1, b1);
+}
+
+// ------------------------------------------------------------------ FP8 row rule
+// amax of 8 packed bf16 values (exact: |x| of a bf16 value is a bf16 value; NaN is dropped)
+__device__ __forceinline__ float amax8(const uint4 q, float m) {
+  const uint32_t w[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+  for (int j = 0; j < 4; ++j)
+    m = fmax3(m, fabsf(__uint_as_float(w[j] << 16)), fabsf(__uint_as_float(w[j] & 0xffff0000u)));
+  return m;
+}
+// The row rule of include/b2f.h: (scale, inverse) of a row whose amax is `amax`; an all-zero row gets (1, 0).
+__device__ __forceinline__ void row_scale_of(float amax, float& s, float& inv) {
+  s = amax > 0.f ? __fdiv_rn(amax, 448.0f) : 1.0f;
+  inv = amax > 0.f ? __fdiv_rn(448.0f, amax) : 0.0f;
 }
 
 __device__ __forceinline__ float bf16r(float x) {  // round-to-nearest-even through bf16

@@ -511,3 +511,75 @@ def linear_qkv_norm_rope_fp8(xq, x_scale, wq, w_scale, bias, nq, nk, cos, sin, *
                                               0 if e3 is None else e3.stride(0), epi_extra, stream_ptr()),
           "b2f_gemm_qkv_norm_rope_fp8")
     return out
+
+
+def _row_pitch(t: torch.Tensor) -> int:
+    """Token pitch of a [B,S,H,dh] view; with S = 1 the stride of that dimension is arbitrary and the batch pitch is it."""
+    B, S = t.shape[:2]
+    return t.stride(1) if S > 1 else t.stride(0) if B > 1 else t.shape[2] * t.shape[3]
+
+
+def _qkv_views(q, k, v):
+    """(B, S, H, dh) of bf16 [B,S,H,dh] views as attention() takes them, with one shape for all three."""
+    for t, n in ((q, "q"), (k, "k"), (v, "v")):
+        _req(t, n)
+        if t.dim() != 4 or t.stride(2) != t.shape[3] or (t.shape[0] > 1 and t.stride(0) != t.shape[1] * _row_pitch(t)):
+            raise _lib.B2FError(f"{n}: expected a [B,S,H,dh] view with contiguous heads and batch stride S*ld")
+    if not (q.shape == k.shape == v.shape):
+        raise _lib.B2FError(f"q, k, v: expected one shape, got {tuple(q.shape)}, {tuple(k.shape)}, {tuple(v.shape)}")
+    return tuple(q.shape)
+
+
+def _fp8_attn_buffers(B, S, H, dh, q8, k8, sq, sk, v8t, sv, device):
+    """The operand buffers of b2f_attention_fp8 (include/b2f.h, "FP8 attention"), allocated where None, checked
+    (dtype, shape, contiguity) where given."""
+    S_pad = (S + 127) // 128 * 128
+    want = (("q8", q8, FP8, (B, S, H, dh)), ("k8", k8, FP8, (B, S, H, dh)), ("sq", sq, torch.float32, (B, H)),
+            ("sk", sk, torch.float32, (B, H)), ("v8t", v8t, FP8, (B, H, dh, S_pad)),
+            ("sv", sv, torch.float32, (B, H, dh)))
+    out = []
+    for n, t, dt, shp in want:
+        if t is None:
+            t = torch.empty(shp, device=device, dtype=dt)
+        _req(t, n, dt)
+        _shape(t, n, shp)
+        if not t.is_contiguous():
+            raise _lib.B2FError(f"{n}: must be contiguous")
+        out.append(t)
+    return out
+
+
+def attn_quant_fp8(q, k, v, *, q8=None, k8=None, sq=None, sk=None, v8t=None, sv=None):
+    """(q8, k8, sq, sk, v8t, sv) of b2f_attn_quant_fp8: q, k, v bf16 [B,S,H,dh] views as attention() takes them ->
+    q8 / k8 e4m3 [B,S,H,dh] with per-head scales sq / sk fp32 [B,H], v8t e4m3 [B,H,dh,S_pad] (tokens contiguous, in the
+    P-fragment order of include/b2f.h, padding +0) with per-channel scales sv fp32 [B,H,dh]."""
+    B, S, H, dh = _qkv_views(q, k, v)
+    bufs = _fp8_attn_buffers(B, S, H, dh, q8, k8, sq, sk, v8t, sv, q.device)
+    q8, k8, sq, sk, v8t, sv = bufs
+    check(_lib.lib.b2f_attn_quant_fp8(ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v), ptr(q8), ptr(k8),
+                                      ptr(sq), ptr(sk), ptr(v8t), ptr(sv), B, H, S, dh, stream_ptr()),
+          "b2f_attn_quant_fp8")
+    return tuple(bufs)
+
+
+def attention_fp8(q8, k8, sq, sk, v8t, sv, *, out=None, scale: float | None = None, causal: bool = False,
+                  bias=None) -> torch.Tensor:
+    """softmax(q k^T * scale) v via b2f_attention_fp8 from the buffers of attn_quant_fp8; out [B,S,H*dh] bf16 (any row
+    pitch).  Non-causal, without a bias: anything else raises."""
+    if bias is not None:
+        raise _lib.B2FError("attention_fp8: a score bias is not supported")
+    _req(q8, "q8", FP8)
+    if q8.dim() != 4:
+        raise _lib.B2FError(f"q8: expected [B,S,H,dh], got {tuple(q8.shape)}")
+    B, S, H, dh = q8.shape
+    q8, k8, sq, sk, v8t, sv = _fp8_attn_buffers(B, S, H, dh, q8, k8, sq, sk, v8t, sv, q8.device)
+    if out is None:
+        out = torch.empty((B, S, H * dh), device=q8.device, dtype=torch.bfloat16)
+    _req(out, "out")
+    _shape(out, "out", (B, S, H * dh))
+    if B > 1 and out.stride(0) != S * out.stride(1):
+        raise _lib.B2FError("out: expected batch stride S * row pitch")
+    check(_lib.lib.b2f_attention_fp8(ptr(q8), ptr(k8), ptr(sq), ptr(sk), ptr(v8t), ptr(sv), ptr(out), out.stride(1), B,
+                                     H, S, dh, float(dh ** -0.5 if scale is None else scale), int(causal), stream_ptr()),
+          "b2f_attention_fp8")
+    return out

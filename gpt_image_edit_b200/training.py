@@ -303,6 +303,9 @@ class FluxTrainGraph:
         if getattr(self.den, "fp8_enabled", False):
             raise _lib.B2FError("the denoiser runs its block linears in FP8 and training uses the bf16 weights: "
                                 "disable_fp8() first")
+        if getattr(self.den, "fp8_attention_enabled", False):
+            raise _lib.B2FError("the denoiser runs its attention in FP8 and the training backward is bf16: "
+                                "disable_fp8() first")
         self.proj = getattr(model.denoise_tower, "denoise_projector", None)
         self.params = params
         self.on_block_done = on_block_done          # callback(bucket) after a block's gradients are complete

@@ -33,7 +33,8 @@ extern "C" {
 typedef void* b2f_stream_t; /* cudaStream_t */
 
 const char* b2f_strerror(int code);
-/* ABI version; bumped on any signature change or addition (2: LoRA entry points, 3: FP8 entry points). */
+/* ABI version; bumped on any signature change or addition (2: LoRA entry points, 3: FP8 entry points, 4: FP8
+ * attention). */
 int b2f_version(void);
 /* Device facts the host needs for grid sizing / reporting. Returns B2F_ERR_NODEVICE without GPU. */
 int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin);
@@ -188,6 +189,51 @@ int b2f_gemm_qkv_norm_rope_fp8(const void* A, int64_t lda, int64_t a_batch_strid
                                int d_model, int K, const void* nw_q, const void* nw_k, const float* cos,
                                const float* sin, int rope_row0, float eps, int n_extra, void* out_extra,
                                int64_t ld_extra, int64_t extra_batch_stride, int epi_extra, b2f_stream_t stream);
+
+/* ------------------------------------------------------------------------------------------
+ * FP8 attention (head_dim 128, non-causal, no bias): b2f_attention_fwd's online softmax with Q / K / V in e4m3 on the
+ * FP8 tensor cores (wgmma m64n128k32 e4m3, fp32 accumulators).
+ *
+ * Scales.  The row rule of "FP8 linear layers" above, unchanged, over a different unit of "row":
+ *   Q, K   one scale per (batch item, head): the row is all S x 128 values of that head (after the per-head RMSNorm and
+ *          RoPE their range is bounded by the norm weight, well inside e4m3's 2^14.8 normal span);
+ *   V      one scale per (batch item, head, channel): the row is that channel's S values.
+ * The range costs nothing, but e4m3 keeps 3 mantissa bits: each score carries a relative error of a few percent of
+ * sum |q_i k_i|, which moves a peaked softmax row far more than a flat one.  With RMSNorm'd q / k under norm weights of
+ * rms 2.5 (median row max p 0.6), S = 4641, the output is 13 % off in rel-L2 (bf16: 0.17 %); see README.
+ * Buffers (contiguous): q8, k8 e4m3 [B, S, H*128] (the token-major layout of the bf16 inputs); sq, sk fp32 [B, H];
+ * v8t e4m3 [B, H, 128, S_pad] with S_pad = S rounded up to 128 and tokens contiguous (FP8 wgmma takes K-major operands
+ * only, and the token is the k dimension of P.V); sv fp32 [B, H, 128].  Padding tokens of v8t are +0.
+ *
+ * Token order of v8t.  Within every group of 32 tokens, k-position p holds token
+ *   token(p) = (p & 16) + 2 ((p & 15) >> 2) + (p & 1) + 8 ((p >> 1) & 1)
+ * i.e. with t = lane % 4, k-positions 4t..4t+3 hold tokens {2t, 2t+1, 8+2t, 9+2t} and 16+4t..16+4t+3 hold
+ * {16+2t, 17+2t, 24+2t, 25+2t}.  That maps the fp32 accumulator layout of S = Q K^T (m64n128: a thread holds columns
+ * 8j + 2t, 8j + 2t + 1) onto the register A fragment of the m64n128k32 e4m3 P.V wgmma (a thread holds k 4t..4t+3 and
+ * 16+4t..16+4t+3), so P converts to e4m3 in place, without shuffles.
+ *
+ * Kernel arithmetic, per 128-token KV block in the order of attention.cu:
+ *   c = fp32(fp32(sq * sk) * fp32(scale * log2 e)), the last product of the fp32 scale taken in double;  acc = Q8 K8^T (tensor cores, fp32);  m = running max of c * acc;
+ *   p' = ex2(fmaf(acc, c, 8 - m)) = 256 p with p = 2^(t - m), t = c * acc (fp32; masked tail columns give p' = 0);
+ *   l' = l' * ex2(m_old - m) + sum(p') (fp32 p', so l' = 256 l);  P8 = e4m3(p') (p' <= 256 never saturates);
+ *   O = O * ex2(m_old - m) + P8 V8 (tensor cores, fp32; the rescale is skipped where every factor of a warp is 1),
+ * and at the end, per channel c:  out = bf16((O[c] * sv[c]) * (1 / l')).
+ * The factor 256 keeps p in e4m3's normal range; it sits in the exponent of ex2 rather than in a multiply, which the
+ * softmax-bound kernel needs.  Up to fp32 rounding this is P8 = e4m3(256 p), out = O sv / (256 l).  The e4m3 products
+ * are accumulated as the FP8 GEMM's are: tests/test_attn_fp8_gpu.py states the measured allowance.
+ */
+/* Quantize bf16 q / k / v (the pitched views of b2f_attention_fwd, Sq = Skv = S, H = Hkv heads) into the buffers above:
+ * an amax pass (atomicMax on the bits of non-negative floats, so order-independent), a quantize / transpose pass and a
+ * pass that turns the amaxes into scales (three launches).  NaN and zero inputs behave as in the row rule.  ldq / ldk /
+ * ldv multiples of 8; q, k, v, q8, k8, v8t 16-byte aligned. */
+int b2f_attn_quant_fp8(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv, void* q8,
+                       void* k8, float* sq, float* sk, void* v8t, float* sv, int B, int H, int S, int head_dim,
+                       b2f_stream_t stream);
+/* out [B, S, H*128] (row pitch ldo, a multiple of 8) = softmax(Q K^T * scale) V from the buffers of b2f_attn_quant_fp8.
+ * head_dim != 128 or causal != 0: B2F_ERR_UNSUPPORTED. */
+int b2f_attention_fp8(const void* q8, const void* k8, const float* sq, const float* sk, const void* v8t, const float* sv,
+                      void* out, int64_t ldo, int B, int H, int S, int head_dim, float scale, int causal,
+                      b2f_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * AdaLN modulate (HBM-bound): out = LayerNorm(x; eps, no affine) * (1 + scale[b]) + shift[b].
@@ -385,7 +431,8 @@ int b2f_flux_forward(b2f_flux* ctx, const void* hidden, const void* enc, const v
  * ff.net.2 / ff_context.net.0.proj / ff_context.net.2, single_transformer_blocks.{i}.qkv_mlp / proj_out); numel =
  * out * in; w8 == NULL unbinds.  b2f_flux_set_fp8(ctx, 1) makes b2f_flux_forward run those ten linears per block in FP8:
  * it requires every one to be bound and no LoRA adapter to be bound (b2f_flux_bind_lora is refused while FP8 is on;
- * fuse adapters first).  Every other linear (embedders, AdaLN, norm_out / proj_out) and attention stay bf16.  The
+ * fuse adapters first).  Every other linear (embedders, AdaLN, norm_out / proj_out) stays bf16, and so does attention
+ * unless b2f_flux_set_fp8_attention is on.  The
  * inputs are quantized per token: the block's modulated LayerNorms by b2f_ln_modulate_fp8, the attention output
  * (input of to_out / to_add_out), the MLP activations (ff.net.2 / ff_context.net.2) and the single block's [attn | mlp]
  * (proj_out) by one b2f_quant_fp8_rows launch each over all tokens.  While FP8 is on b2f_flux_workspace_bytes adds an
@@ -393,6 +440,11 @@ int b2f_flux_forward(b2f_flux* ctx, const void* hidden, const void* enc, const v
  * training entry points refuse.  b2f_flux_finalize drops the FP8 bindings and switches FP8 off. */
 int b2f_flux_bind_fp8(b2f_flux* ctx, const char* name, const void* w8, const float* w_scale, int64_t numel);
 int b2f_flux_set_fp8(b2f_flux* ctx, int on);
+/* FP8 attention, independent of b2f_flux_set_fp8: while on, the double and single blocks quantize Q / K / V with
+ * b2f_attn_quant_fp8 and run b2f_attention_fp8 where they run b2f_attention_fwd.  b2f_flux_workspace_bytes then adds
+ * q8, k8, v8t and their scales, and the training entry points refuse.  Unfused LoRA adapters stay allowed (they act on
+ * the linears only).  b2f_flux_finalize switches it off. */
+int b2f_flux_set_fp8_attention(b2f_flux* ctx, int on);
 
 /* ------------------------------------------------------------------------------------------
  * Kernels of the Qwen2.5-VL conditioning prefill (transformers Qwen2_5_VL*, SURVEY.md Appendix B;

@@ -1,14 +1,19 @@
-"""FP8 block linears on the 1024^2 edit (S_txt 544 + S_img 8192 = 8736 tokens, d 3072, 19 + 38 blocks, B = 1), H100.
+"""FP8 block linears and attention on the 1024^2 edit (S_txt 544 + S_img 8192 = 8736 tokens, d 3072, 19 + 38 blocks,
+B = 1), H100.
 
-  step    per-step ms of one transformer forward with the AdaLN modulation hoisted (as the sampling loop runs it), bf16
-          and FP8 (enable_fp8) alternating within every round, reported as the range over --rounds rounds, with the
-          denoise-only images/s that implies (28 steps) and torch.cuda.max_memory_allocated of each configuration
+  step    per-step ms of one transformer forward with the AdaLN modulation hoisted (as the sampling loop runs it), in four
+          configurations alternating within every round: bf16, fp8 (enable_fp8: linears), fp8+attn (linears and
+          attention) and attn (enable_fp8(linears=False, attention=True)), reported as the range over --rounds rounds,
+          with the denoise-only images/s that implies (28 steps) and torch.cuda.max_memory_allocated of each
+  attn    TFLOP/s (4 S^2 d per call) of bf16 b2f_attention_fwd and FP8 b2f_attention_fp8 at the loop shape (B 1, H 24,
+          S 8736), alternating, and the ms of the b2f_attn_quant_fp8 pass that feeds the FP8 kernel; each timed window
+          is ATTN_ITERS back-to-back calls (about a quarter of a second), so one round's ratio is not a 30 ms sample
   gemm    TFLOP/s of the bf16 GEMM (b2f_gemm_bf16) and the FP8 GEMM (b2f_gemm_fp8) on each loop shape, alternating
   quant   ms of the launches FP8 adds or replaces per forward: b2f_ln_modulate_fp8 against b2f_ln_modulate, and the
           b2f_quant_fp8_rows launches over cat's [0, d), [d, 5d) and [0, 5d) columns, times their count per forward
 The card's name and power limit are read in the same process.
 
-  python scripts/bench_fp8.py [--rounds 3] [--iters 5] [--out-dir bench_out]
+  python scripts/bench_fp8.py [--rounds 3] [--iters 5] [--what step,attn,gemm,quant] [--out-dir bench_out]
 """
 import argparse
 import json
@@ -24,6 +29,7 @@ sys.path.insert(0, str(Path(__file__).resolve().parent))
 from bench_lora import card, timed  # noqa: E402
 
 S_TXT, N_IMG, D = 544, 4096, 3072
+ATTN_ITERS = 200
 S = S_TXT + 2 * N_IMG
 
 
@@ -48,13 +54,14 @@ def step_bench(args):
     m.prepare_schedule(inp["timestep"], inp["guidance"], inp["pooled_projections"])
     jak = {"_b2f_schedule_step": 0, "_b2f_out_rows": N_IMG}
     f = lambda: m(**inp, joint_attention_kwargs=jak, return_dict=False)
-    per = {"bf16": [], "fp8": []}
-    peak = {"bf16": 0, "fp8": 0}
+    confs = {"bf16": None, "fp8": dict(), "fp8+attn": dict(attention=True), "attn": dict(linears=False, attention=True)}
+    per = {c: [] for c in confs}
+    peak = {c: 0 for c in confs}
     outs = {}
     for rnd in range(args.rounds):
-        for conf in ("bf16", "fp8"):
-            if conf == "fp8":
-                m.enable_fp8()
+        for conf, kw in confs.items():
+            if kw is not None:
+                m.enable_fp8(**kw)
             torch.cuda.synchronize()
             torch.cuda.reset_peak_memory_stats()
             for _ in range(args.warmup):
@@ -63,11 +70,13 @@ def step_bench(args):
             peak[conf] = max(peak[conf], torch.cuda.max_memory_allocated())
             m.disable_fp8()
         print(f"round {rnd}: " + ", ".join(f"{c} {per[c][-1]:.1f} ms" for c in per), flush=True)
-    a, b = outs["fp8"].double(), outs["bf16"].double()
+    b = outs["bf16"].double()
     res = {c: {"step_ms": _rng(v), "denoise_img_per_s": [1000 / (28 * max(v)), 1000 / (28 * min(v))],
                "max_memory_allocated_GB": peak[c] / 1e9} for c, v in per.items()}
-    res["fp8_vs_bf16_time"] = _rng([x / y for x, y in zip(per["fp8"], per["bf16"])])
-    res["fp8_vs_bf16_output_rel_l2"] = ((a - b).norm() / b.norm()).item()
+    for c in ("fp8", "fp8+attn", "attn"):
+        a = outs[c].double()
+        res[f"{c}_vs_bf16_time"] = _rng([x / y for x, y in zip(per[c], per["bf16"])])
+        res[f"{c}_vs_bf16_output_rel_l2"] = ((a - b).norm() / b.norm()).item()
     del m, outs
     torch.cuda.empty_cache()
     return res
@@ -98,6 +107,35 @@ def gemm_bench(args):
         print(name, json.dumps(row), flush=True)
         del x, w, xq, wq, y
     return out
+
+
+def attn_bench(args):
+    from gpt_image_edit_b200 import ops
+    H = D // 128
+    g = torch.Generator(device="cuda").manual_seed(5)
+    # the model's layout: q, k, v as column slices of one qkv [1, S, 3d] buffer, out into cat [1, S, 5d]; q / k with
+    # the spread RMSNorm + RoPE leave them (unit rms per head)
+    qkv = torch.randn(1, S, 3 * D, device="cuda", generator=g).bfloat16()
+    q, k, v = (qkv[:, :, i * D:(i + 1) * D].unflatten(-1, (H, 128)) for i in range(3))
+    cat = torch.empty(1, S, 5 * D, device="cuda", dtype=torch.bfloat16)
+    bufs = ops.attn_quant_fp8(q, k, v)
+    runs = {"bf16": lambda: ops.attention(q, k, v, out=cat[:, :, :D]),
+            "fp8": lambda: ops.attention_fp8(*bufs, out=cat[:, :, :D]),
+            "quant": lambda: ops.attn_quant_fp8(q, k, v, q8=bufs[0], k8=bufs[1], sq=bufs[2], sk=bufs[3], v8t=bufs[4],
+                                                sv=bufs[5])}
+    t = {k_: [] for k_ in runs}
+    for _ in range(args.rounds):
+        for k_, fn in runs.items():
+            fn()
+            t[k_].append(timed(fn, ATTN_ITERS))
+    fl = 4.0 * S * S * D
+    res = {"shape": f"B1 H{H} S{S}", "bf16_tflops": [fl / max(t["bf16"]) / 1e9, fl / min(t["bf16"]) / 1e9],
+           "fp8_tflops": [fl / max(t["fp8"]) / 1e9, fl / min(t["fp8"]) / 1e9],
+           "bf16_ms": _rng(t["bf16"]), "fp8_ms": _rng(t["fp8"]), "quant_ms": _rng(t["quant"]),
+           "fp8_speedup": _rng([a / c for a, c in zip(t["bf16"], t["fp8"])]),
+           "fp8_plus_quant_speedup": _rng([a / (c + e) for a, c, e in zip(t["bf16"], t["fp8"], t["quant"])])}
+    print("attn", json.dumps(res), flush=True)
+    return res
 
 
 def quant_bench(args):
@@ -139,7 +177,7 @@ def main():
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--warmup", type=int, default=2)
-    ap.add_argument("--what", default="step,gemm,quant")
+    ap.add_argument("--what", default="step,attn,gemm,quant")
     ap.add_argument("--out-dir", default="bench_out")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -147,6 +185,8 @@ def main():
     res = {"card_before": card(), "time": time.strftime("%Y-%m-%d %H:%M:%S")}
     if "step" in args.what:
         res["step"] = step_bench(args)
+    if "attn" in args.what:
+        res["attn"] = attn_bench(args)
     if "gemm" in args.what:
         res["gemm"] = gemm_bench(args)
     if "quant" in args.what:

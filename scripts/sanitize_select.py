@@ -27,6 +27,9 @@ WANT = [
                                      "test_attention_matches_fp32_reference[2-2-2-640-640-False]",
                                      "test_attention_matches_fp32_reference[1-4-2-768-1000-False]",
                                      "test_attention_matches_fp32_reference[1-4-2-384-384-True]", "test_attention_peaked_softmax_rows"]),
+    # FP8 attention: the amax / quantize / scale passes and the e4m3 kernel with its 16 KB tiles and two slots
+    ("tests/test_attn_fp8_gpu.py", ["test_attn_quant_fp8_bit_exact[3-129]", "test_attention_fp8_matches_emulation[2-129]",
+                                    "test_attention_fp8_matches_emulation[1-255]", "test_attention_fp8_refusals"]),
     ("tests/test_elementwise_gpu.py", ["test_ln_modulate_matches_eager_chain[1-33-256]", "test_ln_modulate_matches_eager_chain[2-300-3072]",
                                        "test_rmsnorm_rope_matches_eager_chain", "test_euler_step_bit_exact"]),
     ("tests/test_vae_gpu.py", ["test_conv3x3_matches_torch[1-8-16-64-128-1]", "test_conv3x3_matches_torch[1-33-50-64-256-1]",
