@@ -66,4 +66,10 @@ struct FluxCtx {
   std::map<std::string, std::pair<float*, int64_t>> grads;
 };
 
+// b2f_flux_forward (flux_model.cu) after the handle cast.  x0, when set, receives the image rows of h right after the
+// embedders ([B, S_img, d] contiguous): the first-block cache (flux_cache.cu) compares block 0's output with them.
+int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mod, int64_t mod_ld, void* out, int B,
+                 int S_img, int S_txt, int n_out_rows, void* ws, size_t ws_bytes, int first_block, int last_block,
+                 bf16_t* x0, cudaStream_t st);
+
 }  // namespace b2f

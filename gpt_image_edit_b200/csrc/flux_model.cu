@@ -519,7 +519,18 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
                      int64_t mod_ld, void* out, int B, int S_img, int S_txt, int n_out_rows,
                      void* ws, size_t ws_bytes, int first_block, int last_block,
                      b2f_stream_t stream_) {
-  FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
+  return flux_forward(reinterpret_cast<FluxCtx*>(h), hidden, enc, mod, mod_ld, out, B, S_img, S_txt, n_out_rows, ws,
+                      ws_bytes, first_block, last_block, nullptr, static_cast<cudaStream_t>(stream_));
+}
+
+}  // extern "C"
+
+namespace b2f {
+
+int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mod, int64_t mod_ld, void* out, int B,
+                 int S_img, int S_txt, int n_out_rows, void* ws, size_t ws_bytes, int first_block, int last_block,
+                 bf16_t* x0, cudaStream_t st) {
+  b2f_flux* h = reinterpret_cast<b2f_flux*>(c);
   if (!c || !c->finalized) return B2F_ERR_INVALID;
   if (!hidden || !enc || !mod || !out || !ws || B <= 0 || S_img <= 0 || S_txt <= 0)
     return B2F_ERR_INVALID;
@@ -530,7 +541,6 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
     return B2F_ERR_INVALID;
   }
   if (ws_bytes < b2f_flux_workspace_bytes(h, B, S_img, S_txt)) return B2F_ERR_WORKSPACE;
-  cudaStream_t st = static_cast<cudaStream_t>(stream_);
   const b2f_flux_cfg& g = c->cfg;
   const int64_t d = c->d;
   const int H = g.num_heads;
@@ -601,6 +611,10 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
                 d, h_bs, B, S_img, (int)d, g.in_channels, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
     RUN(lin_fwd(c->context_embedder, tb, ls, enc, g.joint_dim, (int64_t)S_txt * g.joint_dim, g.joint_dim, h_txt, d,
                 h_bs, B, S_txt, (int)d, g.joint_dim, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st));
+    if (x0)   // the first-block cache's x0: the image rows of h before block 0, [B, S_img, d] contiguous
+      RUN(cuda_err(cudaMemcpy2DAsync(x0, (size_t)S_img * d * 2, h_img, (size_t)h_bs * 2, (size_t)S_img * d * 2, B,
+                                     cudaMemcpyDeviceToDevice, st),
+                   "flux_forward: x0 copy"));
   }
 
   for (int blk = first_block; blk < last_block; ++blk) {
@@ -682,4 +696,4 @@ int b2f_flux_forward(b2f_flux* h, const void* hidden, const void* enc, const voi
   return B2F_OK;
 }
 
-}  // extern "C"
+}  // namespace b2f

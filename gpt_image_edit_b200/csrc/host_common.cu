@@ -29,7 +29,7 @@ extern "C" const char* b2f_strerror(int code) {
   }
 }
 
-extern "C" int b2f_version(void) { return 4; }
+extern "C" int b2f_version(void) { return 5; }
 
 extern "C" int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin) {
   int n = 0;

@@ -11,7 +11,9 @@ accept the diffusers names (SURVEY.md A.6) as views, so checkpoints interchange.
 from __future__ import annotations
 
 import ctypes as C
+import math
 from collections import OrderedDict
+from dataclasses import dataclass
 from types import SimpleNamespace
 
 import torch
@@ -38,6 +40,51 @@ class FluxTransformerConfig(SimpleNamespace):
 
 class Transformer2DModelOutput(SimpleNamespace):
     pass
+
+
+@dataclass(frozen=True)
+class FirstBlockCacheConfig:
+    """First-block cache (`B200FluxTransformer2DModel.enable_cache`; the shape of diffusers' later
+    `FirstBlockCacheConfig`): a forward whose block-0 residual moved by less than `threshold` (relative L1 distance to the
+    last step that ran in full, pooled over the batch) skips the other blocks and reuses their residual from that step.
+    0 never skips; +inf skips every step after the first of a run."""
+    threshold: float
+
+    def __post_init__(self):
+        t = float(self.threshold)
+        if math.isnan(t) or t < 0:
+            raise ValueError(f"FirstBlockCacheConfig: threshold must be >= 0 (got {self.threshold})")
+
+
+class _CacheState:
+    """One branch's b2f_flux_cache over device memory owned here."""
+
+    def __init__(self):
+        self.mem = None
+        self.h = None
+        self.key = None
+        self.calls = 0
+
+    def ensure(self, nbytes: int, device):
+        if self.mem is not None and self.mem.numel() >= nbytes:
+            return
+        self.close()
+        self.mem = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        h = C.c_void_p()
+        check(_lib.lib.b2f_flux_cache_create(C.byref(h), ptr(self.mem), nbytes), "b2f_flux_cache_create")
+        self.h = h
+
+    def reset(self):
+        if self.h:
+            check(_lib.lib.b2f_flux_cache_reset(self.h), "b2f_flux_cache_reset")
+        self.key = None
+        self.calls = 0
+
+    def close(self):
+        if self.h and _lib is not None and getattr(_lib, "lib", None) is not None:
+            _lib.lib.b2f_flux_cache_destroy(self.h)
+        self.h = None
+        self.mem = None
 
 
 def _fused_layout(cfg: FluxTransformerConfig):
@@ -146,9 +193,15 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         self.gradient_checkpointing = False
         self._fp8 = None   # bound name -> (e4m3 weight, fp32 scales) while FP8 is enabled
         self._fp8_attn = False
+        self._cache_cfg = None      # FirstBlockCacheConfig while the first-block cache is on
+        self._cache_states = {}     # branch name -> _CacheState
+        self._cache_epoch = 0       # bumped by every change of the weights or FP8 switches
+        self.cache_log = []         # one dict(branch, step, dist, hit) per cached forward since cache_reset()
         self._lora_init()
 
     def __del__(self):
+        for st in getattr(self, "_cache_states", {}).values():
+            st.close()
         h = getattr(self, "_h", None)
         if h and _lib is not None and getattr(_lib, "lib", None) is not None:  # not during interpreter teardown
             _lib.lib.b2f_flux_destroy(h)
@@ -178,6 +231,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
                         raise RuntimeError(f"{k}: shape {tuple(sd[k].shape)} != {tuple(v.shape)}")
                     v.copy_(sd[k])
         self._fp8_requantize()
+        self._cache_epoch += 1
         return SimpleNamespace(missing_keys=missing, unexpected_keys=unexpected)
 
     @torch.no_grad()
@@ -197,6 +251,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
                     n = min(step, flat.numel() - o)
                     flat[o:o + n] = (torch.randn(n, device=self.device, generator=g) * s_).to(torch.bfloat16)
         self._fp8_requantize()
+        self._cache_epoch += 1
         return self
 
     def named_parameters_diffusers(self):
@@ -245,6 +300,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         if attention and not self._fp8_attn:
             check(_lib.lib.b2f_flux_set_fp8_attention(self._h, 1), "b2f_flux_set_fp8_attention")
             self._fp8_attn = True
+        self._cache_epoch += 1
         return self
 
     def _enable_fp8_linears(self):
@@ -264,6 +320,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
 
     def disable_fp8(self):
         """Back to bf16 block linears and attention; the FP8 weight copies are released."""
+        self._cache_epoch += 1
         if self._fp8_attn:
             check(_lib.lib.b2f_flux_set_fp8_attention(self._h, 0), "b2f_flux_set_fp8_attention")
             self._fp8_attn = False
@@ -285,6 +342,80 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
             w = self._store[name + ".weight"]
             check(_lib.lib.b2f_quant_fp8_rows(ptr(w), w.stride(0), 0, ptr(w8), w8.stride(0), 0, ptr(ws), 0, 1,
                                               w.shape[0], w.shape[1], stream_ptr()), f"b2f_quant_fp8_rows {name}")
+
+    # ------------------------------------------------------------------ first-block cache
+    @property
+    def cache_enabled(self) -> bool:
+        return self._cache_cfg is not None
+
+    def enable_cache(self, config: FirstBlockCacheConfig):
+        """Turn on the first-block cache (include/b2f.h, b2f_flux_forward_cached): every full forward runs the
+        embedders and block 0, and skips blocks 1.. when block 0's residual moved by less than `config.threshold` since
+        the last step of the same branch that ran in full.  An approximation whose hit rate and image quality depend on
+        the checkpoint.  The decision is taken for the whole batch, so an item's result can depend on its batch-mates.
+        Each branch (joint_attention_kwargs["_b2f_cache_branch"]; FluxKontextPipeline routes the positive forward as
+        "cond", the true-CFG negative one as "uncond") keeps its own state of about 10 d bytes per image token plus 4 d
+        per output token (302 MB at 1024^2, B = 1).  A cached forward waits on the device once (it reads the decision
+        back), so it cannot be captured into a CUDA graph."""
+        if not isinstance(config, FirstBlockCacheConfig):
+            raise TypeError("enable_cache takes a FirstBlockCacheConfig")
+        self._cache_cfg = config
+        self.cache_reset()
+        return self
+
+    def disable_cache(self):
+        """Back to uncached forwards; the states' memory is released."""
+        self._cache_cfg = None
+        for st in self._cache_states.values():
+            st.close()
+        self._cache_states = {}
+        self.cache_log = []
+        return self
+
+    def cache_reset(self):
+        """Invalidate every branch's state and clear `cache_log` (FluxKontextPipeline calls this at the start of each
+        call, so every image starts with a full step)."""
+        for st in self._cache_states.values():
+            st.reset()
+        self.cache_log = []
+
+    def _cache_forward(self, jak, lora_scale, hs, enc, mod, out, B, S_img, S_txt, n_out, ws, nws):
+        branch = str(jak.get("_b2f_cache_branch", "default"))
+        st = self._cache_states.get(branch)
+        if st is None:
+            st = self._cache_states[branch] = _CacheState()
+        st.ensure(int(_lib.lib.b2f_flux_cache_bytes(self._h, B, S_img, S_txt, n_out)), self.device)
+        key = (self._cache_epoch, self._lora_version, lora_scale)
+        if st.key != key:   # weights, adapters, LoRA scale or FP8 switches changed what the blocks compute
+            check(_lib.lib.b2f_flux_cache_reset(st.h), "b2f_flux_cache_reset")
+            st.key = key
+        hit, dist = C.c_int(), C.c_float()
+        check(_lib.lib.b2f_flux_forward_cached(self._h, st.h, float(self._cache_cfg.threshold), ptr(hs), ptr(enc),
+                                               ptr(mod), mod.stride(0), ptr(out), B, S_img, S_txt, n_out, ptr(ws), nws,
+                                               C.byref(hit), C.byref(dist), stream_ptr()), "b2f_flux_forward_cached")
+        self.cache_log.append(dict(branch=branch, step=st.calls, dist=float(dist.value), hit=bool(hit.value)))
+        st.calls += 1
+
+    def debug_cache(self, branch: str, B: int, S_img: int, n_out: int) -> SimpleNamespace:
+        """Views of one branch's cache state in include/b2f.h's layout: r (the slot holding r_prev) and r_other [B,
+        S_img, d] fp32, R [B, n_out, d] fp32, y0 [B, S_img, d] bf16 (block 0's output rows of the last call), and
+        `valid`.  For tests; only for reading."""
+        st = self._cache_states[branch]
+        valid, slot = C.c_int(), C.c_int()
+        check(_lib.lib.b2f_flux_cache_state(st.h, C.byref(valid), C.byref(slot)), "b2f_flux_cache_state")
+        a = lambda n: (n + 255) // 256 * 256
+        d = self.inner_dim
+        N = B * S_img * d
+        off = (-st.mem.data_ptr()) % 256
+        o_r1 = a(4 * N)
+        o_R = o_r1 + a(4 * N)
+        o_p = o_R + a(4 * B * n_out * d)
+        o_xy = o_p + a(16 * ((B * S_img + 7) // 8)) + 256
+        m = st.mem[off:]
+        r = [m[0:4 * N].view(torch.float32).view(B, S_img, d), m[o_r1:o_r1 + 4 * N].view(torch.float32).view(B, S_img, d)]
+        return SimpleNamespace(valid=bool(valid.value), r=r[slot.value], r_other=r[1 - slot.value],
+                               R=m[o_R:o_R + 4 * B * n_out * d].view(torch.float32).view(B, n_out, d),
+                               y0=m[o_xy:o_xy + 2 * N].view(torch.bfloat16).view(B, S_img, d))
 
     # ------------------------------------------------------------------ helpers
     def _workspace(self, nbytes: int, tag) -> torch.Tensor:
@@ -396,6 +527,12 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         out = torch.empty((B, n_out, cfg.out_channels), device=self.device, dtype=torch.bfloat16)
         nws = int(_lib.lib.b2f_flux_workspace_bytes(self._h, B, S_img, S_txt))
         ws = self._workspace(nws, "fwd")
+        if self._cache_cfg is not None:
+            if "_b2f_block_range" in jak:
+                raise _lib.B2FError("_b2f_block_range with the first-block cache on: the cache runs whole forwards only "
+                                    "(disable_cache() first)")
+            self._cache_forward(jak, lora_scale, hs, enc, mod, out, B, S_img, S_txt, n_out, ws, nws)
+            return (out,) if not return_dict else Transformer2DModelOutput(sample=out)
         first, last = jak.get("_b2f_block_range", (0, -1))
         check(_lib.lib.b2f_flux_forward(self._h, ptr(hs), ptr(enc), ptr(mod), mod.stride(0), ptr(out), B, S_img,
                                         S_txt, n_out, ptr(ws), nws, int(first), int(last), stream_ptr()),

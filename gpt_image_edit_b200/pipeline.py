@@ -12,6 +12,8 @@ What this file adds over the reference loop, without changing results:
     (`transformer.prepare_schedule`), when the transformer offers it;
   * the transformer is asked for the target tokens only (the reference slices them afterwards,
     flux_pipeline.py:1078), so the Euler update reads a contiguous tensor.
+With the transformer's opt-in first-block cache on (`enable_cache`), results change by design: each call resets the
+cache and routes the positive forward as branch "cond", the true-CFG negative forward as "uncond".
 """
 from __future__ import annotations
 
@@ -511,6 +513,11 @@ class FluxKontextPipeline:
             sched_kw = {"lora_scale": float(jak["scale"])} if "scale" in jak else {}
             self.transformer.prepare_schedule(timesteps.to(dtype) / 1000, guidance, pooled_prompt_embeds, **sched_kw)
             jak["_b2f_out_rows"] = n_tgt
+            # first-block cache: every call starts from a full step; the positive and the true-CFG negative forward
+            # each keep their own state
+            jak["_b2f_cache_branch"] = "cond"
+            if hasattr(self.transformer, "cache_reset"):
+                self.transformer.cache_reset()
 
         self.scheduler.set_begin_index(0)
         for i, t in enumerate(timesteps):
@@ -529,6 +536,8 @@ class FluxKontextPipeline:
             if do_true_cfg:
                 # the hoisted modulation belongs to the positive pooled vector: the negative forward computes its own
                 neg_jak = {k: v for k, v in jak.items() if k != "_b2f_schedule_step"}
+                if hoist:
+                    neg_jak["_b2f_cache_branch"] = "uncond"
                 neg_noise_pred = self.transformer(
                     hidden_states=x_in, timestep=timestep / 1000, guidance=guidance,
                     pooled_projections=negative_pooled_prompt_embeds, encoder_hidden_states=negative_prompt_embeds,

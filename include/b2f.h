@@ -34,7 +34,7 @@ typedef void* b2f_stream_t; /* cudaStream_t */
 
 const char* b2f_strerror(int code);
 /* ABI version; bumped on any signature change or addition (2: LoRA entry points, 3: FP8 entry points, 4: FP8
- * attention). */
+ * attention, 5: first-block cache). */
 int b2f_version(void);
 /* Device facts the host needs for grid sizing / reporting. Returns B2F_ERR_NODEVICE without GPU. */
 int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin);
@@ -445,6 +445,57 @@ int b2f_flux_set_fp8(b2f_flux* ctx, int on);
  * q8, k8, v8t and their scales, and the training entry points refuse.  Unfused LoRA adapters stay allowed (they act on
  * the linears only).  b2f_flux_finalize switches it off. */
 int b2f_flux_set_fp8_attention(b2f_flux* ctx, int on);
+
+/* First-block cache (opt-in; the approach of ParaAttention's FBCache / diffusers' FirstBlockCacheConfig, with this
+ * engine's own semantics and rounding points).  Consecutive Euler steps change the hidden states little, so when block
+ * 0's residual barely moved since the last step that ran in full, blocks 1..nblk-1 are skipped and their residual from
+ * that step is reused.  An approximation: how often it hits and what it does to images depend on the checkpoint.
+ *
+ * A cached forward on cache state C (full block range only):
+ *   1. Head.  The embedders and block 0 run exactly as in b2f_flux_forward.  x0 = the image-stream rows of h after
+ *      x_embedder (all S_img rows, target and context, bf16), y0 = the same rows after block 0,
+ *      r_k = float(y0) - float(x0) in fp32.
+ *   2. Distance.  If C holds a full step with the same (ctx, B, S_img, S_txt, n_out_rows):
+ *        dist = sum |r_k - r_prev| / sum |r_prev|   over all B * S_img * d elements, pooled over the batch,
+ *      summed in a fixed order: fp32 per thread over its elements, the 256 threads of a CTA (8 rows each) by a fixed
+ *      fp64 tree, then the per-CTA partials in fp64 (each thread of one CTA over CTAs t, t + 256, ... in index order,
+ *      then a fixed tree), dist = fp32(num / den).  No float atomics: dist is bit-reproducible run to run.
+ *   3. Hit iff dist < threshold (strict: threshold 0 never hits).  NaN or infinite dist is a miss, and so is
+ *      sum |r_prev| == 0.  A call without a valid state is a miss.
+ *   4. Hit.  Blocks 1..nblk-1 are skipped; h' = bf16(float(y0[:n_out]) + R) (round to nearest) is written over the
+ *      first n_out_rows image rows of h, and norm_out / proj_out run on it exactly as the uncached tail runs on the final
+ *      h (so the sum is rounded to bf16 before the LayerNorm statistics).  C is left unchanged: the next step is
+ *      compared with the last FULL step, not with this one.
+ *   5. Miss.  Blocks 1..nblk-1 and the tail run unchanged: the output is bit-identical to b2f_flux_forward's.  Then
+ *      R = float(h_final[:n_out]) - float(y0[:n_out]) (fp32), r_prev = r_k (fp32), and C records the shapes.
+ * The decision is taken for the whole batch: with the cache on, an item's result can depend on its batch-mates.
+ *
+ * Memory.  The caller owns all of it; nothing is allocated inside the forward.  b2f_flux_cache_bytes gives the size
+ * for one shape (0 for an invalid one):
+ *   2 x 4 B S_img d (r, two slots) + 4 B n_out d (R) + 16 ceil(B S_img / 8) (partials) + 2 B S_img d (x0 / y0 scratch)
+ * plus 256-byte alignment of each region: about 100.7 + 100.7 + 50.3 + 50.3 MB at 1024^2, B = 1 (d 3072, S_img 8192,
+ * n_out 4096).  Regions, in order from mem's first 256-aligned byte, each starting 256-aligned: r slot 0, r slot 1, R
+ * [B, n_out, d], partials, an 8-byte decision, the scratch (x0, overwritten with y0 by the distance pass).
+ * b2f_flux_cache_create makes a state over mem (borrowed) and allocates 8 bytes of pinned host memory for the
+ * decision; a state holds shapes up to its bytes.  b2f_flux_cache_reset invalidates it (the next call misses): do so
+ * whenever what the blocks compute changes (weights, adapters, LoRA scale, FP8 switches).  A call with other shapes
+ * than the state's invalidates it itself.  b2f_flux_cache_state reports whether the state is valid and which r slot
+ * holds r_prev (the other one holds the r_k of a call that hit).
+ *
+ * b2f_flux_forward_cached takes b2f_flux_forward's arguments minus the block range.  It is the one entry point that
+ * waits on the device: with a valid state it reads (dist, hit) back, 8 bytes, and synchronises the stream once per
+ * call, so it cannot be captured into a CUDA graph (b2f_flux_forward stays capturable).  *hit and *dist receive the
+ * decision (dist NaN when there was no valid state).  threshold < 0 or NaN: B2F_ERR_INVALID; +inf is allowed and means
+ * "hit whenever there is a state". */
+typedef struct b2f_flux_cache b2f_flux_cache;
+size_t b2f_flux_cache_bytes(const b2f_flux* ctx, int B, int S_img, int S_txt, int n_out_rows);
+int b2f_flux_cache_create(b2f_flux_cache** out, void* mem, size_t bytes);
+void b2f_flux_cache_destroy(b2f_flux_cache* cache);
+int b2f_flux_cache_reset(b2f_flux_cache* cache);
+int b2f_flux_cache_state(const b2f_flux_cache* cache, int* valid, int* r_slot);
+int b2f_flux_forward_cached(b2f_flux* ctx, b2f_flux_cache* cache, float threshold, const void* hidden, const void* enc,
+                            const void* mod, int64_t mod_ld, void* out, int B, int S_img, int S_txt, int n_out_rows,
+                            void* ws, size_t ws_bytes, int* hit, float* dist, b2f_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * Kernels of the Qwen2.5-VL conditioning prefill (transformers Qwen2_5_VL*, SURVEY.md Appendix B;

@@ -14,6 +14,8 @@ WANT = [
                                 "test_lora_gemm_qkv_norm_rope[True]", "test_lora_fuse_kernel"]),
     # the composed forward's workspace offsets, pitches and split rows, stage by stage (d 256, B 3, one text token)
     ("tests/test_flux_blocks_gpu.py", ["test_stagewise_forward_matches_fp64[toy_text_of_one]"]),
+    # the first-block cache's residual / distance / apply / capture kernels (d 256, B 3, one text token)
+    ("tests/test_flux_cache_gpu.py", ["test_cached_forward_equals_the_engines_stages[toy]"]),
     ("tests/test_train_kernels_gpu.py", ["test_gemm_dgrad[1-128-128-64]", "test_gemm_dgrad[1-200-136-72]", "test_gemm_dgrad[2-300-256-512]",
                                          "test_gemm_dgrad[2-1024-1024-4096]", "test_gemm_dgrad_pitched_views_and_epilogues",
                                          "test_gemm_wgrad[1-64-128-128]", "test_gemm_wgrad[1-100-136-200]", "test_gemm_wgrad[3-150-256-384]",

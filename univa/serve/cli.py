@@ -261,6 +261,9 @@ def main(args):
     pipe, tokenizers, text_encoders = load_pipe(model.denoise_tower.denoiser, args.flux_path, device, args.synthetic, args.small)
     if getattr(args, "fp8", False) or getattr(args, "fp8_attention", False):
         pipe.transformer.enable_fp8(linears=getattr(args, "fp8", False), attention=getattr(args, "fp8_attention", False))
+    if getattr(args, "cache_threshold", None) is not None:
+        from gpt_image_edit_b200.flux_transformer import FirstBlockCacheConfig
+        pipe.transformer.enable_cache(FirstBlockCacheConfig(threshold=args.cache_threshold))
     session = ChatSession(args, model, task_head, pipe, processor, tokenizers, text_encoders, device)
 
     if args.prompt is not None or args.image is not None:       # one non-interactive turn
@@ -304,6 +307,9 @@ def build_parser():
                    "tensor cores, per-head Q / K and per-channel V scales); combines with --fp8.  Faster, but heads "
                    "with peaked attention lose accuracy (e4m3 scores: about 13%% rel-L2 on peaked synthetic heads, "
                    "against 0.2%% in bf16), which can show in the image")
+    p.add_argument("--cache-threshold", type=float, default=None, help="first-block cache of the denoiser (off when "
+                   "absent): skip blocks 1.. on steps whose block-0 residual moved by less than this relative L1 "
+                   "distance since the last full step.  An approximation; its effect on images depends on the checkpoint")
     p.add_argument("--prompt", type=str, default=None)
     p.add_argument("--image", type=str, default=None)
     p.add_argument("--output", type=str, default="output.png")
