@@ -12,7 +12,12 @@
 //                         act/gate/resid → global with 16-byte accesses, 16 threads per row; a fused QKV head runs one
 //                         thread per row; the fp32 wgrad output goes straight from registers
 //
-// Every output element sees the same k16 accumulation order as a one-tile-per-CTA kernel with the same k-blocks.
+// gemm_wide_kernel     the plain forward GEMM on 128 x 256 tiles for the loop's large linears: both consumers on one tile,
+//                      one m64n256k16 each per k16 step, a 3-stage ring of 48 KB stages; launch_gemm picks the tile per
+//                      launch from the shape (tile_width)
+//
+// Every output element sees the same k16 accumulation order as a one-tile-per-CTA kernel with the same k-blocks, on
+// either tile.
 // Both operands of the forward GEMM are K-major ([rows, K] row-major), which is what nn.Linear stores
 // (SURVEY.md A.6) — no transposes anywhere.  The tile shape and ring layout are shared with conv.cu (gemm_sm90.cuh).
 //
@@ -608,6 +613,233 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   }
 }
 
+// ---------------------------------------------------------------------------------------------------- the wide tile
+// The plain forward GEMM (MODE 0, bf16, no LoRA, no FP8) on 128 x 256 tiles, for the large linears of the denoising
+// loop.  Both consumer warpgroups work on the same tile: consumer c owns rows [64 c, 64 c + 64) and issues one
+// m64n256k16 per k16 step, 128 fp32 accumulators per thread as in the ping-pong kernel.  Per unit of tensor work this
+// reads about 17 % fewer operand bytes from shared memory (2 KB of A and 8 KB of W per 64 x 256 x 16 MACs instead of
+// 2 + 4 KB per 64 x 128 x 16) and moves 25 % fewer bytes through L2 and TMA (48 KB per 128 x 256 x 64 tile-k-block
+// instead of 32 KB per 128 x 128 x 64).  The price is that the epilogues no longer overlap the MMAs; the producer still
+// streams the next tile's first k-blocks into the ring while they run.  Each consumer runs the epilogue of its own 64
+// rows, so the two consumers meet only at the ring's barriers.
+// A stage is 48 KB: three stages and a 128 x (256 + 8) bf16 staging tile take 210 KB of the 227 KB (211 KB with the
+// barriers and the alignment pad); a fourth stage would leave room for only half the staging tile.  W arrives as two
+// 128-row TMA boxes, so both tiles share one W map.
+// Every output element sees the same k16 steps in the same order, and the same rounding chain from x = bf16(acc + bias),
+// as on the 128 x 128 tile.
+// Sharing the W tile across a 2-CTA cluster along M (each CTA loads its A tile and half of W, multicast to both; each
+// consumer warp releases a stage to both CTAs' empty barriers; grid from cudaOccupancyMaxActiveClusters, which gave 66)
+// was built and gave bit-identical results, but ran 26-48 % slower on the loop's shapes (sustained TFLOP/s, H100 SXM
+// 80 GB, 700 W, cluster against this kernel: proj_out 405-406 / 606-611, ff2 433-434 / 653-660, ff1 428-431 / 576-578,
+// to_out 410-412 / 560, single-block qkv+mlp 409-410 / 548-554, text ff1 227-230 / 433-439), so each CTA loads its own
+// W tile.
+constexpr int WIDE_N = 256;
+constexpr int WIDE_STAGES = 3;
+constexpr int WIDE_STAGE_BYTES = A_BYTES + WIDE_N * BLOCK_K * 2;
+constexpr int WIDE_SROW = WIDE_N * 2 + 16;   // as SROW: 16-byte accesses of 8 rows hit 32 banks
+constexpr int WIDE_SMEM_BYTES = WIDE_STAGES * WIDE_STAGE_BYTES + BLOCK_M * WIDE_SROW + 2 * WIDE_STAGES * 8 + 1024;
+static_assert(WIDE_SMEM_BYTES <= 227 * 1024, "wide tile exceeds the shared memory of an SM");
+
+__global__ void __launch_bounds__(THREADS, 1)
+gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* ring = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint64_t* full = reinterpret_cast<uint64_t*>(ring + WIDE_STAGES * WIDE_STAGE_BYTES + BLOCK_M * WIDE_SROW);
+  uint64_t* empty = full + WIDE_STAGES;
+  const int wg = threadIdx.x >> 7;
+  if (threadIdx.x == 0) {
+    tma_prefetch_desc(&tmA);
+    tma_prefetch_desc(&tmB);
+    for (int i = 0; i < WIDE_STAGES; ++i) {
+      mbar_init(&full[i], 1);
+      mbar_init(&empty[i], 8);   // one arrive per consumer warp: both consumers read every stage
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  const int num_tiles = p.num_m_blocks * p.num_n_blocks;
+  const int n_local = (num_tiles - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int num_kb = (p.K + BLOCK_K - 1) / BLOCK_K;
+
+  if (wg == 0) {
+    setmaxnreg_dec<PRODUCER_REGS>();
+    if (threadIdx.x == 0) {
+      int stage = 0;
+      uint32_t phase = 0;
+      for (int i = 0; i < n_local; ++i) {
+        int n_blk, bb, mb;
+        tile_origin(p, blockIdx.x + i * gridDim.x, n_blk, bb, mb);
+        for (int kb = 0; kb < num_kb; ++kb) {
+          mbar_wait(&empty[stage], phase ^ 1);
+          uint8_t* sa = ring + stage * WIDE_STAGE_BYTES;
+          uint8_t* sb = sa + A_BYTES;
+          mbar_expect_tx(&full[stage], WIDE_STAGE_BYTES);
+          tma_load_3d(sa, &tmA, &full[stage], kb * BLOCK_K, mb * BLOCK_M, bb);
+          tma_load_2d(sb, &tmB, &full[stage], kb * BLOCK_K, n_blk * WIDE_N);
+          tma_load_2d(sb + B_BYTES, &tmB, &full[stage], kb * BLOCK_K, n_blk * WIDE_N + BLOCK_N);
+          if (++stage == WIDE_STAGES) {
+            stage = 0;
+            phase ^= 1;
+          }
+        }
+      }
+    }
+    return;
+  }
+  setmaxnreg_inc<CONSUMER_REGS>();
+
+  const int c = wg - 1;
+  const int tid = threadIdx.x & 127, w = tid >> 5, lane = tid & 31;
+  uint8_t* stg = ring + WIDE_STAGES * WIDE_STAGE_BYTES + 64 * c * WIDE_SROW;   // this consumer's 64 staged rows
+  const uint32_t ring_u = smem_u32(ring);
+  const uint64_t da0 = make_sdesc_sw128(ring_u + 8192 * c, 16, 1024);   // rows 64 c.. of the A tile start 8 KB c in
+  const uint64_t db0 = make_sdesc_sw128(ring_u + A_BYTES, 16, 1024);
+  int stage = 0;
+  uint32_t phase = 0;
+  for (int i = 0; i < n_local; ++i) {
+    int n_blk, bb, mb;
+    tile_origin(p, blockIdx.x + i * gridDim.x, n_blk, bb, mb);
+
+    float acc[128];
+#pragma unroll
+    for (int j = 0; j < 128; ++j) acc[j] = 0.f;
+    int prev = -1;
+    for (int kb = 0; kb < num_kb; ++kb) {
+      mbar_wait(&full[stage], phase);
+      const uint64_t soff = uint64_t((stage * WIDE_STAGE_BYTES) >> 4);
+      reg_fence(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < BLOCK_K / 16; ++k) {
+        const uint64_t ks = soff + uint64_t((k * 32) >> 4);
+        wgmma_m64n256_ss<0, 0>(acc, da0 + ks, db0 + ks, 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<1>();   // the previous stage's MMAs are complete: hand it back to the producer
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&empty[prev]);
+      }
+      prev = stage;
+      if (++stage == WIDE_STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    reg_fence(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+
+    // ---- epilogue of rows [64 c, 64 c + 64).  Accumulator element j of a thread is row 16 w + lane / 4 + 8 ((j / 2) & 1),
+    // column 8 (j / 4) + 2 (lane % 4) + (j & 1) of this consumer's rows.
+    const int r_lo = 16 * w + (lane >> 2);
+    named_bar_sync(BAR_EPI + c, 128);   // this consumer's previous epilogue is done reading the staging rows
+#pragma unroll
+    for (int j = 0; j < WIDE_N / 8; ++j) {
+      const int col = 8 * j + 2 * (lane & 3);
+      const int n = n_blk * WIDE_N + col;
+      const bool has_bias = p.bias && n < p.N;
+      const float2 b2 = has_bias ? unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n))) : make_float2(0.f, 0.f);
+      float x0 = acc[4 * j], x1 = acc[4 * j + 1], x2 = acc[4 * j + 2], x3 = acc[4 * j + 3];
+      if (has_bias) {
+        x0 += b2.x;
+        x1 += b2.y;
+        x2 += b2.x;
+        x3 += b2.y;
+      }
+      uint8_t* s0 = stg + r_lo * WIDE_SROW + col * 2;
+      *reinterpret_cast<uint32_t*>(s0) = pack_bf16x2(x0, x1);
+      *reinterpret_cast<uint32_t*>(s0 + 8 * WIDE_SROW) = pack_bf16x2(x2, x3);
+    }
+    named_bar_sync(BAR_EPI + c, 128);
+
+    const int n_tile0 = n_blk * WIDE_N;
+    const long long row_c = (long long)mb * BLOCK_M + 64 * c;   // first row of this consumer's half
+    const __nv_bfloat16* gate_row = p.gate ? p.gate + (long long)bb * p.gate_ld : nullptr;
+    int epi = p.epi;
+    __nv_bfloat16* out_base = p.out + bb * p.out_bs;
+    long long ld = p.ldc;
+    if (epi == B2F_EPI_QKV_NORM_ROPE) {
+      const int which = n_tile0 / p.d_model;   // d_model % 256 == 0: both heads of the tile are in the same block
+      if (which < 2) {
+        // two normalised heads per tile: one thread per (row, head)
+        const int r = tid & 63, h = tid >> 6;
+        const long long row = row_c + r;
+        if (row < p.M)
+          epilogue_head_norm_rope(p, stg + r * WIDE_SROW + h * 256, n_tile0 + 128 * h, row, out_base + row * ld,
+                                  which == 1);
+        continue;
+      }
+      const bool second = p.split_n > 0 && n_tile0 >= p.split_n;
+      epi = second ? p.epi2 : B2F_EPI_BIAS;
+      if (second) {
+        out_base = p.out2 + bb * p.out2_bs - p.split_n;
+        ld = p.ldc2;
+      }
+    }
+    // 32 threads per row, one 8-column group each: a warp reads and writes one 512-byte row segment.  Rows go in batches
+    // of 4 per thread, as in the ping-pong kernel.
+    const int n = n_tile0 + 8 * lane;
+    if (n < p.N) {
+      constexpr int RB = 4;
+      const bool reads_resid = epi == B2F_EPI_GATE_RESID || epi == B2F_EPI_RESID;
+      const uint4 gq = epi == B2F_EPI_GATE_RESID ? __ldg(reinterpret_cast<const uint4*>(gate_row + n))
+                                                 : make_uint4(0, 0, 0, 0);
+#pragma unroll 1
+      for (int rb = w; rb < 64; rb += 4 * RB) {   // staged rows rb + 4 r, r < RB
+        const long long row0 = row_c + rb;
+        if (row0 >= p.M) break;
+        uint4 rq[RB];
+#pragma unroll
+        for (int r = 0; r < RB; ++r) {
+          const long long row = row0 + 4 * r;
+          rq[r] = make_uint4(0, 0, 0, 0);
+          if (reads_resid && row < p.M)
+            rq[r] = *reinterpret_cast<const uint4*>(p.resid + bb * p.resid_bs + row * p.ldr + n);
+        }
+#pragma unroll
+        for (int r = 0; r < RB; ++r) {
+          const long long row = row0 + 4 * r;
+          if (row >= p.M) break;
+          float v[8];
+          unpack_bf16x8(*reinterpret_cast<const uint4*>(stg + (rb + 4 * r) * WIDE_SROW + lane * 16), v);
+          epilogue_group(epi, v, rq[r], gq, out_base + row * ld + n);
+        }
+      }
+    }
+  }
+}
+
+// 0: the launcher picks the tile; 128 / 256: b2f_gemm_set_tile_override forced it (tests and benchmarks).
+int g_tile_override = 0;
+
+// Time of one 128 x 256 tile over that of one 128 x 128 tile: WIDE_COST_LOOP + (WIDE_COST_EPI + WIDE_COST_NORM q) / K,
+// q the share of the columns that are RMS-normalised QKV heads.  The main loop of the wide tile runs faster per FLOP
+// (the constant part, below 2), but its epilogue no longer hides behind the other consumer's MMAs (the part that falls
+// with K; the one-thread-per-head norm epilogue exposes more).  Fitted to scripts/bench_kernels.py --what loop
+// --sustained on an H100 80GB HBM3 at 700 W: the ratio measured 1.89 (to_out, K 3072), 1.84 (ff1, K 3072), 1.98 (image
+// QKV, K 3072), 1.56 (ff2, K 12288) and 1.53 (proj_out, K 15360).
+constexpr double WIDE_COST_LOOP = 1.45, WIDE_COST_EPI = 1280.0, WIDE_COST_NORM = 530.0;
+
+// Tile width of a plain forward launch.  A persistent launch takes ceil(tiles / SMs) rounds of tiles, so the wide tile
+// wins where its rounds, each the cost ratio above times as long, add up to less.  On 132 SMs the single blocks'
+// proj_out (M 8736, N 3072) runs 828 wide tiles in 7 rounds against 1656 narrow ones in 13 (7 x 1.53 < 13) and goes
+// wide; the image QKV (2304 wide tiles in 18 rounds against 35, 18 x 1.98 > 35) and the M = 544 text linears with
+// N = 3072 or 9216 (no fewer rounds on the wide tile) stay on 128.  The fused QKV epilogue needs d_model % 256 == 0, so
+// that a wide tile never straddles the Q / K / V blocks.
+int tile_width(const GemmParams& p) {
+  if (p.epi == B2F_EPI_QKV_NORM_ROPE && p.d_model % WIDE_N) return BLOCK_N;
+  if (g_tile_override) return g_tile_override;
+  const int sms = device_info().num_sms;
+  const long long rounds128 = ((long long)p.num_m_blocks * ((p.N + BLOCK_N - 1) / BLOCK_N) + sms - 1) / sms;
+  const long long rounds256 = ((long long)p.num_m_blocks * ((p.N + WIDE_N - 1) / WIDE_N) + sms - 1) / sms;
+  const double q = p.epi == B2F_EPI_QKV_NORM_ROPE ? 2.0 * p.d_model / p.N : 0.0;
+  const double cost = WIDE_COST_LOOP + (WIDE_COST_EPI + WIDE_COST_NORM * q) / p.K;
+  return rounds256 * cost < rounds128 ? WIDE_N : BLOCK_N;
+}
+
 template <int MODE, bool LORA = false, bool FP8 = false>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream,
                 const LoraParams<LORA>& lx = LoraParams<LORA>{}, const Fp8Params<FP8>& fx = Fp8Params<FP8>{}) {
@@ -618,12 +850,17 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cu
     cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<MODE, LORA, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          PP_SMEM_BYTES);
     if (e != cudaSuccess) return cuda_err(e, "gemm smem attribute");
+    if (MODE == 0 && !LORA && !FP8) {
+      e = cudaFuncSetAttribute(gemm_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM_BYTES);
+      if (e != cudaSuccess) return cuda_err(e, "gemm smem attribute");
+    }
     attr_set = true;
   }
   p.m_blocks_per_batch = (p.M + BLOCK_M - 1) / BLOCK_M;
   p.num_m_blocks = p.batch * p.m_blocks_per_batch;
-  p.num_n_blocks = (p.N + BLOCK_N - 1) / BLOCK_N;
-  p.panel_n = 16;
+  const int tile_n = MODE == 0 && !LORA && !FP8 ? tile_width(p) : BLOCK_N;
+  p.num_n_blocks = (p.N + tile_n - 1) / tile_n;
+  p.panel_n = 16 * BLOCK_N / tile_n;   // the same W-panel footprint on either tile
   const int num_tiles = p.num_m_blocks * p.num_n_blocks;
   const int grid = std::min(num_tiles, device_info().num_sms);   // persistent: at most one CTA per SM
   int k_ext = 0;
@@ -634,7 +871,10 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cu
   }
   const double kk = MODE == 2 ? (double)p.kbatch * p.K : (double)p.K + k_ext;
   prof_begin(KC_GEMM, stream);
-  gemm_bf16_kernel<MODE, LORA, FP8><<<grid, THREADS, PP_SMEM_BYTES, stream>>>(tmA, tmB, p, lx, fx);
+  if (tile_n == WIDE_N)
+    gemm_wide_kernel<<<grid, THREADS, WIDE_SMEM_BYTES, stream>>>(tmA, tmB, p);
+  else
+    gemm_bf16_kernel<MODE, LORA, FP8><<<grid, THREADS, PP_SMEM_BYTES, stream>>>(tmA, tmB, p, lx, fx);
   {
     char tag_[96];
     const double ab = FP8 ? 1.0 : 2.0;   // bytes per A / W element
@@ -644,11 +884,11 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cu
       snprintf(tag_, sizeof tag_, "gemm lora %dx%dx%d+%d b%d e%d%s", p.M, p.N, p.K, k_ext, p.batch, p.epi,
                down ? " down" : "");
     else
-      snprintf(tag_, sizeof tag_, "gemm m%d %dx%dx%d b%d e%d", MODE, p.M, p.N, (int)kk, p.batch, p.epi);
+      snprintf(tag_, sizeof tag_, "gemm m%d %dx%dx%d b%d e%d t%d", MODE, p.M, p.N, (int)kk, p.batch, p.epi, tile_n);
     prof_end_tagged(KC_GEMM, stream, 2.0 * p.batch * (double)p.M * p.N * kk,
                     ab * ((double)p.batch * p.M * kk + (double)p.N * kk) + 2.0 * (double)p.batch * p.M * p.N, tag_);
   }
-  B2F_LAUNCHED("gemm_bf16_kernel", 1);
+  B2F_LAUNCHED(tile_n == WIDE_N ? "gemm_wide_kernel" : "gemm_bf16_kernel", 1);
   return B2F_OK;
 }
 
@@ -806,6 +1046,12 @@ extern "C" int b2f_gemm_bf16(const void* A, int64_t lda, int64_t a_bs, const voi
   if (epilogue == B2F_EPI_QKV_NORM_ROPE) return B2F_ERR_INVALID;  // needs the extended entry point
   return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, N, K, epilogue, resid, ldr,
                         resid_bs, gate, gate_ld, nullptr, stream);
+}
+
+extern "C" int b2f_gemm_set_tile_override(int tile_n) {
+  if (tile_n != 0 && tile_n != BLOCK_N && tile_n != WIDE_N) return B2F_ERR_INVALID;
+  g_tile_override = tile_n;
+  return B2F_OK;
 }
 
 // dX[batch, M, N] = epi(dY[batch, M, K] . W[K, N]) with W exactly as nn.Linear stores it ([out = K, in = N]): the

@@ -2,7 +2,8 @@
 // 128B-swizzled A | B stages a TMA producer fills, and (for conv.cu) a one-tile-per-CTA consumer path.
 //
 // gemm.cu uses the tile and ring constants with its own persistent ping-pong kernel (each consumer warpgroup owns
-// whole tiles; see there).  conv.cu uses everything below:
+// whole tiles; see there), and BLOCK_M / BLOCK_K / A_BYTES with its 128 x 256 forward tile (both consumers on one tile,
+// W as two 128-row boxes of B_BYTES, its own 3-stage ring).  conv.cu uses everything below:
 //   warpgroup 0 (1 lane)   TMA producer      cp.async.bulk.tensor -> 128B-swizzled smem ring of STAGES stages
 //   warpgroups 1, 2        consumers         wgmma m64n128k16 on rows [64 c, 64 c + 64) of the 128 x 128 tile,
 //                                            fp32 accumulators in registers

@@ -34,7 +34,7 @@ typedef void* b2f_stream_t; /* cudaStream_t */
 
 const char* b2f_strerror(int code);
 /* ABI version; bumped on any signature change or addition (2: LoRA entry points, 3: FP8 entry points, 4: FP8
- * attention, 5: first-block cache). */
+ * attention, 5: first-block cache, 6: GEMM tile override). */
 int b2f_version(void);
 /* Device facts the host needs for grid sizing / reporting. Returns B2F_ERR_NODEVICE without GPU. */
 int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin);
@@ -90,6 +90,18 @@ int b2f_gemm_bf16(const void* A, int64_t lda, int64_t a_batch_stride, const void
                   int M, int N, int K, int epilogue, const void* resid, int64_t ldr,
                   int64_t resid_batch_stride, const void* gate, int64_t gate_ld,
                   b2f_stream_t stream);
+
+/* Tiles: the forward GEMM runs on 128 x 128 tiles (two consumer warpgroups taking turns, so one tile's epilogue overlaps
+ * the next tile's MMAs) or, for the large linears of the denoising loop, on 128 x 256 tiles (both warpgroups on one
+ * tile, one m64n256k16 each per k16 step: fewer shared-memory and L2 bytes per FLOP).  b2f_gemm_bf16 and
+ * b2f_gemm_qkv_norm_rope pick the tile per launch from the shape: the wide tile where its rounds of tiles over the SMs,
+ * at the measured cost of a wide tile, finish first (the fused QKV epilogue also needs d_model % 256 == 0).  Both tiles
+ * give bit-identical results.  The LoRA, FP8 and backward GEMMs always use 128 x 128.  The profiling tag of a launch
+ * (b2f_prof_shapes) ends in " t128" or " t256".
+ * b2f_gemm_set_tile_override is for tests and benchmarks only: 0 restores the automatic choice (the default), 128 or
+ * 256 forces that tile on every later launch that supports it (process-wide, not thread-safe); anything else returns
+ * B2F_ERR_INVALID. */
+int b2f_gemm_set_tile_override(int tile_n);
 
 /* Fused QKV projection of an MMDiT attention block: out[.., 3*d] = A · Wqkv^T + b with per-head
  * RMSNorm(eps, weight nw_q / nw_k) and interleaved-pair RoPE applied to the Q and K heads in the GEMM

@@ -9,7 +9,7 @@ from pathlib import Path
 import torch
 
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
-from gpt_image_edit_b200 import ops  # noqa: E402
+from gpt_image_edit_b200 import _lib, ops  # noqa: E402
 
 
 def timeit(fn, iters=20, warmup=5, flush=None):
@@ -52,10 +52,50 @@ def sustained(fn, seconds=1.2):
     return s.elapsed_time(e) / n
 
 
+def _auto_tile(fn):
+    """The tile width the automatic rule gives the launch of `fn`, read from its profiling tag (" t128" / " t256")."""
+    _lib.prof_enable(True)
+    try:
+        _lib.prof_shapes()
+        fn()
+        tags = [t for t, *_ in _lib.prof_shapes()]
+        _lib.prof_collect()
+    finally:
+        _lib.prof_enable(False)
+    return [int(t.rsplit(" t", 1)[1]) for t in tags]
+
+
+def cublas_kernels():
+    """Names of the kernels cuBLAS (torch.nn.functional.linear) runs for the loop's plain-bias GEMM shapes, recorded with
+    torch.profiler."""
+    from torch.profiler import ProfilerActivity, profile
+
+    d = 3072
+    shapes = [(8192, 3 * d, d), (544, 3 * d, d), (8736, 7 * d, d), (8192, d, d), (544, d, d), (8192, 4 * d, d),
+              (544, 4 * d, d), (8192, d, 4 * d), (544, d, 4 * d), (8736, d, 5 * d), (8192, 8192, 8192)]
+    res = []
+    for M, N, K in shapes:
+        x = torch.randn(M, K, device="cuda").bfloat16()
+        w = (torch.randn(N, K, device="cuda") * K ** -0.5).bfloat16()
+        b = torch.randn(N, device="cuda").bfloat16()
+        for _ in range(3):
+            torch.nn.functional.linear(x, w, b)
+        torch.cuda.synchronize()
+        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+            torch.nn.functional.linear(x, w, b)
+            torch.cuda.synchronize()
+        names = [e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA]
+        r = dict(kind="cublas_kernels", M=M, N=N, K=K, kernels=sorted(set(names)))
+        print(json.dumps(r), flush=True)
+        res.append(r)
+    return res
+
+
 def loop_gemms(args, flush):
     """The GEMMs of the 1024^2 edit loop (image M 8192, text M 544, single blocks M 8736, d 3072) and of the text
     encoders (Qwen M 288, T5 M 256), each with the epilogue it runs with; dgrad / wgrad at train512 (S 2336).
-    cuBLAS (torch) is timed beside the plain-bias shapes only."""
+    Each forward GEMM is timed with the automatic tile, forced onto 128 x 128 and onto 128 x 256, and beside cuBLAS
+    (torch) on its plain-bias twin."""
     from gpt_image_edit_b200 import train_ops as T
 
     d = 3072
@@ -68,6 +108,9 @@ def loop_gemms(args, flush):
         ("ff2 gate_resid", 8192, d, 4 * d, ops.EPI_GATE_RESID),
         ("single proj_out gate_resid", 8736, d, 5 * d, ops.EPI_GATE_RESID),
         ("ff1 gelu", 8192, 4 * d, d, ops.EPI_GELU_TANH),
+        ("to_out txt gate_resid", 544, d, d, ops.EPI_GATE_RESID),
+        ("ff1 txt gelu", 544, 4 * d, d, ops.EPI_GELU_TANH),
+        ("ff2 txt gate_resid", 544, d, 4 * d, ops.EPI_GATE_RESID),
         ("adaln M28", 28, 6 * d, d, ops.EPI_BIAS),
         ("adaln single M28", 28, 3 * d, d, ops.EPI_BIAS),
         ("qwen gate_up M288", 288, 2 * 18944, 3584, ops.EPI_BIAS),
@@ -108,9 +151,16 @@ def loop_gemms(args, flush):
                                     gate=gate)
         r["b2f_ms"] = t_of(fn)
         r["b2f_tflops"] = 2.0 * M * N * K / r["b2f_ms"] / 1e9
-        if epi == ops.EPI_BIAS:
-            r["cublas_ms"] = t_of(lambda: torch.nn.functional.linear(x, w, b))
-            r["cublas_tflops"] = 2.0 * M * N * K / r["cublas_ms"] / 1e9
+        # the same launch forced onto each tile of the forward GEMM (b2f_ms above is the automatic choice), and cuBLAS
+        # on the shape's plain-bias twin (cuBLAS has none of the fused epilogues)
+        for tile in (128, 256):
+            _lib.check(_lib.lib.b2f_gemm_set_tile_override(tile), "b2f_gemm_set_tile_override")
+            r[f"t{tile}_ms"] = t_of(fn)
+            r[f"t{tile}_tflops"] = 2.0 * M * N * K / r[f"t{tile}_ms"] / 1e9
+        _lib.check(_lib.lib.b2f_gemm_set_tile_override(0), "b2f_gemm_set_tile_override")
+        r["auto_tile"] = _auto_tile(fn)
+        r["cublas_ms"] = t_of(lambda: torch.nn.functional.linear(x, w, b))
+        r["cublas_tflops"] = 2.0 * M * N * K / r["cublas_ms"] / 1e9
         print(json.dumps(r), flush=True)
         res.append(r)
         del x, w, b, out
@@ -138,9 +188,18 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--what", default="gemm", help="any of gemm, loop (the edit loop's and training's GEMMs), attn")
     ap.add_argument("--sustained", action="store_true")
+    ap.add_argument("--cublas-kernels", action="store_true", help="record the cuBLAS kernel names of the loop's GEMM "
+                    "shapes with torch.profiler (a run of its own: no timing)")
     ap.add_argument("--tag", default="", help="label of the library under test (B2F_LIB), added to rows and file name")
     ap.add_argument("--out-dir", default="bench_out", help="directory of the bench_kernels_<what>[_<tag>].json file")
     args = ap.parse_args()
+    if args.cublas_kernels:
+        res = cublas_kernels()
+        out_dir = Path(args.out_dir)
+        out_dir.mkdir(parents=True, exist_ok=True)
+        with open(out_dir / "bench_kernels_cublas_kernels.json", "w") as f:
+            json.dump(res, f, indent=1)
+        return
     flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")
     res = []
     if "gemm" in args.what:
