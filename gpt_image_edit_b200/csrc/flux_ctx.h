@@ -58,8 +58,9 @@ struct FluxCtx {
   float lora_scale = 1.f;
   int lora_count = 0;
   int lora_rmax() const;
-  // b2f_flux_set_fp8: the block linears of b2f_flux_forward run in FP8
+  // b2f_flux_set_fp8: the block linears of b2f_flux_forward run in FP8; fp8_lora (mode 2): with unfused adapters
   bool fp8 = false;
+  bool fp8_lora = false;
   // b2f_flux_set_fp8_attention: the blocks' attention runs in FP8 (b2f_attn_quant_fp8 + b2f_attention_fp8)
   bool fp8_attn = false;
   // fp32 gradient buffers of the trainable tensors, bound by name (flux_train.cu); an unbound name is frozen

@@ -106,13 +106,13 @@ struct Q8 {
 // A linear layer of the forward with its unfused LoRA, if one is bound:
 //   T = bf16(colscale * cs_mul * (A Acat^T))  into tb [batch, M, r_pad]    (gemm_colscale)
 //   out = epi(A W^T + T Bcat^T + bias)                                      (gemm_bf16_lora: r_pad / 64 more k-blocks)
-// Without one it is exactly the plain gemm_bf16 launch.  With q8 (FP8 on; no adapter can be bound then) it is the FP8
-// launch on (q8, w8).
+// Without one it is exactly the plain gemm_bf16 launch.  With q8 (FP8 on) it is the FP8 launch on (q8, w8); an adapter
+// (FP8 mode 2) then runs its down projection on the bf16 input A and extends the FP8 launch (gemm_fp8_lora).
 static int lin_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_t lda, int64_t a_bs, int64_t ldw,
                    void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epi, const void* resid,
                    int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld, cudaStream_t st,
                    const Q8* q8 = nullptr) {
-  if (q8)
+  if (q8 && !l.lora.A)
     return b2f_gemm_fp8(q8->a, q8->lda, q8->a_bs, q8->s, q8->s_bs, l.w8, K, l.ws, l.b, out, ldc, out_bs, batch, M, N, K,
                         epi, resid, ldr, resid_bs, gate, gate_ld, st);
   if (!l.lora.A)
@@ -122,6 +122,9 @@ static int lin_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_
   const int64_t t_bs = (int64_t)M * r;
   int rc = b2f_gemm_colscale(A, lda, a_bs, l.lora.A, K, tb, r, t_bs, batch, M, r, K, l.lora.cs, cs_mul, st);
   if (rc) return rc;
+  if (q8)
+    return b2f_gemm_fp8_lora(q8->a, q8->lda, q8->a_bs, q8->s, q8->s_bs, l.w8, K, l.ws, l.b, out, ldc, out_bs, batch, M,
+                             N, K, epi, resid, ldr, resid_bs, gate, gate_ld, tb, r, t_bs, l.lora.Bc, r, r, st);
   return b2f_gemm_bf16_lora(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, N, K, epi, resid, ldr, resid_bs,
                             gate, gate_ld, tb, r, t_bs, l.lora.Bc, r, r, st);
 }
@@ -130,7 +133,7 @@ static int qkv_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_
                    const void* nw_k, const float* cos, const float* sin, int rope_row0, float eps, int n_extra,
                    void* out_extra, int64_t ld_extra, int64_t bs_extra, int epi_extra, cudaStream_t st,
                    const Q8* q8 = nullptr) {
-  if (q8)
+  if (q8 && !l.lora.A)
     return b2f_gemm_qkv_norm_rope_fp8(q8->a, q8->lda, q8->a_bs, q8->s, q8->s_bs, l.w8, K, l.ws, l.b, out, ldc, out_bs,
                                       batch, M, d_model, K, nw_q, nw_k, cos, sin, rope_row0, eps, n_extra, out_extra,
                                       ld_extra, bs_extra, epi_extra, st);
@@ -141,6 +144,10 @@ static int qkv_fwd(const Lin& l, bf16_t* tb, float cs_mul, const void* A, int64_
   const int64_t t_bs = (int64_t)M * r;
   int rc = b2f_gemm_colscale(A, lda, a_bs, l.lora.A, K, tb, r, t_bs, batch, M, r, K, l.lora.cs, cs_mul, st);
   if (rc) return rc;
+  if (q8)
+    return b2f_gemm_qkv_norm_rope_fp8_lora(q8->a, q8->lda, q8->a_bs, q8->s, q8->s_bs, l.w8, K, l.ws, l.b, out, ldc,
+                                           out_bs, batch, M, d_model, K, nw_q, nw_k, cos, sin, rope_row0, eps, n_extra,
+                                           out_extra, ld_extra, bs_extra, epi_extra, tb, r, t_bs, l.lora.Bc, r, r, st);
   return b2f_gemm_qkv_norm_rope_lora(A, lda, a_bs, l.w, ldw, l.b, out, ldc, out_bs, batch, M, d_model, K, nw_q, nw_k, cos,
                                      sin, rope_row0, eps, n_extra, out_extra, ld_extra, bs_extra, epi_extra, tb, r, t_bs,
                                      l.lora.Bc, r, r, st);
@@ -263,6 +270,7 @@ int b2f_flux_finalize(b2f_flux* h) {
   });
   c->adaln_lora.clear();
   c->fp8 = false;
+  c->fp8_lora = false;
   c->fp8_attn = false;
   c->finalized = true;
   return B2F_OK;
@@ -393,7 +401,7 @@ int b2f_flux_bind_lora(b2f_flux* h, const char* target, const void* Acat, const 
   FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
   if (!c || !c->finalized || !target) return B2F_ERR_INVALID;
   const bool unbind = Acat == nullptr;
-  if (!unbind && c->fp8) {
+  if (!unbind && c->fp8 && !c->fp8_lora) {
     fprintf(stderr, "[b2f] flux_bind_lora: FP8 is on; fuse the adapter or switch FP8 off first\n");
     return B2F_ERR_UNSUPPORTED;
   }
@@ -479,14 +487,16 @@ int b2f_flux_bind_fp8(b2f_flux* h, const char* name, const void* w8, const float
   return rc;
 }
 
-int b2f_flux_set_fp8(b2f_flux* h, int on) {
+int b2f_flux_set_fp8(b2f_flux* h, int mode) {
   FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
   if (!c || !c->finalized) return B2F_ERR_INVALID;
-  if (!on) {
+  if (!mode) {
     c->fp8 = false;
+    c->fp8_lora = false;
     return B2F_OK;
   }
-  if (c->lora_rmax() > 0) {
+  const bool with_lora = mode == 2;
+  if (!with_lora && c->lora_rmax() > 0) {
     fprintf(stderr, "[b2f] flux_set_fp8: unfused LoRA adapters are bound; fuse or unbind them first\n");
     return B2F_ERR_UNSUPPORTED;
   }
@@ -499,6 +509,7 @@ int b2f_flux_set_fp8(b2f_flux* h, int on) {
   });
   if (rc) return rc;
   c->fp8 = true;
+  c->fp8_lora = with_lora;
   return B2F_OK;
 }
 
@@ -627,7 +638,8 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
       if (f8) {
         RUN(b2f_ln_modulate_fp8(hb, d, h_bs, mt + d, mt, mod_ld, q8, 5 * d, q8_bs, qs, S, B, S, (int)d, eps, S_txt,
                                 mi + d, mi, st));
-      } else {
+      }
+      if (!f8 || w.qkv.lora.A || w.add_qkv.lora.A) {   // FP8 mode 2: the bf16 rows an adapter's down projection reads
         RUN(b2f_ln_modulate(hb, d, h_bs, mt + d, mt, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt, mi + d, mi, st));
       }
       // QKV projections with per-head RMSNorm + RoPE fused into the GEMM epilogue; both streams write
@@ -647,7 +659,8 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
       if (f8) {
         RUN(b2f_ln_modulate_fp8(hb, d, h_bs, mt + 4 * d, mt + 3 * d, mod_ld, q8, 5 * d, q8_bs, qs, S, B, S, (int)d, eps,
                                 S_txt, mi + 4 * d, mi + 3 * d, st));
-      } else {
+      }
+      if (!f8 || w.ff1.lora.A || w.ffc1.lora.A) {
         RUN(b2f_ln_modulate(hb, d, h_bs, mt + 4 * d, mt + 3 * d, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt,
                             mi + 4 * d, mi + 3 * d, st));
       }
@@ -668,7 +681,8 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
       if (f8) {
         RUN(b2f_ln_modulate_fp8(hb, d, h_bs, ms + d, ms, mod_ld, q8, 5 * d, q8_bs, qs, S, B, S, (int)d, eps, 0, nullptr,
                                 nullptr, st));
-      } else {
+      }
+      if (!f8 || w.qkv_mlp.lora.A) {
         RUN(b2f_ln_modulate(hb, d, h_bs, ms + d, ms, mod_ld, xn, d, h_bs, B, S, (int)d, eps, 0, nullptr, nullptr, st));
       }
       // ONE launch for [to_q;to_k;to_v;proj_mlp] (N = 7d): Q/K get RMSNorm+RoPE, V passes through into

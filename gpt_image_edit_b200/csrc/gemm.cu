@@ -276,11 +276,18 @@ struct LoraParams<true> {
   float cs_mul;
 };
 
-// FP8 mode (FP8 = true, MODE 0 only, not with LORA): A and W are e4m3 with one fp32 scale per row of A (a_scale, per
-// token) and per row of W (w_scale, per output channel).  A k-block is still 128 bytes of K, now 128 elements, so the
-// ring, the swizzle and the 32-byte descriptor step are unchanged; each k32 step is one m64n128k32 e4m3 wgmma.  The
-// staged value is x = bf16(fmaf(acc, fp32(a_scale[m] * w_scale[n]), bias[n])) (bf16(acc * scale) without a bias), and
-// every epilogue runs from x as in the bf16 kernel.  FP8 = false has an empty parameter and compiles to the plain kernel.
+// FP8 mode (FP8 = true, MODE 0 only): A and W are e4m3 with one fp32 scale per row of A (a_scale, per token) and per
+// row of W (w_scale, per output channel).  A k-block is still 128 bytes of K, now 128 elements, so the ring, the swizzle
+// and the 32-byte descriptor step are unchanged; each k32 step is one m64n128k32 e4m3 wgmma.  The staged value is
+// x = bf16(fmaf(acc, fp32(a_scale[m] * w_scale[n]), bias[n])) (bf16(acc * scale) without a bias), and every epilogue
+// runs from x as in the bf16 kernel.  FP8 = false has an empty parameter and compiles to the plain kernel.
+// FP8 with LORA (an unfused adapter on an FP8 linear; no colscale): the bf16 (T, Bcat) k-blocks are 128 bytes wide too,
+// so they follow the e4m3 ones through the same ring.  Before its first LoRA k-block a consumer drains its MMAs and
+// scales its accumulators in registers, acc *= fp32(a_scale[m] * w_scale[n]); the LoRA k-blocks then accumulate into
+// them with m64n128k16 bf16 wgmma, and the staged value is x = bf16(acc + bias) as in the bf16 kernel.  The drain costs
+// one emptied pipeline per tile; pre-scaling T by 1 / a_scale and Bcat by 1 / w_scale would avoid it, but on the loop's
+// K = 3072 shapes the drain and the extra k-block together cost 6-16 % of the FP8 GEMM (H100 80GB HBM3, 700 W,
+// scripts/bench_lora.py --fp8), small beside the adapter's down projection, so the scaling stays in registers.
 template <bool FP8>
 struct Fp8Params {};
 template <>
@@ -289,6 +296,72 @@ struct Fp8Params<true> {
   long long a_scale_bs;
   const float* w_scale;
 };
+
+// One k-block of a consumer's main loop: wait for its stage, issue its MMAs (m64n128k32 e4m3 or m64n128k16 bf16, two
+// per k step: rows 0..63 and 64..127 of the tile), and hand the previous stage back to the producer once they are done.
+template <bool E4M3, int TA, int TB>
+__device__ __forceinline__ void consume_kblock(float (&acc0)[64], float (&acc1)[64], uint64_t* full, uint64_t* empty,
+                                               int& stage, uint32_t& phase, int& prev, uint64_t da0,
+                                               uint64_t da1, uint64_t db0, int lane) {
+  constexpr int A_KSTEP = TA ? 2048 : 32;
+  constexpr int B_KSTEP = TB ? 2048 : 32;
+  mbar_wait(&full[stage], phase);
+  const uint64_t soff = uint64_t((stage * STAGE_BYTES) >> 4);
+  reg_fence(acc0);
+  reg_fence(acc1);
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < BLOCK_K / 16; ++k) {
+    const uint64_t ka = soff + uint64_t((k * A_KSTEP) >> 4), kb16 = soff + uint64_t((k * B_KSTEP) >> 4);
+    if constexpr (E4M3) {
+      wgmma_m64n128k32_e4m3_ss(acc0, da0 + ka, db0 + kb16, 1u);
+      wgmma_m64n128k32_e4m3_ss(acc1, da1 + ka, db0 + kb16, 1u);
+    } else {
+      wgmma_m64n128_ss<TA, TB>(acc0, da0 + ka, db0 + kb16, 1u);
+      wgmma_m64n128_ss<TA, TB>(acc1, da1 + ka, db0 + kb16, 1u);
+    }
+  }
+  wgmma_commit();
+  wgmma_wait<1>();   // the previous stage's MMAs are complete: hand it back to the producer
+  if (prev >= 0) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[prev]);
+  }
+  prev = stage;
+  if (++stage == STAGES) {
+    stage = 0;
+    phase ^= 1;
+  }
+}
+
+// FP8 with LORA: acc *= fp32(a_scale[m] * w_scale[n]) on a consumer's drained accumulators (element j of a thread is
+// row 16 w + lane / 4 + 8 ((j / 2) & 1), column 8 (j / 4) + 2 (lane % 4) + (j & 1) of its 64-row half; scales are 0
+// past M and N, as in the FP8 epilogue).
+__device__ __forceinline__ void fp8_rescale(const GemmParams& p, const Fp8Params<true>& fx, int bb, int mb, int n_blk,
+                                            int w, int lane, float (&acc0)[64], float (&acc1)[64]) {
+  const int r_lo = 16 * w + (lane >> 2);
+  float sa[2][2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+      const long long row = (long long)mb * BLOCK_M + 64 * h + r_lo + 8 * rr;
+      sa[h][rr] = row < p.M ? __ldg(fx.a_scale + bb * fx.a_scale_bs + row) : 0.f;
+    }
+#pragma unroll
+  for (int j = 0; j < BLOCK_N / 8; ++j) {
+    const int n = n_blk * BLOCK_N + 8 * j + 2 * (lane & 3);
+    const float2 ws2 = n < p.N ? __ldg(reinterpret_cast<const float2*>(fx.w_scale + n)) : make_float2(0.f, 0.f);
+    acc0[4 * j] *= sa[0][0] * ws2.x;
+    acc0[4 * j + 1] *= sa[0][0] * ws2.y;
+    acc0[4 * j + 2] *= sa[0][1] * ws2.x;
+    acc0[4 * j + 3] *= sa[0][1] * ws2.y;
+    acc1[4 * j] *= sa[1][0] * ws2.x;
+    acc1[4 * j + 1] *= sa[1][0] * ws2.y;
+    acc1[4 * j + 2] *= sa[1][1] * ws2.x;
+    acc1[4 * j + 3] *= sa[1][1] * ws2.y;
+  }
+}
 
 template <int MODE, bool LORA = false, bool FP8 = false>
 __global__ void __launch_bounds__(THREADS, 1)
@@ -388,8 +461,6 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
   const uint64_t da0 = make_sdesc_sw128(ring_u, TA ? MN_BOX_BYTES : 16, 1024);
   const uint64_t da1 = make_sdesc_sw128(ring_u + 8192, TA ? MN_BOX_BYTES : 16, 1024);
   const uint64_t db0 = make_sdesc_sw128(ring_u + A_BYTES, TB ? MN_BOX_BYTES : 16, 1024);
-  constexpr int A_KSTEP = TA ? 2048 : 32;
-  constexpr int B_KSTEP = TB ? 2048 : 32;
   if (c == 1) named_bar_arrive(BAR_TURN + 0, 256);   // consumer 0 takes the first turn
 
   for (int i = c; i < n_local; i += 2) {
@@ -408,34 +479,18 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     const int slot0 = i * num_kb_all;
     int stage = slot0 % STAGES, prev = -1;
     uint32_t phase = (slot0 / STAGES) & 1;
-    for (int kb = 0; kb < num_kb_all; ++kb) {
-      mbar_wait(&full[stage], phase);
-      const uint64_t soff = uint64_t((stage * STAGE_BYTES) >> 4);
+    // FP8 with LoRA: the e4m3 k-blocks, then the scales, then the bf16 LoRA k-blocks, each in a loop of one wgmma type
+    // (a branch between the two types inside one loop makes ptxas serialize every wgmma of the kernel)
+    const int kb_main = FP8 && LORA ? num_kb : num_kb_all;
+    for (int kb = 0; kb < kb_main; ++kb)
+      consume_kblock<FP8, TA, TB>(acc0, acc1, full, empty, stage, phase, prev, da0, da1, db0, lane);
+    if constexpr (FP8 && LORA) {
+      wgmma_wait<0>();
       reg_fence(acc0);
       reg_fence(acc1);
-      wgmma_fence();
-#pragma unroll
-      for (int k = 0; k < BLOCK_K / 16; ++k) {
-        const uint64_t ka = soff + uint64_t((k * A_KSTEP) >> 4), kb16 = soff + uint64_t((k * B_KSTEP) >> 4);
-        if constexpr (FP8) {
-          wgmma_m64n128k32_e4m3_ss(acc0, da0 + ka, db0 + kb16, 1u);
-          wgmma_m64n128k32_e4m3_ss(acc1, da1 + ka, db0 + kb16, 1u);
-        } else {
-          wgmma_m64n128_ss<TA, TB>(acc0, da0 + ka, db0 + kb16, 1u);
-          wgmma_m64n128_ss<TA, TB>(acc1, da1 + ka, db0 + kb16, 1u);
-        }
-      }
-      wgmma_commit();
-      wgmma_wait<1>();   // the previous stage's MMAs are complete: hand it back to the producer
-      if (prev >= 0) {
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&empty[prev]);
-      }
-      prev = stage;
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1;
-      }
+      fp8_rescale(p, fx, bb, mb, n_blk, w, lane, acc0, acc1);
+      for (int kb = num_kb; kb < num_kb_all; ++kb)
+        consume_kblock<false, 0, 0>(acc0, acc1, full, empty, stage, phase, prev, da0, da1, db0, lane);
     }
     if (i + 1 < n_local) named_bar_arrive(BAR_TURN + (c ^ 1), 256);   // the other consumer's tile goes next
     wgmma_wait<0>();
@@ -483,7 +538,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
     // x = bf16(acc + bias) into this consumer's staging tile, once its previous tile's epilogue is done reading it
     named_bar_sync(BAR_EPI + c, 128);
     float sa[2][2];   // FP8: the token scales of this thread's rows 64 h + r_lo + 8 rr (0 past M)
-    if constexpr (FP8) {
+    if constexpr (FP8 && !LORA) {
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
@@ -506,7 +561,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           cs2.y *= lx.cs_mul;
         }
       }
-      if constexpr (FP8) {
+      if constexpr (FP8 && !LORA) {
         const float2 ws2 = n < p.N ? __ldg(reinterpret_cast<const float2*>(fx.w_scale + n)) : make_float2(0.f, 0.f);
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
@@ -844,7 +899,7 @@ template <int MODE, bool LORA = false, bool FP8 = false>
 int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cudaStream_t stream,
                 const LoraParams<LORA>& lx = LoraParams<LORA>{}, const Fp8Params<FP8>& fx = Fp8Params<FP8>{}) {
   static_assert(!LORA || MODE == 0, "the LoRA K-extension is forward-only");
-  static_assert(!FP8 || (MODE == 0 && !LORA), "FP8 is a mode of the plain forward GEMM");
+  static_assert(!FP8 || MODE == 0, "FP8 is a mode of the forward GEMM");
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<MODE, LORA, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
@@ -870,6 +925,8 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cu
     down = lx.colscale != nullptr;
   }
   const double kk = MODE == 2 ? (double)p.kbatch * p.K : (double)p.K + k_ext;
+  // operand bytes per row of A and of W: the main k-blocks (e4m3 or bf16), then the bf16 LoRA ones
+  const double kbytes = (FP8 ? 1.0 : 2.0) * (MODE == 2 ? kk : (double)p.K) + 2.0 * k_ext;
   prof_begin(KC_GEMM, stream);
   if (tile_n == WIDE_N)
     gemm_wide_kernel<<<grid, THREADS, WIDE_SMEM_BYTES, stream>>>(tmA, tmB, p);
@@ -877,8 +934,9 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cu
     gemm_bf16_kernel<MODE, LORA, FP8><<<grid, THREADS, PP_SMEM_BYTES, stream>>>(tmA, tmB, p, lx, fx);
   {
     char tag_[96];
-    const double ab = FP8 ? 1.0 : 2.0;   // bytes per A / W element
-    if (FP8)
+    if (FP8 && LORA)
+      snprintf(tag_, sizeof tag_, "gemm fp8 lora %dx%dx%d+%d b%d e%d", p.M, p.N, p.K, k_ext, p.batch, p.epi);
+    else if (FP8)
       snprintf(tag_, sizeof tag_, "gemm fp8 %dx%dx%d b%d e%d", p.M, p.N, p.K, p.batch, p.epi);
     else if (LORA)
       snprintf(tag_, sizeof tag_, "gemm lora %dx%dx%d+%d b%d e%d%s", p.M, p.N, p.K, k_ext, p.batch, p.epi,
@@ -886,7 +944,7 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cu
     else
       snprintf(tag_, sizeof tag_, "gemm m%d %dx%dx%d b%d e%d t%d", MODE, p.M, p.N, (int)kk, p.batch, p.epi, tile_n);
     prof_end_tagged(KC_GEMM, stream, 2.0 * p.batch * (double)p.M * p.N * kk,
-                    ab * ((double)p.batch * p.M * kk + (double)p.N * kk) + 2.0 * (double)p.batch * p.M * p.N, tag_);
+                    kbytes * ((double)p.batch * p.M + p.N) + 2.0 * (double)p.batch * p.M * p.N, tag_);
   }
   B2F_LAUNCHED(tile_n == WIDE_N ? "gemm_wide_kernel" : "gemm_bf16_kernel", 1);
   return B2F_OK;
@@ -925,6 +983,33 @@ struct LoraExt {
   float cs_mul;
 };
 
+// Checks the LoRA operands of one launch and fills its LoraParams (tmA / tmB stand in for the maps of an absent
+// extension; they are never read then).
+static int lora_params(const LoraExt* lx, const CUtensorMap& tmA, const CUtensorMap& tmB, int batch, int M, int N,
+                       const void* bias, int epilogue, LoraParams<true>* lp) {
+  if (lx->r_pad < 0 || (lx->r_pad % BLOCK_K)) return B2F_ERR_INVALID;
+  if (lx->colscale && (lx->r_pad || bias || epilogue != B2F_EPI_BIAS)) return B2F_ERR_INVALID;
+  if (!lx->colscale && !lx->r_pad) return B2F_ERR_INVALID;
+  if (lx->colscale && (reinterpret_cast<uintptr_t>(lx->colscale) & 15)) return B2F_ERR_ALIGN;
+  lp->tmT = tmA;
+  lp->tmBc = tmB;
+  lp->num_kb2 = lx->r_pad / BLOCK_K;
+  lp->colscale = lx->colscale;
+  lp->cs_mul = lx->cs_mul;
+  if (lx->r_pad) {
+    if (!lx->T || !lx->Bc) return B2F_ERR_INVALID;
+    if ((lx->ldt & 7) || (lx->t_bs & 7) || (lx->ldbc & 7) || lx->ldt < lx->r_pad || lx->ldbc < lx->r_pad ||
+        ((reinterpret_cast<uintptr_t>(lx->T) | reinterpret_cast<uintptr_t>(lx->Bc)) & 15))
+      return B2F_ERR_ALIGN;
+    int rc = make_tmap_3d_rows(&lp->tmT, lx->T, (uint64_t)lx->r_pad, (uint64_t)M, (uint64_t)batch, (uint64_t)lx->ldt,
+                               batch > 1 ? (uint64_t)lx->t_bs : (uint64_t)M * lx->ldt);
+    if (rc != B2F_OK) return rc;
+    rc = make_tmap_2d_bf16(&lp->tmBc, lx->Bc, (uint64_t)N, (uint64_t)lx->r_pad, (uint64_t)lx->ldbc, BLOCK_N, BLOCK_K);
+    if (rc != B2F_OK) return rc;
+  }
+  return B2F_OK;
+}
+
 static int gemm_bf16_impl(const void* A, int64_t lda, int64_t a_bs, const void* W, int64_t ldw,
               const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch, int M, int N,
               int K, int epilogue, const void* resid, int64_t ldr, int64_t resid_bs, const void* gate,
@@ -935,7 +1020,7 @@ static int gemm_bf16_impl(const void* A, int64_t lda, int64_t a_bs, const void* 
   if ((K & 7) || (N & 7) || (lda & 7) || (ldw & 7) || (ldc & 7) || (a_bs & 7) || (out_bs & 7))
     return B2F_ERR_ALIGN;
   if (fx) {   // byte operands: TMA needs 16-byte pitches
-    if (lx || !fx->a_scale || !fx->w_scale) return B2F_ERR_INVALID;
+    if ((lx && lx->colscale) || !fx->a_scale || !fx->w_scale) return B2F_ERR_INVALID;
     if ((K & 15) || (lda & 15) || (ldw & 15) || (a_bs & 15) || (reinterpret_cast<uintptr_t>(fx->w_scale) & 15) ||
         (reinterpret_cast<uintptr_t>(fx->a_scale) & 3))
       return B2F_ERR_ALIGN;
@@ -1005,7 +1090,10 @@ static int gemm_bf16_impl(const void* A, int64_t lda, int64_t a_bs, const void* 
     fp.a_scale = fx->a_scale;
     fp.a_scale_bs = fx->a_scale_bs;
     fp.w_scale = fx->w_scale;
-    return launch_gemm<0, false, true>(tmA, tmB, p, stream, LoraParams<false>{}, fp);
+    if (!lx || !lx->r_pad) return launch_gemm<0, false, true>(tmA, tmB, p, stream, LoraParams<false>{}, fp);
+    LoraParams<true> lp;
+    if ((rc = lora_params(lx, tmA, tmB, batch, M, N, bias, epilogue, &lp)) != B2F_OK) return rc;
+    return launch_gemm<0, true, true>(tmA, tmB, p, stream, lp, fp);
   }
   rc = make_tmap_3d_rows(&tmA, A, (uint64_t)K, (uint64_t)M, (uint64_t)batch, (uint64_t)lda,
                          batch > 1 ? (uint64_t)a_bs : (uint64_t)M * lda);
@@ -1013,28 +1101,8 @@ static int gemm_bf16_impl(const void* A, int64_t lda, int64_t a_bs, const void* 
   rc = make_tmap_2d_bf16(&tmB, W, (uint64_t)N, (uint64_t)K, (uint64_t)ldw, BLOCK_N, BLOCK_K);
   if (rc != B2F_OK) return rc;
   if (!lx) return launch_gemm<0>(tmA, tmB, p, stream);
-
-  if (lx->r_pad < 0 || (lx->r_pad % BLOCK_K)) return B2F_ERR_INVALID;
-  if (lx->colscale && (lx->r_pad || bias || epilogue != B2F_EPI_BIAS)) return B2F_ERR_INVALID;
-  if (!lx->colscale && !lx->r_pad) return B2F_ERR_INVALID;
-  if (lx->colscale && (reinterpret_cast<uintptr_t>(lx->colscale) & 15)) return B2F_ERR_ALIGN;
   LoraParams<true> lp;
-  lp.tmT = tmA;   // unread without an extension
-  lp.tmBc = tmB;
-  lp.num_kb2 = lx->r_pad / BLOCK_K;
-  lp.colscale = lx->colscale;
-  lp.cs_mul = lx->cs_mul;
-  if (lx->r_pad) {
-    if (!lx->T || !lx->Bc) return B2F_ERR_INVALID;
-    if ((lx->ldt & 7) || (lx->t_bs & 7) || (lx->ldbc & 7) || lx->ldt < lx->r_pad || lx->ldbc < lx->r_pad ||
-        ((reinterpret_cast<uintptr_t>(lx->T) | reinterpret_cast<uintptr_t>(lx->Bc)) & 15))
-      return B2F_ERR_ALIGN;
-    rc = make_tmap_3d_rows(&lp.tmT, lx->T, (uint64_t)lx->r_pad, (uint64_t)M, (uint64_t)batch, (uint64_t)lx->ldt,
-                           batch > 1 ? (uint64_t)lx->t_bs : (uint64_t)M * lx->ldt);
-    if (rc != B2F_OK) return rc;
-    rc = make_tmap_2d_bf16(&lp.tmBc, lx->Bc, (uint64_t)N, (uint64_t)lx->r_pad, (uint64_t)lx->ldbc, BLOCK_N, BLOCK_K);
-    if (rc != B2F_OK) return rc;
-  }
+  if ((rc = lora_params(lx, tmA, tmB, batch, M, N, bias, epilogue, &lp)) != B2F_OK) return rc;
   return launch_gemm<0, true>(tmA, tmB, p, stream, lp);
 }
 
@@ -1160,6 +1228,39 @@ extern "C" int b2f_gemm_qkv_norm_rope_fp8(const void* A, int64_t lda, int64_t a_
   const Fp8Ext fx{a_scale, a_scale_bs, w_scale};
   return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, 3 * d_model + n_extra, K,
                         B2F_EPI_QKV_NORM_ROPE, nullptr, 0, 0, nullptr, 0, &qx, stream, nullptr, &fx);
+}
+
+// b2f_gemm_fp8 / b2f_gemm_qkv_norm_rope_fp8 with the LoRA K-extension of b2f_gemm_bf16_lora: r_pad / 64 bf16 k-blocks of
+// (T, Bcat) after the e4m3 ones, accumulated into the scaled FP8 accumulators (Fp8Params).
+extern "C" int b2f_gemm_fp8_lora(const void* A, int64_t lda, int64_t a_bs, const float* a_scale, int64_t a_scale_bs,
+                                 const void* W, int64_t ldw, const float* w_scale, const void* bias, void* out,
+                                 int64_t ldc, int64_t out_bs, int batch, int M, int N, int K, int epilogue,
+                                 const void* resid, int64_t ldr, int64_t resid_bs, const void* gate, int64_t gate_ld,
+                                 const void* T, int64_t ldt, int64_t t_bs, const void* Bc, int64_t ldbc, int r_pad,
+                                 b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (epilogue == B2F_EPI_QKV_NORM_ROPE || r_pad <= 0) return B2F_ERR_INVALID;
+  const Fp8Ext fx{a_scale, a_scale_bs, w_scale};
+  const LoraExt lx{T, ldt, t_bs, Bc, ldbc, r_pad, nullptr, 1.f};
+  return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, N, K, epilogue, resid, ldr,
+                        resid_bs, gate, gate_ld, nullptr, stream, &lx, &fx);
+}
+
+extern "C" int b2f_gemm_qkv_norm_rope_fp8_lora(const void* A, int64_t lda, int64_t a_bs, const float* a_scale,
+                                               int64_t a_scale_bs, const void* W, int64_t ldw, const float* w_scale,
+                                               const void* bias, void* out, int64_t ldc, int64_t out_bs, int batch,
+                                               int M, int d_model, int K, const void* nw_q, const void* nw_k,
+                                               const float* cos, const float* sin, int rope_row0, float eps,
+                                               int n_extra, void* out_extra, int64_t ld_extra, int64_t bs_extra,
+                                               int epi_extra, const void* T, int64_t ldt, int64_t t_bs, const void* Bc,
+                                               int64_t ldbc, int r_pad, b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (r_pad <= 0) return B2F_ERR_INVALID;
+  QkvExtra qx{nw_q, nw_k, cos, sin, rope_row0, d_model, eps, n_extra, epi_extra, out_extra, ld_extra, bs_extra};
+  const Fp8Ext fx{a_scale, a_scale_bs, w_scale};
+  const LoraExt lx{T, ldt, t_bs, Bc, ldbc, r_pad, nullptr, 1.f};
+  return gemm_bf16_impl(A, lda, a_bs, W, ldw, bias, out, ldc, out_bs, batch, M, 3 * d_model + n_extra, K,
+                        B2F_EPI_QKV_NORM_ROPE, nullptr, 0, 0, nullptr, 0, &qx, stream, &lx, &fx);
 }
 
 // ---------------------------------------------------------------------------------------------------- LoRA

@@ -192,6 +192,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         self._schedule = None
         self.gradient_checkpointing = False
         self._fp8 = None   # bound name -> (e4m3 weight, fp32 scales) while FP8 is enabled
+        self._fp8_unfused = False   # FP8 linears accept unfused LoRA adapters (b2f_flux_set_fp8 mode 2)
         self._fp8_attn = False
         self._cache_cfg = None      # FirstBlockCacheConfig while the first-block cache is on
         self._cache_states = {}     # branch name -> _CacheState
@@ -275,27 +276,46 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         return self._fp8 is not None
 
     @property
+    def fp8_unfused_lora(self) -> bool:
+        """The FP8 block linears run unfused LoRA adapters (enable_fp8(unfused_lora=True))."""
+        return self._fp8 is not None and self._fp8_unfused
+
+    @property
     def fp8_attention_enabled(self) -> bool:
         """The blocks' joint attention runs in FP8."""
         return self._fp8_attn
 
     @torch.no_grad()
-    def enable_fp8(self, linears: bool = True, attention: bool = False):
+    def enable_fp8(self, linears: bool = True, attention: bool = False, unfused_lora: bool = False):
         """Run parts of every transformer block in FP8 (e4m3 operands on the FP8 tensor cores; include/b2f.h).  Each
-        switch turns its part on and leaves the other as it is.
+        switch turns its part on and leaves the others as they are.
 
         linears    the ten block linears: per-token activation scales, per-output-channel weight scales.  Adds an e4m3
                    copy of those weights (912 d^2 bytes: 8.6 GB at FLUX size) and quantizes it on the device.  The
                    bf16 weights stay the master copy: state_dict(), fuse_lora and training keep seeing them, and
                    load_state_dict / randomize_ / fuse_lora / unfuse_lora re-quantize.  Unfused LoRA adapters must be
-                   fused first.
+                   fused first, unless `unfused_lora` is on.
+        unfused_lora  the FP8 block linears (turned on if they are off) also run unfused LoRA adapters: each adapted
+                   linear runs its bf16 down projection T on the linear's bf16 input and adds T Bcat^T as bf16 k-blocks
+                   after the e4m3 ones of the same GEMM (b2f_gemm_fp8_lora), so the update carries no e4m3 rounding.
+                   set_adapters, delete_adapters, disable_lora / enable_lora and the per-call scale then act without
+                   touching the e4m3 weights; a LayerNorm whose output feeds an adapted linear runs one extra bf16
+                   pass.  Adapters loaded before or after this call act alike.  Off by default: then an unfused
+                   adapter is refused while the linears are in FP8.
         attention  the joint attention: Q / K quantized per head, V per channel, P in e4m3 (b2f_attention_fp8).  Adds
                    about 3 bytes per token and channel of workspace.  Touches no weight, so unfused LoRA adapters keep
                    working.  Accuracy cost: e4m3 keeps 3 mantissa bits, so every score carries an error of a few percent
                    of sum |q_i k_i|.  Flat attention rows barely notice; peaked ones do (13 % rel-L2 to exact attention
                    on synthetic heads with a median row max p of 0.6, against 0.17 % for bf16; README), which can be
                    visible in images from checkpoints with such heads."""
-        if linears and self._fp8 is None:
+        if unfused_lora and not self.fp8_unfused_lora:
+            if self._fp8 is None:
+                self._enable_fp8_linears(mode=2)
+            else:
+                check(_lib.lib.b2f_flux_set_fp8(self._h, 2), "b2f_flux_set_fp8")
+                self._fp8_unfused = True
+                self._lora_rebind()   # adapters loaded while FP8 refused them act now
+        elif linears and self._fp8 is None:
             self._enable_fp8_linears()
         if attention and not self._fp8_attn:
             check(_lib.lib.b2f_flux_set_fp8_attention(self._h, 1), "b2f_flux_set_fp8_attention")
@@ -303,8 +323,8 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         self._cache_epoch += 1
         return self
 
-    def _enable_fp8_linears(self):
-        if self._lora_bound:
+    def _enable_fp8_linears(self, mode: int = 1):
+        if self._lora_bound and mode != 2:
             raise _lib.B2FError("enable_fp8: unfused LoRA adapters are active; fuse_lora() them first")
         fp8 = OrderedDict()
         for name in _fp8_linears(self.config):
@@ -316,7 +336,10 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         for name, (w8, ws) in fp8.items():
             check(_lib.lib.b2f_flux_bind_fp8(self._h, name.encode(), ptr(w8), ptr(ws), w8.numel()),
                   f"b2f_flux_bind_fp8 {name}")
-        check(_lib.lib.b2f_flux_set_fp8(self._h, 1), "b2f_flux_set_fp8")
+        check(_lib.lib.b2f_flux_set_fp8(self._h, mode), "b2f_flux_set_fp8")
+        self._fp8_unfused = mode == 2
+        if mode == 2:
+            self._lora_rebind()
 
     def disable_fp8(self):
         """Back to bf16 block linears and attention; the FP8 weight copies are released."""
@@ -327,6 +350,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         if self._fp8 is None:
             return self
         check(_lib.lib.b2f_flux_set_fp8(self._h, 0), "b2f_flux_set_fp8")
+        self._fp8_unfused = False
         for name in self._fp8:
             check(_lib.lib.b2f_flux_bind_fp8(self._h, name.encode(), None, None, 0), f"b2f_flux_bind_fp8 {name}")
         self._fp8 = None
@@ -499,7 +523,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
                 img_ids=None, txt_ids=None, guidance=None, joint_attention_kwargs=None, return_dict=True,
                 **unused):
         cfg = self.config
-        if self._fp8 is not None and self._lora_bound:
+        if self._fp8 is not None and self._lora_bound and not self._fp8_unfused:
             raise _lib.B2FError("FP8 is enabled and LoRA adapters are active unfused: fuse_lora() them first "
                                 "(or disable_fp8())")
         jak = dict(joint_attention_kwargs or {})
@@ -553,7 +577,8 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         """Views of the whole forward workspace in b2f_flux_forward's layout (text rows first): h and xn [B, S, d],
         qkv [B, S, 3d], cat [B, S, 5d].  After a partial-range forward they hold what the last block left (stage-level
         parity tests read them); the views are only for reading.  With FP8 enabled the blocks quantize their
-        LayerNorm outputs straight to e4m3 and do not write xn."""
+        LayerNorm outputs straight to e4m3 and do not write xn, except for a LayerNorm feeding an unfused adapter
+        (enable_fp8(unfused_lora=True))."""
         ws = self._ws["fwd"]
         off = (-ws.data_ptr()) % 256
         S, d = S_img + S_txt, self.inner_dim

@@ -326,8 +326,10 @@ class FluxLoraMixin:
         from . import _lib
         _lib.check(_lib.lib.b2f_flux_clear_lora(self._h), "b2f_flux_clear_lora")
         self._lora_bound = self._lora_concat(self._lora_unfused_set(), pad=True)
-        # with FP8 enabled the engine takes no unfused adapter: the forward refuses until they are fused or FP8 is off
-        for t, (A, B, cs) in ({} if getattr(self, "_fp8", None) is not None else self._lora_bound).items():
+        # with FP8 linears enabled the engine takes unfused adapters only with enable_fp8(unfused_lora=True); otherwise
+        # the forward refuses until they are fused or FP8 is off
+        refused = getattr(self, "_fp8", None) is not None and not getattr(self, "_fp8_unfused", False)
+        for t, (A, B, cs) in ({} if refused else self._lora_bound).items():
             _lib.check(_lib.lib.b2f_flux_bind_lora(self._h, t.encode(), A.data_ptr(), B.data_ptr(), cs.data_ptr(),
                                                    int(A.shape[0])), f"b2f_flux_bind_lora {t}")
         self._lora_version += 1

@@ -513,6 +513,90 @@ def linear_qkv_norm_rope_fp8(xq, x_scale, wq, w_scale, bias, nq, nk, cos, sin, *
     return out
 
 
+def _lora_ext(t, bcat, B, M, N):
+    """(t3, r_pad) of a LoRA K-extension t [.., M, r_pad] / bcat [N, r_pad] checked against the launch."""
+    _req(t, "t")
+    _req(bcat, "bcat")
+    t3 = _as3(t)
+    r_pad = bcat.shape[1]
+    _shape(t3, "t", (B, M, r_pad))
+    _shape(bcat, "bcat", (N, r_pad))
+    return t3, r_pad
+
+
+def linear_fp8_lora(xq, x_scale, wq, w_scale, bias, t, bcat, *, epilogue: int = EPI_BIAS, out=None, resid=None,
+                    gate=None) -> torch.Tensor:
+    """out = epilogue(fp32(x_scale[m] * w_scale[n]) * (xq @ wq^T) + t @ bcat^T + bias) via b2f_gemm_fp8_lora: linear_fp8
+    with the bf16 LoRA K-extension (t, bcat) of linear_lora accumulated onto the scaled FP8 accumulators."""
+    _req(xq, "xq", FP8)
+    _req(wq, "wq", FP8)
+    _req(w_scale, "w_scale", torch.float32)
+    x3 = _as3(xq)
+    B, M, K = x3.shape
+    s2 = _scales(x_scale, "x_scale", B, M)
+    N = wq.shape[0]
+    _fp8_weight_checks(wq, w_scale, bias, N, K)
+    t3, r_pad = _lora_ext(t, bcat, B, M, N)
+    if out is None:
+        out = torch.empty((*xq.shape[:-1], N), device=xq.device, dtype=torch.bfloat16)
+    _req(out, "out")
+    o3 = _as3(out)
+    _shape(o3, "out", (B, M, N))
+    ldr = rbs = gld = 0
+    if epilogue in (EPI_GATE_RESID, EPI_RESID):
+        _req(resid, "resid")
+        r3 = _as3(resid)
+        _shape(r3, "resid", (B, M, N))
+        ldr, rbs = r3.stride(1), r3.stride(0)
+        if epilogue == EPI_GATE_RESID:
+            _req(gate, "gate")
+            _shape(gate, "gate", (B, N) if gate.dim() == 2 else (N,))
+            gld = gate.stride(0) if gate.dim() == 2 else 0
+    check(_lib.lib.b2f_gemm_fp8_lora(ptr(x3), x3.stride(1), x3.stride(0), ptr(s2), s2.stride(0), ptr(wq), wq.stride(0),
+                                     ptr(w_scale), ptr(bias), ptr(o3), o3.stride(1), o3.stride(0), B, M, N, K, epilogue,
+                                     ptr(resid), ldr, rbs, ptr(gate), gld, ptr(t3), t3.stride(1), t3.stride(0),
+                                     ptr(bcat), bcat.stride(0), r_pad, stream_ptr()), "b2f_gemm_fp8_lora")
+    return out
+
+
+def linear_qkv_norm_rope_fp8_lora(xq, x_scale, wq, w_scale, bias, nq, nk, cos, sin, t, bcat, *, rope_row0: int = 0,
+                                  out=None, eps: float = 1e-6, out_extra=None, epi_extra: int = EPI_BIAS):
+    """linear_qkv_norm_rope_fp8 with the LoRA K-extension of linear_fp8_lora (b2f_gemm_qkv_norm_rope_fp8_lora)."""
+    _req(xq, "xq", FP8)
+    _req(wq, "wq", FP8)
+    _req(w_scale, "w_scale", torch.float32)
+    _req(cos, "cos", torch.float32)
+    _req(sin, "sin", torch.float32)
+    x3 = _as3(xq)
+    B, M, K = x3.shape
+    s2 = _scales(x_scale, "x_scale", B, M)
+    n_extra = 0 if out_extra is None else out_extra.shape[-1]
+    N = wq.shape[0] - n_extra
+    _fp8_weight_checks(wq, w_scale, bias, N + n_extra, K)
+    t3, r_pad = _lora_ext(t, bcat, B, M, N + n_extra)
+    _shape(nq, "nq", (128,))
+    _shape(nk, "nk", (128,))
+    if cos.dim() != 2 or cos.shape[0] < rope_row0 + M or cos.shape[1] != 128 or cos.shape != sin.shape:
+        raise _lib.B2FError(f"cos/sin: expected [>= {rope_row0 + M}, 128] tables, got {tuple(cos.shape)} / "
+                            f"{tuple(sin.shape)}")
+    if out is None:
+        out = torch.empty((*xq.shape[:-1], N), device=xq.device, dtype=torch.bfloat16)
+    _req(out, "out")
+    o3 = _as3(out)
+    _shape(o3, "out", (B, M, N))
+    e3 = None
+    if out_extra is not None:
+        _req(out_extra, "out_extra")
+        e3 = _as3(out_extra)
+        _shape(e3, "out_extra", (B, M, n_extra))
+    check(_lib.lib.b2f_gemm_qkv_norm_rope_fp8_lora(
+        ptr(x3), x3.stride(1), x3.stride(0), ptr(s2), s2.stride(0), ptr(wq), wq.stride(0), ptr(w_scale), ptr(bias),
+        ptr(o3), o3.stride(1), o3.stride(0), B, M, N // 3, K, ptr(nq), ptr(nk), ptr(cos), ptr(sin), rope_row0, eps,
+        n_extra, ptr(e3), 0 if e3 is None else e3.stride(1), 0 if e3 is None else e3.stride(0), epi_extra, ptr(t3),
+        t3.stride(1), t3.stride(0), ptr(bcat), bcat.stride(0), r_pad, stream_ptr()), "b2f_gemm_qkv_norm_rope_fp8_lora")
+    return out
+
+
 def _row_pitch(t: torch.Tensor) -> int:
     """Token pitch of a [B,S,H,dh] view; with S = 1 the stride of that dimension is arbitrary and the batch pitch is it."""
     B, S = t.shape[:2]

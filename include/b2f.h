@@ -34,7 +34,7 @@ typedef void* b2f_stream_t; /* cudaStream_t */
 
 const char* b2f_strerror(int code);
 /* ABI version; bumped on any signature change or addition (2: LoRA entry points, 3: FP8 entry points, 4: FP8
- * attention, 5: first-block cache, 6: GEMM tile override). */
+ * attention, 5: first-block cache, 6: GEMM tile override, 7: FP8 GEMMs with unfused LoRA). */
 int b2f_version(void);
 /* Device facts the host needs for grid sizing / reporting. Returns B2F_ERR_NODEVICE without GPU. */
 int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin);
@@ -201,6 +201,30 @@ int b2f_gemm_qkv_norm_rope_fp8(const void* A, int64_t lda, int64_t a_batch_strid
                                int d_model, int K, const void* nw_q, const void* nw_k, const float* cos,
                                const float* sin, int rope_row0, float eps, int n_extra, void* out_extra,
                                int64_t ld_extra, int64_t extra_batch_stride, int epi_extra, b2f_stream_t stream);
+/* FP8 with an unfused LoRA: b2f_gemm_fp8's operands plus b2f_gemm_bf16_lora's K-extension (T, Bcat in bf16, r_pad % 64
+ * == 0, r_pad > 0).  The r_pad / 64 bf16 k-blocks follow the e4m3 ones in the same tile; before the first of them each
+ * tile's accumulators are scaled in registers, so the staged value is
+ *   x = bf16(fp32(acc8 * fp32(sa[m] * sw[n])) + T Bcat^T + bias[n])
+ * with the LoRA products accumulated in fp32 onto the scaled e4m3 accumulator, and the epilogues run from x as
+ * everywhere.  This differs from b2f_gemm_fp8's fmaf(acc, s, bias): an adapter with Bcat = 0 gives results within one
+ * fp32 rounding of b2f_gemm_fp8's before the bf16 rounding, not bit-identical ones.  The adapter sees T, the bf16 down
+ * projection of the linear's bf16 input (b2f_gemm_colscale), so it carries no e4m3 rounding of its own.  128 x 128
+ * tiles. */
+int b2f_gemm_fp8_lora(const void* A, int64_t lda, int64_t a_batch_stride, const float* a_scale,
+                      int64_t a_scale_batch_stride, const void* W, int64_t ldw, const float* w_scale, const void* bias,
+                      void* out, int64_t ldc, int64_t out_batch_stride, int batch, int M, int N, int K, int epilogue,
+                      const void* resid, int64_t ldr, int64_t resid_batch_stride, const void* gate, int64_t gate_ld,
+                      const void* T, int64_t ldt, int64_t t_batch_stride, const void* Bcat, int64_t ldbc, int r_pad,
+                      b2f_stream_t stream);
+/* b2f_gemm_qkv_norm_rope_fp8 with the K-extension of b2f_gemm_fp8_lora. */
+int b2f_gemm_qkv_norm_rope_fp8_lora(const void* A, int64_t lda, int64_t a_batch_stride, const float* a_scale,
+                                    int64_t a_scale_batch_stride, const void* W, int64_t ldw, const float* w_scale,
+                                    const void* bias, void* out, int64_t ldc, int64_t out_batch_stride, int batch,
+                                    int M, int d_model, int K, const void* nw_q, const void* nw_k, const float* cos,
+                                    const float* sin, int rope_row0, float eps, int n_extra, void* out_extra,
+                                    int64_t ld_extra, int64_t extra_batch_stride, int epi_extra, const void* T,
+                                    int64_t ldt, int64_t t_batch_stride, const void* Bcat, int64_t ldbc, int r_pad,
+                                    b2f_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * FP8 attention (head_dim 128, non-causal, no bias): b2f_attention_fwd's online softmax with Q / K / V in e4m3 on the
@@ -443,7 +467,11 @@ int b2f_flux_forward(b2f_flux* ctx, const void* hidden, const void* enc, const v
  * ff.net.2 / ff_context.net.0.proj / ff_context.net.2, single_transformer_blocks.{i}.qkv_mlp / proj_out); numel =
  * out * in; w8 == NULL unbinds.  b2f_flux_set_fp8(ctx, 1) makes b2f_flux_forward run those ten linears per block in FP8:
  * it requires every one to be bound and no LoRA adapter to be bound (b2f_flux_bind_lora is refused while FP8 is on;
- * fuse adapters first).  Every other linear (embedders, AdaLN, norm_out / proj_out) stays bf16, and so does attention
+ * fuse adapters first).  b2f_flux_set_fp8(ctx, 2) is the same with unfused adapters accepted: b2f_flux_bind_lora binds,
+ * and a block linear with an adapter runs b2f_gemm_colscale on its bf16 input, then b2f_gemm_fp8_lora /
+ * b2f_gemm_qkv_norm_rope_fp8_lora.  The bf16 inputs of to_out / to_add_out / ff.net.2 / ff_context.net.2 / proj_out
+ * already exist (the cat buffer); for a LayerNorm whose output feeds an adapted linear the block also runs
+ * b2f_ln_modulate into xn.  Linears without an adapter run exactly as in mode 1.  Every other linear (embedders, AdaLN, norm_out / proj_out) stays bf16, and so does attention
  * unless b2f_flux_set_fp8_attention is on.  The
  * inputs are quantized per token: the block's modulated LayerNorms by b2f_ln_modulate_fp8, the attention output
  * (input of to_out / to_add_out), the MLP activations (ff.net.2 / ff_context.net.2) and the single block's [attn | mlp]
@@ -451,7 +479,7 @@ int b2f_flux_forward(b2f_flux* ctx, const void* hidden, const void* enc, const v
  * e4m3 [B, S, 5d] buffer and an fp32 [B, S] scale vector, the blocks leave the workspace's xn rows unwritten, and the
  * training entry points refuse.  b2f_flux_finalize drops the FP8 bindings and switches FP8 off. */
 int b2f_flux_bind_fp8(b2f_flux* ctx, const char* name, const void* w8, const float* w_scale, int64_t numel);
-int b2f_flux_set_fp8(b2f_flux* ctx, int on);
+int b2f_flux_set_fp8(b2f_flux* ctx, int mode);
 /* FP8 attention, independent of b2f_flux_set_fp8: while on, the double and single blocks quantize Q / K / V with
  * b2f_attn_quant_fp8 and run b2f_attention_fp8 where they run b2f_attention_fwd.  b2f_flux_workspace_bytes then adds
  * q8, k8, v8t and their scales, and the training entry points refuse.  Unfused LoRA adapters stay allowed (they act on
