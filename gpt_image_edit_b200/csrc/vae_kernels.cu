@@ -177,19 +177,33 @@ __global__ void __launch_bounds__(256) u8_nhwc_to_nhwc_pad_kernel(const uint8_t*
   reinterpret_cast<uint4*>(out)[i] = pack8v(f);
 }
 
-// ---------------------------------------------------------------- row softmax, in place, bf16
-// p = softmax(scale * s) per row of length L (L % 8 == 0), one block per row, fp32 math.
-__global__ void __launch_bounds__(256) softmax_rows_kernel(__nv_bfloat16* s, long long ld, int L, float scale) {
+// ---------------------------------------------------------------- row softmax, bf16 out
+// p = softmax(scale * s) per row over [0, L), one block per row, fp32 math; s is bf16 (in place: p == s) or fp32.  Rows
+// are read and written as 8-wide vectors over [0, round_up(L, 8)): the columns [L, round_up(L, 8)) of the last vector
+// are left out of the max and the sum and written as zeros (the VAE's attention contracts P.V over the padded length).
+__device__ __forceinline__ void load8(const __nv_bfloat16* row, int i, float* f) {
+  unpack8v(reinterpret_cast<const uint4*>(row)[i], f);
+}
+__device__ __forceinline__ void load8(const float* row, int i, float* f) {
+  const float4 a = reinterpret_cast<const float4*>(row)[2 * i], b = reinterpret_cast<const float4*>(row)[2 * i + 1];
+  f[0] = a.x, f[1] = a.y, f[2] = a.z, f[3] = a.w, f[4] = b.x, f[5] = b.y, f[6] = b.z, f[7] = b.w;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(256) softmax_rows_kernel(const T* s, long long lds, __nv_bfloat16* p, long long ldp,
+                                                           int L, float scale) {
   __shared__ float red[8];
-  __nv_bfloat16* row = s + (long long)blockIdx.x * ld;
-  const int nvec = L >> 3;
+  const T* row = s + (long long)blockIdx.x * lds;
+  __nv_bfloat16* prow = p + (long long)blockIdx.x * ldp;
+  const int nvec = (L + 7) >> 3;
   const float k = scale * 1.4426950408889634f;
   float mx = -INFINITY;
   for (int i = threadIdx.x; i < nvec; i += 256) {
     float f[8];
-    unpack8v(reinterpret_cast<const uint4*>(row)[i], f);
+    load8(row, i, f);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) mx = fmaxf(mx, f[j]);
+    for (int j = 0; j < 8; ++j)
+      if (i * 8 + j < L) mx = fmaxf(mx, f[j]);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, o));
@@ -202,9 +216,10 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(__nv_bfloat16* s, lon
   float sum = 0.f;
   for (int i = threadIdx.x; i < nvec; i += 256) {
     float f[8];
-    unpack8v(reinterpret_cast<const uint4*>(row)[i], f);
+    load8(row, i, f);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) sum += exp2f((f[j] - mx) * k);
+    for (int j = 0; j < 8; ++j)
+      if (i * 8 + j < L) sum += exp2f((f[j] - mx) * k);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
@@ -216,10 +231,10 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(__nv_bfloat16* s, lon
   const float inv = 1.0f / sum;
   for (int i = threadIdx.x; i < nvec; i += 256) {
     float f[8];
-    unpack8v(reinterpret_cast<const uint4*>(row)[i], f);
+    load8(row, i, f);
 #pragma unroll
-    for (int j = 0; j < 8; ++j) f[j] = exp2f((f[j] - mx) * k) * inv;
-    reinterpret_cast<uint4*>(row)[i] = pack8v(f);
+    for (int j = 0; j < 8; ++j) f[j] = i * 8 + j < L ? exp2f((f[j] - mx) * k) * inv : 0.f;
+    reinterpret_cast<uint4*>(prow)[i] = pack8v(f);
   }
 }
 
@@ -301,11 +316,27 @@ extern "C" int b2f_nchw_to_nhwc_pad(const void* in, int in_is_f32, void* out, in
 extern "C" int b2f_softmax_rows(void* s, int64_t ld, int rows, int L, float scale, b2f_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!device_info().ok) return B2F_ERR_NODEVICE;
-  if (!s || rows <= 0 || L <= 0 || (L & 7) || (ld & 7)) return B2F_ERR_INVALID;
+  if (!s || rows <= 0 || L <= 0 || (ld & 7) || ld < ((L + 7) & ~7)) return B2F_ERR_INVALID;
   prof_begin(KC_OTHER, stream);
-  softmax_rows_kernel<<<rows, 256, 0, stream>>>(static_cast<__nv_bfloat16*>(s), ld, L, scale);
+  softmax_rows_kernel<__nv_bfloat16><<<rows, 256, 0, stream>>>(static_cast<__nv_bfloat16*>(s), ld,
+                                                               static_cast<__nv_bfloat16*>(s), ld, L, scale);
   prof_end(KC_OTHER, stream, 0.0, 4.0 * (double)rows * L);
   B2F_LAUNCHED("softmax_rows_kernel", 1);
+  return B2F_OK;
+}
+
+extern "C" int b2f_softmax_rows_f32(const void* s, int64_t lds, void* p, int64_t ldp, int rows, int L, float scale,
+                                    b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!device_info().ok) return B2F_ERR_NODEVICE;
+  const int L8 = (L + 7) & ~7;
+  if (!s || !p || rows <= 0 || L <= 0 || (lds & 7) || (ldp & 7) || lds < L8 || ldp < L8) return B2F_ERR_INVALID;
+  if ((reinterpret_cast<uintptr_t>(s) | reinterpret_cast<uintptr_t>(p)) & 15) return B2F_ERR_ALIGN;
+  prof_begin(KC_OTHER, stream);
+  softmax_rows_kernel<float><<<rows, 256, 0, stream>>>(static_cast<const float*>(s), lds,
+                                                       static_cast<__nv_bfloat16*>(p), ldp, L, scale);
+  prof_end(KC_OTHER, stream, 0.0, 6.0 * (double)rows * L);
+  B2F_LAUNCHED("softmax_rows_kernel<float>", 1);
   return B2F_OK;
 }
 

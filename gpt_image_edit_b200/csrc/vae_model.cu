@@ -4,7 +4,9 @@
 //   3x3 convs            wgmma implicit GEMM (conv.cu), residual add fused into conv2's epilogue
 //   1x1 shortcut convs   plain wgmma GEMM over [pixels, C]
 //   GroupNorm+SiLU       two HBM-bound passes (vae_kernels.cu)
-//   mid-block attention  single head, dh = C: QK^T and PV as wgmma GEMMs around a row softmax
+//   mid-block attention  single head, dh = C: QK^T (fp32 scores, through the weight-gradient GEMM) and PV as wgmma
+//                        GEMMs around a row softmax, over the P = h*w latent pixels padded to P8 = round_up(P, 8)
+// b2f_vae_set_stop_stage ends a run after one stage of the numbering in b2f.h (tests read each stage's activation).
 #include <map>
 #include <string>
 #include <vector>
@@ -20,6 +22,7 @@ struct VaeCtx {
   std::map<std::string, std::pair<const void*, int64_t>> bound;
   bool finalized = false;
   int max_c = 0;
+  int stop_stage = 0;  // b2f_vae_set_stop_stage: 0 runs to the end
 };
 
 struct VaeRun {
@@ -28,8 +31,20 @@ struct VaeRun {
   bf16_t *X, *A, *B;   // three activation buffers (NHWC)
   bf16_t* attn_ws;     // mid-attention scratch
   double* stats;       // [N,32,2]
+  bf16_t* ws0;         // start of the 256-aligned workspace
   int N;
   int rc = 0;
+  int stage = 0;       // stages finished so far
+
+  // Ends a stage whose activation X is [N, h, w, ch]; true when the run stops here (or has failed): the activation is
+  // then at the start of the workspace.
+  bool stage_done(int h, int w, int ch) {
+    if (rc) return true;
+    if (++stage != c->stop_stage) return false;
+    if (X != ws0) run(cuda_err(cudaMemcpyAsync(ws0, X, (size_t)N * h * w * ch * sizeof(bf16_t), cudaMemcpyDeviceToDevice,
+                                               st), "vae stage copy"));
+    return true;
+  }
 
   const bf16_t* w(const std::string& k) {
     auto it = c->bound.find(k);
@@ -76,28 +91,41 @@ struct VaeRun {
     const bf16_t* wo = w(name + ".to_out.0.weight");
     const bf16_t* bo = w(name + ".to_out.0.bias");
     if (rc) return;
+    // The scores stay in fp32 (diffusers' SDPA keeps them so; bf16 logits err by |s| 2^-9 in every exponent): S = Q K^T
+    // is the weight-gradient GEMM of Q^T and K^T.  Queries, keys and values are padded to P8 pixels with zeros: the
+    // softmax normalises [0, P) and zeroes [P, P8), and P V contracts over P8 against zero columns of V^T.
+    const long long P8 = (P + 7) / 8 * 8;
     bf16_t* qkv = attn_ws;                          // [P, 3C]
-    bf16_t* vT = qkv + P * 3 * C;                   // [C, P]
-    bf16_t* S = vT + (long long)C * P;              // [P, P]
+    bf16_t* qT = qkv + P * 3 * C;                   // [C, P8] x 3: Q^T, K^T, V^T, columns [P, P8) zero
+    bf16_t* kT = qT + (long long)C * P8;
+    bf16_t* vT = kT + (long long)C * P8;
+    bf16_t* S = vT + (long long)C * P8;             // [P, P8] bf16 probabilities
+    float* Sf = reinterpret_cast<float*>(S + P * P8);  // [P8, P8] fp32 scores
     const float scale = 1.0f / sqrtf((float)C);
+    if (P8 != P) run(cuda_err(cudaMemsetAsync(qT, 0, (size_t)3 * C * P8 * sizeof(bf16_t), st), "vae attn pad"));
     for (int n = 0; n < N && !rc; ++n) {
       bf16_t* xa = A + (long long)n * P * C;
       bf16_t* xx = X + (long long)n * P * C;
       run(b2f_gemm_bf16(xa, C, 0, wqkv, C, bqkv, qkv, 3 * C, 0, 1, (int)P, 3 * C, C, B2F_EPI_BIAS, nullptr, 0, 0,
                         nullptr, 0, st));
-      run(b2f_gemm_bf16(qkv, 3 * C, 0, qkv + C, 3 * C, nullptr, S, P, 0, 1, (int)P, (int)P, C, B2F_EPI_BIAS,
-                        nullptr, 0, 0, nullptr, 0, st));
-      run(b2f_softmax_rows(S, P, (int)P, (int)P, scale, st));
-      run(b2f_transpose_bf16(qkv + 2 * C, 3 * C, vT, P, (int)P, C, st));
-      run(b2f_gemm_bf16(S, P, 0, vT, P, nullptr, xa, C, 0, 1, (int)P, C, (int)P, B2F_EPI_BIAS, nullptr, 0, 0,
+      run(b2f_transpose_bf16(qkv, 3 * C, qT, P8, (int)P, C, st));
+      run(b2f_transpose_bf16(qkv + C, 3 * C, kT, P8, (int)P, C, st));
+      run(b2f_transpose_bf16(qkv + 2 * C, 3 * C, vT, P8, (int)P, C, st));
+      run(b2f_gemm_wgrad(qT, P8, 0, kT, P8, 0, Sf, P8, 1, C, (int)P8, (int)P8, 0, st));
+      run(b2f_softmax_rows_f32(Sf, P8, S, P8, (int)P, (int)P, scale, st));
+      run(b2f_gemm_bf16(S, P8, 0, vT, P8, nullptr, xa, C, 0, 1, (int)P, C, (int)P8, B2F_EPI_BIAS, nullptr, 0, 0,
                         nullptr, 0, st));
       run(b2f_gemm_bf16(xa, C, 0, wo, C, bo, xx, C, 0, 1, (int)P, C, C, B2F_EPI_RESID, xx, C, 0, nullptr, 0, st));
     }
   }
-  void mid(const std::string& name, int H, int W, int C) {
+  // the mid block's three stages; true when the run stops inside it
+  bool mid(const std::string& name, int H, int W, int C) {
     resnet(name + ".resnets.0", H, W, C, C);
+    if (stage_done(H, W, C)) return true;
     attention(name + ".attentions.0", (long long)H * W, C);
+    if (stage_done(H, W, C)) return true;
     resnet(name + ".resnets.1", H, W, C, C);
+    return stage_done(H, W, C);
   }
   void swapXA() {
     bf16_t* t = X;
@@ -116,9 +144,10 @@ static void ws_layout(const b2f_vae_cfg& g, int N, int H, int W, size_t* act_ele
   size_t m = full * (size_t)(g.block_out[1] > g.block_out[0] ? g.block_out[1] : g.block_out[0]);
   if (m < full * 64) m = full * 64;
   *act_elems = m;
-  const size_t P = (size_t)(H / 8) * (W / 8);
+  const size_t P = (size_t)(H / 8) * (W / 8), P8 = (P + 7) / 8 * 8;
   const size_t C = g.block_out[3];
-  *attn_elems = P * 3 * C + C * P + P * P;
+  // qkv, Q^T / K^T / V^T, bf16 probabilities and fp32 scores (two bf16 elements each)
+  *attn_elems = P * 3 * C + 3 * C * P8 + P * P8 + 2 * P8 * P8;
 }
 
 }  // namespace b2f
@@ -150,6 +179,13 @@ int b2f_vae_bind_weight(b2f_vae* h, const char* key, const void* dptr, int64_t n
   return B2F_OK;
 }
 
+int b2f_vae_set_stop_stage(b2f_vae* h, int stage) {
+  VaeCtx* c = reinterpret_cast<VaeCtx*>(h);
+  if (!c || stage < 0) return B2F_ERR_INVALID;
+  c->stop_stage = stage;
+  return B2F_OK;
+}
+
 size_t b2f_vae_workspace_bytes(const b2f_vae* h, int N, int H, int W) {
   const VaeCtx* c = reinterpret_cast<const VaeCtx*>(h);
   if (!c || N <= 0 || H <= 0 || W <= 0) return 0;
@@ -167,6 +203,7 @@ static int vae_setup(VaeCtx* c, VaeRun* r, int N, int H, int W, void* ws, size_t
   r->c = c;
   r->st = st;
   r->N = N;
+  r->ws0 = reinterpret_cast<bf16_t*>(p);
   r->X = reinterpret_cast<bf16_t*>(p);
   r->A = reinterpret_cast<bf16_t*>(p + ab);
   r->B = reinterpret_cast<bf16_t*>(p + 2 * ab);
@@ -188,11 +225,13 @@ int b2f_vae_encode(b2f_vae* h, const void* image_nchw, int image_is_f32, int N, 
   r.run(b2f_nchw_to_nhwc_pad(image_nchw, image_is_f32, r.A, N, g.in_channels, H, W, 64, st));
   r.conv("encoder.conv_in", r.A, r.X, nullptr, H, W, 64, g.block_out[0]);
   int ch = g.block_out[0], hh = H, ww = W;
+  if (r.stage_done(hh, ww, ch)) return r.rc;
   for (int i = 0; i < 4; ++i) {
     for (int j = 0; j < g.layers_per_block; ++j) {
       r.resnet("encoder.down_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), hh, ww, ch,
                g.block_out[i]);
       ch = g.block_out[i];
+      if (r.stage_done(hh, ww, ch)) return r.rc;
     }
     if (i != 3) {
       r.conv("encoder.down_blocks." + std::to_string(i) + ".downsamplers.0.conv", r.X, r.A, nullptr, hh, ww,
@@ -200,9 +239,10 @@ int b2f_vae_encode(b2f_vae* h, const void* image_nchw, int image_is_f32, int N, 
       r.swapXA();
       hh /= 2;
       ww /= 2;
+      if (r.stage_done(hh, ww, ch)) return r.rc;
     }
   }
-  r.mid("encoder.mid_block", hh, ww, ch);
+  if (r.mid("encoder.mid_block", hh, ww, ch)) return r.rc;
   r.gn("encoder.conv_norm_out", r.X, r.A, (long long)hh * ww, ch, 1);
   r.conv("encoder.conv_out", r.A, static_cast<bf16_t*>(moments_nchw), nullptr, hh, ww, ch,
          2 * g.latent_channels, 1, 1);
@@ -222,18 +262,21 @@ static int vae_decode_impl(b2f_vae* h, const void* z_nchw, int N, int h_lat, int
   r.run(b2f_nchw_to_nhwc_pad(z_nchw, 0, r.A, N, g.latent_channels, h_lat, w_lat, 64, st));
   int ch = g.block_out[3], hh = h_lat, ww = w_lat;
   r.conv("decoder.conv_in", r.A, r.X, nullptr, hh, ww, 64, ch);
-  r.mid("decoder.mid_block", hh, ww, ch);
+  if (r.stage_done(hh, ww, ch)) return r.rc;
+  if (r.mid("decoder.mid_block", hh, ww, ch)) return r.rc;
   for (int i = 0; i < 4; ++i) {
     const int co = g.block_out[3 - i];
     for (int j = 0; j < g.layers_per_block + 1; ++j) {
       r.resnet("decoder.up_blocks." + std::to_string(i) + ".resnets." + std::to_string(j), hh, ww, ch, co);
       ch = co;
+      if (r.stage_done(hh, ww, ch)) return r.rc;
     }
     if (i != 3) {
       r.run(b2f_upsample2x(r.X, r.A, N, hh, ww, ch, st));
       hh *= 2;
       ww *= 2;
       r.conv("decoder.up_blocks." + std::to_string(i) + ".upsamplers.0.conv", r.A, r.X, nullptr, hh, ww, ch, ch);
+      if (r.stage_done(hh, ww, ch)) return r.rc;
     }
   }
   r.gn("decoder.conv_norm_out", r.X, r.A, (long long)hh * ww, ch, 1);

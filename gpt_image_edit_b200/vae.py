@@ -82,6 +82,30 @@ def _spec(cfg):
     return s
 
 
+def stage_shapes(cfg, side: str, h: int, w: int) -> list:
+    """(name, C, h, w) of every stage's output in the engine's numbering (b2f_vae_set_stop_stage, include/b2f.h);
+    h, w: the image size for the encoder, the latent size for the decoder."""
+    boc, L = cfg.block_out_channels, cfg.layers_per_block
+    mid = lambda p, c, h, w: [(f"{p}.mid_block.{n}", c, h, w) for n in ("resnets.0", "attentions.0", "resnets.1")]
+    if side == "encoder":
+        out = [("encoder.conv_in", boc[0], h, w)]
+        for i, c in enumerate(boc):
+            out += [(f"encoder.down_blocks.{i}.resnets.{j}", c, h, w) for j in range(L)]
+            if i != len(boc) - 1:
+                h, w = h // 2, w // 2
+                out.append((f"encoder.down_blocks.{i}.downsamplers.0", c, h, w))
+        return out + mid("encoder", boc[-1], h, w) + [("encoder.conv_out", 2 * cfg.latent_channels, h, w)]
+    if side != "decoder":
+        raise ValueError(f"side must be 'encoder' or 'decoder', not {side!r}")
+    out = [("decoder.conv_in", boc[-1], h, w)] + mid("decoder", boc[-1], h, w)
+    for i, c in enumerate(reversed(boc)):
+        out += [(f"decoder.up_blocks.{i}.resnets.{j}", c, h, w) for j in range(L + 1)]
+        if i != len(boc) - 1:
+            h, w = 2 * h, 2 * w
+            out.append((f"decoder.up_blocks.{i}.upsamplers.0", c, h, w))
+    return out + [("decoder.conv_out", cfg.out_channels, h, w)]
+
+
 class DiagonalGaussianDistribution:
     """diffusers' latent_dist over the moments the encoder produced (mean | logvar on dim 1)."""
 
@@ -149,7 +173,7 @@ class B200AutoencoderKL(torch.nn.Module):
         self.use_slicing = False
 
     def enable_tiling(self, *a, **k):
-        raise _lib.B2FError("tiled VAE encode / decode is not built: a 1024x1024 decode needs < 2 GB of workspace here")
+        raise _lib.B2FError("tiled VAE encode / decode is not built: a 1024x1024 decode needs < 4 GB of workspace here")
 
     def disable_tiling(self):
         pass
@@ -302,6 +326,29 @@ class B200AutoencoderKL(torch.nn.Module):
         img = torch.empty((N, self.config.out_channels, 8 * h, 8 * w), device=self._dev, dtype=torch.bfloat16)
         check(_lib.lib.b2f_vae_decode(self._h, ptr(z), N, h, w, ptr(img), ptr(ws), n, stream_ptr()), "b2f_vae_decode")
         return SimpleNamespace(sample=img) if return_dict else (img,)
+
+    # ------------------------------------------------------------------ stages (tests)
+    @torch.no_grad()
+    def stage_output(self, x: torch.Tensor, side: str, stage: int) -> torch.Tensor:
+        """The NCHW bf16 activation after stage `stage` (1-based, `stage_shapes` order) of encode(x) or decode(x), run
+        through the engine's own code path up to that stage; the last stage is the moments / the image."""
+        shapes = stage_shapes(self.config, side, *x.shape[-2:])
+        if not 1 <= stage <= len(shapes):
+            raise ValueError(f"{side} stage {stage} outside 1..{len(shapes)}")
+        if stage == len(shapes):
+            return self.encode(x).latent_dist.parameters if side == "encoder" else self.decode(x, return_dict=False)[0]
+        check(_lib.lib.b2f_vae_set_stop_stage(self._h, stage), "b2f_vae_set_stop_stage")
+        sliced, self.use_slicing = self.use_slicing, False      # one run over the whole batch fills the workspace
+        try:
+            self.encode(x) if side == "encoder" else self.decode(x)
+        finally:
+            self.use_slicing = sliced
+            check(_lib.lib.b2f_vae_set_stop_stage(self._h, 0), "b2f_vae_set_stop_stage")
+        _, c, h, w = shapes[stage - 1]
+        n = x.shape[0] * h * w * c
+        off = -self._ws.data_ptr() % 256
+        act = self._ws[off:off + 2 * n].view(torch.bfloat16).view(x.shape[0], h, w, c)
+        return act.permute(0, 3, 1, 2).contiguous()
 
     @torch.no_grad()
     def decode_u8(self, z: torch.Tensor) -> torch.Tensor:

@@ -34,7 +34,8 @@ typedef void* b2f_stream_t; /* cudaStream_t */
 
 const char* b2f_strerror(int code);
 /* ABI version; bumped on any signature change or addition (2: LoRA entry points, 3: FP8 entry points, 4: FP8
- * attention, 5: first-block cache, 6: GEMM tile override, 7: FP8 GEMMs with unfused LoRA). */
+ * attention, 5: first-block cache, 6: GEMM tile override, 7: FP8 GEMMs with unfused LoRA, 8: VAE stop stage, ragged
+ * and fp32-input softmax rows). */
 int b2f_version(void);
 /* Device facts the host needs for grid sizing / reporting. Returns B2F_ERR_NODEVICE without GPU. */
 int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin);
@@ -579,8 +580,14 @@ int b2f_upsample2x(const void* in, void* out, int N, int H, int W, int C, b2f_st
 /* NCHW (bf16, or fp32 when in_is_f32) -> NHWC bf16 with channels zero-padded to Cpad. */
 int b2f_nchw_to_nhwc_pad(const void* in, int in_is_f32, void* out, int N, int C, int H, int W,
                          int Cpad, b2f_stream_t stream);
-/* In-place row softmax p = softmax(scale * s) over rows of length L (bf16, fp32 math). */
+/* In-place row softmax p = softmax(scale * s) over rows of length L (bf16, fp32 math).  Any L >= 1; the pitch ld must be
+ * a multiple of 8 and at least round_up(L, 8): columns [L, round_up(L, 8)) of every row are written as zeros, columns
+ * past that are not touched. */
 int b2f_softmax_rows(void* s, int64_t ld, int rows, int L, float scale, b2f_stream_t stream);
+/* The same from fp32 scores s [rows, lds] into bf16 p [rows, ldp] (no rounding of the logits); same rules on L and the
+ * pitches, 16-byte aligned s and p. */
+int b2f_softmax_rows_f32(const void* s, int64_t lds, void* p, int64_t ldp, int rows, int L, float scale,
+                         b2f_stream_t stream);
 /* out[c, r] = in[r, c] for an [R, Cc] bf16 matrix. */
 int b2f_transpose_bf16(const void* in, int64_t ld_in, void* out, int64_t ld_out, int R, int Cc,
                        b2f_stream_t stream);
@@ -726,6 +733,16 @@ int b2f_vae_create(b2f_vae** out, const b2f_vae_cfg* cfg);
 void b2f_vae_destroy(b2f_vae* ctx);
 int b2f_vae_bind_weight(b2f_vae* ctx, const char* key, const void* dptr, int64_t numel);
 size_t b2f_vae_workspace_bytes(const b2f_vae* ctx, int N, int H, int W);
+/* For tests only: later encode / decode calls on ctx stop after stage `stage` (1-based; 0, the default, runs to the
+ * end) and leave that stage's activation, NHWC bf16 [N, h, w, C], at the start of the workspace rounded up to 256 bytes;
+ * the output tensor is not written.  Stages, with L = layers_per_block:
+ *   encoder  1 conv_in; per down block i = 0..3: L ResnetBlock2D stages, then (i < 3) the downsampler (pad + stride-2
+ *            conv); mid_block resnets.0, attentions.0, resnets.1; conv_norm_out + conv_out (the moments).
+ *            4L + 8 stages.
+ *   decoder  1 conv_in; mid_block resnets.0, attentions.0, resnets.1; per up block i = 0..3: L + 1 ResnetBlock2D
+ *            stages, then (i < 3) nearest 2x upsample + conv; conv_norm_out + conv_out (the image).  4L + 12 stages.
+ * A stop at or past the last stage is a full run.  The stop is a host-side check between launches. */
+int b2f_vae_set_stop_stage(b2f_vae* ctx, int stage);
 /* image -> moments [N, 2*latent, H/8, W/8] bf16 (mean | logvar, un-clamped; `latent_dist.mode()` is the first half).
  * image_is_f32 selects the input format: 0 = bf16 [N,3,H,W], 1 = fp32 [N,3,H,W], 2 = uint8 [N,H,W,3] pixels (PIL / numpy
  * layout): the reference's host-side normalisation `(u/255 - 0.5)/0.5` and `.to(bf16)` (univa/serve/cli.py:99-116) run inside

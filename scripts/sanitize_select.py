@@ -34,6 +34,11 @@ WANT = [
                                     "test_attention_fp8_matches_emulation[1-255]", "test_attention_fp8_refusals"]),
     ("tests/test_elementwise_gpu.py", ["test_ln_modulate_matches_eager_chain[1-33-256]", "test_ln_modulate_matches_eager_chain[2-300-3072]",
                                        "test_rmsnorm_rope_matches_eager_chain", "test_euler_step_bit_exact"]),
+    # the VAE's composed encode / decode stage by stage at toy widths: padded (P = 35) and unpadded (P = 96) attention
+    ("tests/test_vae_stages_gpu.py", ["test_stagewise_vae_matches_fp64[toy_40x56-encoder]",
+                                      "test_stagewise_vae_matches_fp64[toy_40x56-decoder]",
+                                      "test_stagewise_vae_matches_fp64[toy_64x96-encoder]",
+                                      "test_stagewise_vae_matches_fp64[toy_64x96-decoder]"]),
     ("tests/test_vae_gpu.py", ["test_conv3x3_matches_torch[1-8-16-64-128-1]", "test_conv3x3_matches_torch[1-33-50-64-256-1]",
                                "test_conv3x3_matches_torch[1-32-48-128-128-2]", "test_groupnorm_silu_matches_torch_chain[1-48-32-1]"]),
 ]

@@ -656,18 +656,48 @@ def test_groupnorm_silu_edges(C, P):
     c.finish()
 
 
-@pytest.mark.parametrize("L_", [8, 2056])
+# ragged L (the VAE's mid-block attention over P = 13 x 21 and 90 x 182 latent pixels) and its 1024^2 row, L = 16384
+@pytest.mark.parametrize("L_", [8, 2056, 273, 16380, 16384])
 def test_softmax_rows_edges(L_):
     from gpt_image_edit_b200 import _lib as L
 
     g = _g(L_)
     rows = 5
-    s = _bf(rows, L_ + 8, g=g, scale=4.0)
+    L8 = -(-L_ // 8) * 8
+    s = _bf(rows, L8 + 8, g=g, scale=4.0)                 # pitch ld = L8 + 8: one vector past the padded row
     x = s[:, :L_].clone()
     before = s.clone()
     L.check(L.lib.b2f_softmax_rows(L.ptr(s), s.stride(0), rows, L_, 512 ** -0.5, L.stream_ptr()), "softmax")
     emu, fl, mth = RR.softmax_rows_emu(x, 512 ** -0.5)
     c = R.Checker(f"softmax_rows L{L_}")
     c.bf16("p", s[:, :L_], emu, fl, math_ref=mth, rel_l2_max=1e-2, dims=("row", "col"), **TH)
-    _outside(c, "p", s, before, (slice(None), slice(0, L_)))
+    c.equal("p: zeroed tail [L, round_up(L, 8))", s[:, L_:L8].view(torch.int16), torch.zeros_like(s[:, L_:L8]).view(torch.int16))
+    _outside(c, "p", s, before, (slice(None), slice(0, L8)))
+    c.finish()
+    # the pitch must be a multiple of 8 and hold the padded row
+    for ld in (L8 - 8, L8 + 4):
+        if ld > 0 and ld != L8:
+            assert L.lib.b2f_softmax_rows(L.ptr(s), ld, 1, L_, 1.0, L.stream_ptr()) != 0, f"ld {ld} accepted"
+
+
+# fp32 scores in, bf16 probabilities out (the VAE's mid-block attention, whose logits are never rounded to bf16)
+@pytest.mark.parametrize("L_", [8, 273, 16380, 16384])
+def test_softmax_rows_f32_edges(L_):
+    from gpt_image_edit_b200 import _lib as L
+
+    g = _g(L_ + 1)
+    rows = 5
+    L8 = -(-L_ // 8) * 8
+    s = torch.randn(rows, L8 + 8, device="cuda", generator=g) * 90.0      # unscaled logits of std 4 after 512^-0.5
+    s_before = s.clone()
+    p = torch.full((rows, L8 + 16), math.nan, device="cuda", dtype=BF)
+    before = p.clone()
+    L.check(L.lib.b2f_softmax_rows_f32(L.ptr(s), s.stride(0), L.ptr(p), p.stride(0), rows, L_, 512 ** -0.5,
+                                       L.stream_ptr()), "softmax f32")
+    emu, fl, mth = RR.softmax_rows_emu(s[:, :L_], 512 ** -0.5)
+    c = R.Checker(f"softmax_rows_f32 L{L_}")
+    c.bf16("p", p[:, :L_], emu, fl, math_ref=mth, rel_l2_max=1e-2, dims=("row", "col"), **TH)
+    c.equal("p: zeroed tail [L, round_up(L, 8))", p[:, L_:L8].view(torch.int16), torch.zeros_like(p[:, L_:L8]).view(torch.int16))
+    _outside(c, "p", p, before, (slice(None), slice(0, L8)))
+    c.equal("s untouched", s.view(torch.int32), s_before.view(torch.int32))
     c.finish()
