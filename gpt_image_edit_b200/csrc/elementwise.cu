@@ -200,26 +200,28 @@ __global__ void __launch_bounds__(256) quant_fp8_rows_kernel(const QuantParams p
 }
 
 // ------------------------------------------------------------------------------------------------
-// Per-head RMSNorm (eps, weight) + interleaved-pair RoPE, in place on the Q and K column blocks of
-// a fused QKV projection buffer [batch, S, >= 2*H*128]:
+// Per-head RMSNorm (eps, weight) + interleaved-pair RoPE on the Q and K column blocks of a fused QKV
+// projection buffer [batch, S, >= 2*H*128], into an output of the same layout:
 //   y = bf16(x * rsqrt(mean(x^2) + eps));  z = bf16(y * w);  out = bf16(z*cos + rot(z)*sin)
 // (diffusers RMSNorm + apply_rotary_emb, SURVEY.md A.2).  Half a warp owns one 128-wide head vector
 // (8 elements = 4 RoPE pairs per lane); lanes 0-15 do Q, lanes 16-31 do K of the same head.
 // The first `n_a` tokens of every batch item use weight set A (norm_added_q/k: text tokens), the
-// rest weight set B (norm_q/k).
+// rest weight set B (norm_q/k).  The output may be the input (b2f_rmsnorm_rope): a lane reads its 8
+// elements of a head with plain loads before it writes them, and no other thread touches them.
 // Algorithmic bytes per token: 2 (Q,K) * H*128 * 2 B read + the same written.
-struct NormRopeParams {
-  __nv_bfloat16* q;
-  __nv_bfloat16* k;
-  long long ld, batch_stride;
+struct NormRopeOutParams {
+  const __nv_bfloat16* xq;
+  const __nv_bfloat16* xk;
+  __nv_bfloat16* oq;
+  __nv_bfloat16* ok;
+  long long ldx, x_batch_stride, ldo, o_batch_stride;
   const __nv_bfloat16 *wq_a, *wk_a, *wq_b, *wk_b;
   const float* cos;  // [S, 128]
   const float* sin;
   int batch, S, H, n_a;
   float eps;
 };
-
-__global__ void __launch_bounds__(256) rmsnorm_rope_kernel(const NormRopeParams p) {
+__global__ void __launch_bounds__(256) rmsnorm_rope_out_kernel(const NormRopeOutParams p) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long tok = (long long)blockIdx.x * 8 + warp;
   if (tok >= (long long)p.batch * p.S) return;
@@ -227,7 +229,8 @@ __global__ void __launch_bounds__(256) rmsnorm_rope_kernel(const NormRopeParams 
   const int s = int(tok - (long long)b * p.S);
   const int is_k = lane >> 4;
   const int l16 = lane & 15;
-  __nv_bfloat16* base = (is_k ? p.k : p.q) + b * p.batch_stride + s * p.ld + l16 * 8;
+  const __nv_bfloat16* xb = (is_k ? p.xk : p.xq) + b * p.x_batch_stride + s * p.ldx + l16 * 8;
+  __nv_bfloat16* ob = (is_k ? p.ok : p.oq) + b * p.o_batch_stride + s * p.ldo + l16 * 8;
   const bool set_a = s < p.n_a;
   const __nv_bfloat16* wptr = is_k ? (set_a ? p.wk_a : p.wk_b) : (set_a ? p.wq_a : p.wq_b);
   float w[8], cs[8], sn[8];
@@ -243,9 +246,8 @@ __global__ void __launch_bounds__(256) rmsnorm_rope_kernel(const NormRopeParams 
   }
 #pragma unroll 4
   for (int h = 0; h < p.H; ++h) {
-    __nv_bfloat16* ptr = base + h * 128;
     float x[8];
-    unpack8(*reinterpret_cast<const uint4*>(ptr), x);
+    unpack8(*reinterpret_cast<const uint4*>(xb + h * 128), x);
     float ss = 0.f;
 #pragma unroll
     for (int j = 0; j < 8; ++j) ss += x[j] * x[j];
@@ -260,7 +262,7 @@ __global__ void __launch_bounds__(256) rmsnorm_rope_kernel(const NormRopeParams 
       o8[j] = z[j] * cs[j] - z[j + 1] * sn[j];
       o8[j + 1] = z[j + 1] * cs[j + 1] + z[j] * sn[j + 1];
     }
-    *reinterpret_cast<uint4*>(ptr) = pack8(o8);
+    *reinterpret_cast<uint4*>(ob + h * 128) = pack8(o8);
   }
 }
 
@@ -506,15 +508,43 @@ extern "C" int b2f_rmsnorm_rope(void* q, void* k, int64_t ld, int64_t batch_stri
   if (head_dim != 128) return B2F_ERR_UNSUPPORTED;
   if (n_a > 0 && (!wq_a || !wk_a)) return B2F_ERR_INVALID;
   if ((ld & 7) || (batch_stride & 7)) return B2F_ERR_ALIGN;
-  NormRopeParams p{static_cast<__nv_bfloat16*>(q), static_cast<__nv_bfloat16*>(k), ld, batch_stride,
-                   static_cast<const __nv_bfloat16*>(wq_a), static_cast<const __nv_bfloat16*>(wk_a),
-                   static_cast<const __nv_bfloat16*>(wq_b), static_cast<const __nv_bfloat16*>(wk_b),
-                   cos, sin, batch, S, H, n_a, eps};
+  NormRopeOutParams p{static_cast<const __nv_bfloat16*>(q), static_cast<const __nv_bfloat16*>(k),
+                      static_cast<__nv_bfloat16*>(q), static_cast<__nv_bfloat16*>(k), ld, batch_stride, ld, batch_stride,
+                      static_cast<const __nv_bfloat16*>(wq_a), static_cast<const __nv_bfloat16*>(wk_a),
+                      static_cast<const __nv_bfloat16*>(wq_b), static_cast<const __nv_bfloat16*>(wk_b),
+                      cos, sin, batch, S, H, n_a, eps};
   const long long total = (long long)batch * S;
   prof_begin(KC_NORMROPE, stream);
-  rmsnorm_rope_kernel<<<(unsigned)((total + 7) / 8), 256, 0, stream>>>(p);
+  rmsnorm_rope_out_kernel<<<(unsigned)((total + 7) / 8), 256, 0, stream>>>(p);
   prof_end(KC_NORMROPE, stream, 0.0, 8.0 * (double)total * H * 128);
-  B2F_LAUNCHED("rmsnorm_rope_kernel", 1);
+  B2F_LAUNCHED("rmsnorm_rope_out_kernel", 1);
+  return B2F_OK;
+}
+
+extern "C" int b2f_rmsnorm_rope_out(const void* xq, const void* xk, int64_t ldx, int64_t x_bs, void* oq, void* ok,
+                                    int64_t ldo, int64_t o_bs, const void* wq_a, const void* wk_a, const void* wq_b,
+                                    const void* wk_b, const float* cos, const float* sin, int batch, int S, int H,
+                                    int n_a, float eps, b2f_stream_t stream_) {
+  cudaStream_t st = static_cast<cudaStream_t>(stream_);
+  if (!xq || !xk || !oq || !ok || !wq_b || !wk_b || !cos || !sin || batch <= 0 || S <= 0 || H <= 0) return B2F_ERR_INVALID;
+  if (n_a > 0 && (!wq_a || !wk_a)) return B2F_ERR_INVALID;
+  if ((ldx | x_bs | ldo | o_bs) & 7) return B2F_ERR_ALIGN;
+  NormRopeOutParams p{};
+  p.xq = static_cast<const __nv_bfloat16*>(xq);
+  p.xk = static_cast<const __nv_bfloat16*>(xk);
+  p.oq = static_cast<__nv_bfloat16*>(oq);
+  p.ok = static_cast<__nv_bfloat16*>(ok);
+  p.ldx = ldx; p.x_batch_stride = x_bs; p.ldo = ldo; p.o_batch_stride = o_bs;
+  p.wq_a = static_cast<const __nv_bfloat16*>(n_a > 0 ? wq_a : wq_b);
+  p.wk_a = static_cast<const __nv_bfloat16*>(n_a > 0 ? wk_a : wk_b);
+  p.wq_b = static_cast<const __nv_bfloat16*>(wq_b);
+  p.wk_b = static_cast<const __nv_bfloat16*>(wk_b);
+  p.cos = cos; p.sin = sin; p.batch = batch; p.S = S; p.H = H; p.n_a = n_a; p.eps = eps;
+  const long long tokens = (long long)batch * S;
+  prof_begin(KC_NORMROPE, st);
+  rmsnorm_rope_out_kernel<<<(unsigned)((tokens + 7) / 8), 256, 0, st>>>(p);
+  prof_end(KC_NORMROPE, st, 0, 8.0 * tokens * H * 128);
+  B2F_LAUNCHED("rmsnorm_rope_out_kernel", 1);
   return B2F_OK;
 }
 

@@ -10,11 +10,12 @@
 //   FP8 mode              e4m3 A and W (per-token / per-channel fp32 scales), m64n128k32 e4m3 wgmma; see Fp8Params
 //   epilogue              x = bf16(acc + bias) from registers → the consumer's own bf16 staging tile →
 //                         act/gate/resid → global with 16-byte accesses, 16 threads per row; a fused QKV head runs one
-//                         thread per row; the fp32 wgrad output goes straight from registers
+//                         thread per row (the epilogue tail, shared with the wide tile); the fp32 wgrad output goes
+//                         straight from registers
 //
 // gemm_wide_kernel     the plain forward GEMM on 128 x 256 tiles for the loop's large linears: both consumers on one tile,
-//                      one m64n256k16 each per k16 step, a 3-stage ring of 48 KB stages; launch_gemm picks the tile per
-//                      launch from the shape (tile_width)
+//                      one m64n256k16 each per k16 step, a 3-stage ring of 48 KB stages, the same epilogue tail with
+//                      32 threads per row; launch_gemm picks the tile per launch from the shape (tile_width)
 //
 // Every output element sees the same k16 accumulation order as a one-tile-per-CTA kernel with the same k-blocks, on
 // either tile.
@@ -195,7 +196,7 @@ __device__ __forceinline__ void unpack_bf16x8(const uint4 q, float (&v)[8]) {
 // One 128-column head of a fused QKV projection for one token, from its row of the staged tile x = bf16(acc + bias):
 //   y = bf16(x * rsqrt(mean(x^2) + eps));  z = bf16(y * w);
 //   out = bf16(z * cos + rot(z) * sin)        (diffusers RMSNorm + apply_rotary_emb, SURVEY.md A.2)
-// — the same rounding chain as rmsnorm_rope_kernel, but without the extra HBM round trip.  The sum of squares runs over
+// — the same rounding chain as rmsnorm_rope_out_kernel, but without the extra HBM round trip.  The sum of squares runs over
 // the columns in order, one thread per row.  Every rounding is the packed cvt.rn.bf16x2.
 __device__ __forceinline__ void epilogue_head_norm_rope(const GemmParams& p, const uint8_t* srow, int n_head0,
                                                         long long row, __nv_bfloat16* out_row, bool is_k) {
@@ -236,6 +237,93 @@ __device__ __forceinline__ void epilogue_head_norm_rope(const GemmParams& p, con
       o[jj] = pack_bf16x2(z0 * cc8[2 * jj] - z1 * sc8[2 * jj], z1 * cc8[2 * jj + 1] + z0 * sc8[2 * jj + 1]);
     }
     *reinterpret_cast<uint4*>(out_row + n_head0 + c) = make_uint4(o[0], o[1], o[2], o[3]);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------- epilogue tail
+// What both forward kernels run once a consumer's accumulators are final: stage_bias into the consumer's staging rows,
+// tile_out to find where the tile goes, then epilogue_head_norm_rope or epilogue_rows from the staged rows.
+
+// x = bf16(acc + bias) of a thread's 2 x 2 accumulator group a[0..3] (rows r, r + 8; columns col, col + 1, whose bias
+// is b2) into a staging tile of PITCH bytes per row, s pointing at (r, col).
+template <int PITCH>
+__device__ __forceinline__ void stage_bias(uint8_t* s, const float* a, bool has_bias, float2 b2) {
+  float x0 = a[0], x1 = a[1], x2 = a[2], x3 = a[3];
+  if (has_bias) {
+    x0 += b2.x;
+    x1 += b2.y;
+    x2 += b2.x;
+    x3 += b2.y;
+  }
+  *reinterpret_cast<uint32_t*>(s) = pack_bf16x2(x0, x1);
+  *reinterpret_cast<uint32_t*>(s + 8 * PITCH) = pack_bf16x2(x2, x3);
+}
+
+// Where the tile whose first column is n_tile0, of batch item bb, goes.  With the fused QKV epilogue a tile of Q or K
+// heads (norm 0 / 1) goes through epilogue_head_norm_rope, a V tile is a plain bias store, and a tile at or past
+// split_n goes to the second output block with epi2.  Every other tile stores epi(x) at base + row * ld + column.
+struct TileOut {
+  int norm;   // 0 / 1: RMS-normalised Q / K heads; -1: none
+  int epi;
+  __nv_bfloat16* base;
+  long long ld;
+};
+// One return for every tile: an early return for the Q / K tiles merges base into a value NVVM no longer knows to be a
+// global pointer, and the epilogues' 16-byte stores become generic ones.
+__device__ __forceinline__ TileOut tile_out(const GemmParams& p, int n_tile0, int bb) {
+  TileOut o{-1, p.epi, p.out + bb * p.out_bs, p.ldc};
+  if (o.epi == B2F_EPI_QKV_NORM_ROPE) {
+    const int which = n_tile0 / p.d_model;   // 0 = Q, 1 = K, 2 = V, >= 3: second output block
+    if (which < 2) {
+      o.norm = which;
+    } else {
+      const bool second = p.split_n > 0 && n_tile0 >= p.split_n;
+      o.epi = second ? p.epi2 : B2F_EPI_BIAS;
+      if (second) {
+        o.base = p.out2 + bb * p.out2_bs - p.split_n;
+        o.ld = p.ldc2;
+      }
+    }
+  }
+  return o;
+}
+
+// epi over ROWS staged rows of PITCH bytes, global rows row_c, row_c + 1, ...: TPR threads per row, one 8-column group
+// each, so the 128 threads of a consumer cover STEP = 128 / TPR rows at a time.  A thread's rows go in batches of RB
+// whose residual / pre-activation loads are all issued before the first store, so their latencies overlap; a batch,
+// not all of them, keeps the unrolled activation code small.  BWD: the backward epilogues (DGELU / DSILU) can occur.
+template <int TPR, int ROWS, int PITCH, bool BWD>
+__device__ __forceinline__ void epilogue_rows(const GemmParams& p, const TileOut& o, const uint8_t* stg, int tid,
+                                              long long row_c, int n_tile0, int bb) {
+  constexpr int STEP = 128 / TPR, RB = 4;
+  const int cg = tid % TPR;
+  const int n = n_tile0 + 8 * cg;
+  if (n >= p.N) return;
+  const bool reads_resid = o.epi == B2F_EPI_GATE_RESID || o.epi == B2F_EPI_RESID ||
+                           (BWD && (o.epi == B2F_EPI_DGELU || o.epi == B2F_EPI_DSILU));
+  const __nv_bfloat16* gate_row = p.gate ? p.gate + (long long)bb * p.gate_ld : nullptr;
+  const uint4 gq = o.epi == B2F_EPI_GATE_RESID ? __ldg(reinterpret_cast<const uint4*>(gate_row + n))
+                                               : make_uint4(0, 0, 0, 0);
+#pragma unroll 1
+  for (int rb = tid / TPR; rb < ROWS; rb += STEP * RB) {   // staged rows rb + STEP r, r < RB
+    const long long row0 = row_c + rb;
+    if (row0 >= p.M) break;
+    uint4 rq[RB];
+#pragma unroll
+    for (int r = 0; r < RB; ++r) {
+      const long long row = row0 + STEP * r;
+      rq[r] = make_uint4(0, 0, 0, 0);
+      if (reads_resid && row < p.M)
+        rq[r] = *reinterpret_cast<const uint4*>(p.resid + bb * p.resid_bs + row * p.ldr + n);
+    }
+#pragma unroll
+    for (int r = 0; r < RB; ++r) {
+      const long long row = row0 + STEP * r;
+      if (row >= p.M) break;
+      float v[8];
+      unpack_bf16x8(*reinterpret_cast<const uint4*>(stg + (rb + STEP * r) * PITCH + cg * 16), v);
+      epilogue_group(o.epi, v, rq[r], gq, o.base + row * o.ld + n);
+    }
   }
 }
 
@@ -583,7 +671,7 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
           *reinterpret_cast<uint32_t*>(s0p) = pack_bf16x2(x0, x1);
           *reinterpret_cast<uint32_t*>(s0p + 8 * SROW) = pack_bf16x2(x2, x3);
         }
-      } else {
+      } else if constexpr (LORA) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const float* a = h ? acc1 : acc0;
@@ -594,77 +682,34 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
             x2 += b2.x;
             x3 += b2.y;
           }
-          if constexpr (LORA) {
-            if (lx.colscale) {
-              x0 *= cs2.x;
-              x1 *= cs2.y;
-              x2 *= cs2.x;
-              x3 *= cs2.y;
-            }
+          if (lx.colscale) {
+            x0 *= cs2.x;
+            x1 *= cs2.y;
+            x2 *= cs2.x;
+            x3 *= cs2.y;
           }
           uint8_t* s0 = stg + (64 * h + r_lo) * SROW + col * 2;
           *reinterpret_cast<uint32_t*>(s0) = pack_bf16x2(x0, x1);
           *reinterpret_cast<uint32_t*>(s0 + 8 * SROW) = pack_bf16x2(x2, x3);
         }
+      } else {
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+          stage_bias<SROW>(stg + (64 * h + r_lo) * SROW + col * 2, (h ? acc1 : acc0) + 4 * j, has_bias, b2);
       }
     }
     named_bar_sync(BAR_EPI + c, 128);
 
+    // 16 threads per row: a warp reads and writes two 256-byte row segments
     const int n_tile0 = n_blk * BLOCK_N;
-    const __nv_bfloat16* gate_row = p.gate ? p.gate + (long long)bb * p.gate_ld : nullptr;
-    int epi = p.epi;
-    __nv_bfloat16* out_base = p.out + bb * p.out_bs;
-    long long ld = p.ldc;
-    if (epi == B2F_EPI_QKV_NORM_ROPE) {
-      const int which = n_tile0 / p.d_model;  // 0 = Q, 1 = K, 2 = V, >= 3: second output block
-      if (which < 2) {
-        // one normalised head per tile: one thread per row
-        const long long row = (long long)mb * BLOCK_M + tid;
-        if (row < p.M)
-          epilogue_head_norm_rope(p, stg + tid * SROW, n_tile0, row, out_base + row * ld, which == 1);
-        continue;
-      }
-      const bool second = p.split_n > 0 && n_tile0 >= p.split_n;
-      epi = second ? p.epi2 : B2F_EPI_BIAS;
-      if (second) {
-        out_base = p.out2 + bb * p.out2_bs - p.split_n;
-        ld = p.ldc2;
-      }
+    const TileOut o = tile_out(p, n_tile0, bb);
+    if (o.norm >= 0) {
+      // one normalised head per tile: one thread per row
+      const long long row = (long long)mb * BLOCK_M + tid;
+      if (row < p.M) epilogue_head_norm_rope(p, stg + tid * SROW, n_tile0, row, o.base + row * o.ld, o.norm == 1);
+      continue;
     }
-    // 16 threads per row, one 8-column group each: a warp reads and writes two 256-byte row segments.  Rows go in
-    // batches of 4 per thread whose residual / pre-activation loads are all issued before the first store, so their
-    // latencies overlap; a batch, not all 16 rows, keeps the unrolled activation code small.
-    const int cg = tid & 15;
-    const int n = n_tile0 + 8 * cg;
-    if (n < p.N) {
-      constexpr int RB = 4;
-      const int r0 = tid >> 4;
-      const bool reads_resid = epi == B2F_EPI_GATE_RESID || epi == B2F_EPI_RESID || epi == B2F_EPI_DGELU ||
-                               epi == B2F_EPI_DSILU;
-      const uint4 gq = epi == B2F_EPI_GATE_RESID ? __ldg(reinterpret_cast<const uint4*>(gate_row + n))
-                                                 : make_uint4(0, 0, 0, 0);
-#pragma unroll 1
-      for (int rb = r0; rb < BLOCK_M; rb += 8 * RB) {     // tile rows rb + 8 r, r < RB
-        const long long row0 = (long long)mb * BLOCK_M + rb;
-        if (row0 >= p.M) break;
-        uint4 rq[RB];
-#pragma unroll
-        for (int r = 0; r < RB; ++r) {
-          const long long row = row0 + 8 * r;
-          rq[r] = make_uint4(0, 0, 0, 0);
-          if (reads_resid && row < p.M)
-            rq[r] = *reinterpret_cast<const uint4*>(p.resid + bb * p.resid_bs + row * p.ldr + n);
-        }
-#pragma unroll
-        for (int r = 0; r < RB; ++r) {
-          const long long row = row0 + 8 * r;
-          if (row >= p.M) break;
-          float v[8];
-          unpack_bf16x8(*reinterpret_cast<const uint4*>(stg + (rb + 8 * r) * SROW + cg * 16), v);
-          epilogue_group(epi, v, rq[r], gq, out_base + row * ld + n);
-        }
-      }
-    }
+    epilogue_rows<16, BLOCK_M, SROW, MODE != 0>(p, o, stg, tid, (long long)mb * BLOCK_M, n_tile0, bb);
   }
 }
 
@@ -675,8 +720,8 @@ gemm_bf16_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
 // reads about 17 % fewer operand bytes from shared memory (2 KB of A and 8 KB of W per 64 x 256 x 16 MACs instead of
 // 2 + 4 KB per 64 x 128 x 16) and moves 25 % fewer bytes through L2 and TMA (48 KB per 128 x 256 x 64 tile-k-block
 // instead of 32 KB per 128 x 128 x 64).  The price is that the epilogues no longer overlap the MMAs; the producer still
-// streams the next tile's first k-blocks into the ring while they run.  Each consumer runs the epilogue of its own 64
-// rows, so the two consumers meet only at the ring's barriers.
+// streams the next tile's first k-blocks into the ring while they run.  Each consumer runs the epilogue tail on its own
+// 64 rows, so the two consumers meet only at the ring's barriers.
 // A stage is 48 KB: three stages and a 128 x (256 + 8) bf16 staging tile take 210 KB of the 227 KB (211 KB with the
 // barriers and the alignment pad); a fourth stage would leave room for only half the staging tile.  W arrives as two
 // 128-row TMA boxes, so both tiles share one W map.
@@ -797,73 +842,24 @@ gemm_wide_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant_
       const int n = n_blk * WIDE_N + col;
       const bool has_bias = p.bias && n < p.N;
       const float2 b2 = has_bias ? unpack_bf16x2(__ldg(reinterpret_cast<const uint32_t*>(p.bias + n))) : make_float2(0.f, 0.f);
-      float x0 = acc[4 * j], x1 = acc[4 * j + 1], x2 = acc[4 * j + 2], x3 = acc[4 * j + 3];
-      if (has_bias) {
-        x0 += b2.x;
-        x1 += b2.y;
-        x2 += b2.x;
-        x3 += b2.y;
-      }
-      uint8_t* s0 = stg + r_lo * WIDE_SROW + col * 2;
-      *reinterpret_cast<uint32_t*>(s0) = pack_bf16x2(x0, x1);
-      *reinterpret_cast<uint32_t*>(s0 + 8 * WIDE_SROW) = pack_bf16x2(x2, x3);
+      stage_bias<WIDE_SROW>(stg + r_lo * WIDE_SROW + col * 2, acc + 4 * j, has_bias, b2);
     }
     named_bar_sync(BAR_EPI + c, 128);
 
+    // 32 threads per row: a warp reads and writes one 512-byte row segment
     const int n_tile0 = n_blk * WIDE_N;
     const long long row_c = (long long)mb * BLOCK_M + 64 * c;   // first row of this consumer's half
-    const __nv_bfloat16* gate_row = p.gate ? p.gate + (long long)bb * p.gate_ld : nullptr;
-    int epi = p.epi;
-    __nv_bfloat16* out_base = p.out + bb * p.out_bs;
-    long long ld = p.ldc;
-    if (epi == B2F_EPI_QKV_NORM_ROPE) {
-      const int which = n_tile0 / p.d_model;   // d_model % 256 == 0: both heads of the tile are in the same block
-      if (which < 2) {
-        // two normalised heads per tile: one thread per (row, head)
-        const int r = tid & 63, h = tid >> 6;
-        const long long row = row_c + r;
-        if (row < p.M)
-          epilogue_head_norm_rope(p, stg + r * WIDE_SROW + h * 256, n_tile0 + 128 * h, row, out_base + row * ld,
-                                  which == 1);
-        continue;
-      }
-      const bool second = p.split_n > 0 && n_tile0 >= p.split_n;
-      epi = second ? p.epi2 : B2F_EPI_BIAS;
-      if (second) {
-        out_base = p.out2 + bb * p.out2_bs - p.split_n;
-        ld = p.ldc2;
-      }
+    const TileOut o = tile_out(p, n_tile0, bb);   // d_model % 256 == 0: both heads of a tile are in the same block
+    if (o.norm >= 0) {
+      // two normalised heads per tile: one thread per (row, head)
+      const int r = tid & 63, h = tid >> 6;
+      const long long row = row_c + r;
+      if (row < p.M)
+        epilogue_head_norm_rope(p, stg + r * WIDE_SROW + h * 256, n_tile0 + 128 * h, row, o.base + row * o.ld,
+                                o.norm == 1);
+      continue;
     }
-    // 32 threads per row, one 8-column group each: a warp reads and writes one 512-byte row segment.  Rows go in batches
-    // of 4 per thread, as in the ping-pong kernel.
-    const int n = n_tile0 + 8 * lane;
-    if (n < p.N) {
-      constexpr int RB = 4;
-      const bool reads_resid = epi == B2F_EPI_GATE_RESID || epi == B2F_EPI_RESID;
-      const uint4 gq = epi == B2F_EPI_GATE_RESID ? __ldg(reinterpret_cast<const uint4*>(gate_row + n))
-                                                 : make_uint4(0, 0, 0, 0);
-#pragma unroll 1
-      for (int rb = w; rb < 64; rb += 4 * RB) {   // staged rows rb + 4 r, r < RB
-        const long long row0 = row_c + rb;
-        if (row0 >= p.M) break;
-        uint4 rq[RB];
-#pragma unroll
-        for (int r = 0; r < RB; ++r) {
-          const long long row = row0 + 4 * r;
-          rq[r] = make_uint4(0, 0, 0, 0);
-          if (reads_resid && row < p.M)
-            rq[r] = *reinterpret_cast<const uint4*>(p.resid + bb * p.resid_bs + row * p.ldr + n);
-        }
-#pragma unroll
-        for (int r = 0; r < RB; ++r) {
-          const long long row = row0 + 4 * r;
-          if (row >= p.M) break;
-          float v[8];
-          unpack_bf16x8(*reinterpret_cast<const uint4*>(stg + (rb + 4 * r) * WIDE_SROW + lane * 16), v);
-          epilogue_group(epi, v, rq[r], gq, out_base + row * ld + n);
-        }
-      }
-    }
+    epilogue_rows<32, 64, WIDE_SROW, false>(p, o, stg, tid, row_c, n_tile0, bb);
   }
 }
 

@@ -250,7 +250,7 @@ __global__ void __launch_bounds__(256) ln_modulate_bwd_kernel(const LnBwdParams 
 }
 
 // ------------------------------------------------------------------------------------------------
-// Backward of per-head RMSNorm + interleaved-pair RoPE (rmsnorm_rope_kernel / the QKV GEMM epilogue):
+// Backward of per-head RMSNorm + interleaved-pair RoPE (rmsnorm_rope_out_kernel / the QKV GEMM epilogue):
 //   fwd: r = rsqrt(mean(x^2) + eps); y = x r w; o = rope(y)
 //   bwd: dy0 = do0 c0 + do1 s1, dy1 = do1 c1 - do0 s0;  dw += dy x r;  g = dy w;
 //        dx = r (g - x r^2 mean(g x))
@@ -344,64 +344,6 @@ __global__ void __launch_bounds__(256) rmsnorm_rope_bwd_kernel(const NormRopeBwd
     for (int wi = 0; wi < 8; ++wi)
       if (set_sm[wi] == set) sum += acc_sm[wi][c];
     p.partial[(long long)blockIdx.x * 512 + i] = sum;
-  }
-}
-
-// out-of-place forward used by the training step (keeps the pre-norm projections for the kernel above)
-struct NormRopeOutParams {
-  const __nv_bfloat16* xq;
-  const __nv_bfloat16* xk;
-  __nv_bfloat16* oq;
-  __nv_bfloat16* ok;
-  long long ldx, x_batch_stride, ldo, o_batch_stride;
-  const __nv_bfloat16 *wq_a, *wk_a, *wq_b, *wk_b;
-  const float* cos;
-  const float* sin;
-  int batch, S, H, n_a;
-  float eps;
-};
-__global__ void __launch_bounds__(256) rmsnorm_rope_out_kernel(const NormRopeOutParams p) {
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const long long tok = (long long)blockIdx.x * 8 + warp;
-  if (tok >= (long long)p.batch * p.S) return;
-  const int b = int(tok / p.S);
-  const int s = int(tok - (long long)b * p.S);
-  const int is_k = lane >> 4;
-  const int l16 = lane & 15;
-  const __nv_bfloat16* xb = (is_k ? p.xk : p.xq) + b * p.x_batch_stride + s * p.ldx + l16 * 8;
-  __nv_bfloat16* ob = (is_k ? p.ok : p.oq) + b * p.o_batch_stride + s * p.ldo + l16 * 8;
-  const bool set_a = s < p.n_a;
-  const __nv_bfloat16* wptr = is_k ? (set_a ? p.wk_a : p.wk_b) : (set_a ? p.wq_a : p.wq_b);
-  float w[8], cs[8], sn[8];
-  unpack8(__ldg(reinterpret_cast<const uint4*>(wptr + l16 * 8)), w);
-  {
-    const float4* c4 = reinterpret_cast<const float4*>(p.cos + (long long)s * 128 + l16 * 8);
-    const float4* s4 = reinterpret_cast<const float4*>(p.sin + (long long)s * 128 + l16 * 8);
-    const float4 c0 = __ldg(c4), c1 = __ldg(c4 + 1), s0 = __ldg(s4), s1 = __ldg(s4 + 1);
-    cs[0] = c0.x; cs[1] = c0.y; cs[2] = c0.z; cs[3] = c0.w;
-    cs[4] = c1.x; cs[5] = c1.y; cs[6] = c1.z; cs[7] = c1.w;
-    sn[0] = s0.x; sn[1] = s0.y; sn[2] = s0.z; sn[3] = s0.w;
-    sn[4] = s1.x; sn[5] = s1.y; sn[6] = s1.z; sn[7] = s1.w;
-  }
-#pragma unroll 4
-  for (int h = 0; h < p.H; ++h) {
-    float x[8];
-    unpack8(*reinterpret_cast<const uint4*>(xb + h * 128), x);
-    float ss = 0.f;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) ss += x[j] * x[j];
-#pragma unroll
-    for (int o = 8; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-    const float r = rsqrtf(ss * (1.0f / 128.0f) + p.eps);
-    float z[8], o8[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) z[j] = bf16r(bf16r(x[j] * r) * w[j]);
-#pragma unroll
-    for (int j = 0; j < 8; j += 2) {
-      o8[j] = z[j] * cs[j] - z[j + 1] * sn[j];
-      o8[j + 1] = z[j + 1] * cs[j + 1] + z[j] * sn[j + 1];
-    }
-    *reinterpret_cast<uint4*>(ob + h * 128) = pack8(o8);
   }
 }
 
@@ -752,33 +694,6 @@ extern "C" int b2f_ln_modulate_bwd(const void* x, int64_t ldx, int64_t x_bs, con
   ln_modulate_bwd_kernel<<<grid, 256, 0, st>>>(p);
   prof_end(KC_LNMOD, st, 0, (dres_in ? 8.0 : 6.0) * batch * rows * D);
   B2F_LAUNCHED("ln_modulate_bwd_kernel", 1);
-  return B2F_OK;
-}
-
-extern "C" int b2f_rmsnorm_rope_out(const void* xq, const void* xk, int64_t ldx, int64_t x_bs, void* oq, void* ok,
-                                    int64_t ldo, int64_t o_bs, const void* wq_a, const void* wk_a, const void* wq_b,
-                                    const void* wk_b, const float* cos, const float* sin, int batch, int S, int H,
-                                    int n_a, float eps, b2f_stream_t stream_) {
-  cudaStream_t st = static_cast<cudaStream_t>(stream_);
-  if (!xq || !xk || !oq || !ok || !wq_b || !wk_b || !cos || !sin || batch <= 0 || S <= 0 || H <= 0) return B2F_ERR_INVALID;
-  if (n_a > 0 && (!wq_a || !wk_a)) return B2F_ERR_INVALID;
-  if ((ldx | x_bs | ldo | o_bs) & 7) return B2F_ERR_ALIGN;
-  NormRopeOutParams p{};
-  p.xq = static_cast<const __nv_bfloat16*>(xq);
-  p.xk = static_cast<const __nv_bfloat16*>(xk);
-  p.oq = static_cast<__nv_bfloat16*>(oq);
-  p.ok = static_cast<__nv_bfloat16*>(ok);
-  p.ldx = ldx; p.x_batch_stride = x_bs; p.ldo = ldo; p.o_batch_stride = o_bs;
-  p.wq_a = static_cast<const __nv_bfloat16*>(n_a > 0 ? wq_a : wq_b);
-  p.wk_a = static_cast<const __nv_bfloat16*>(n_a > 0 ? wk_a : wk_b);
-  p.wq_b = static_cast<const __nv_bfloat16*>(wq_b);
-  p.wk_b = static_cast<const __nv_bfloat16*>(wk_b);
-  p.cos = cos; p.sin = sin; p.batch = batch; p.S = S; p.H = H; p.n_a = n_a; p.eps = eps;
-  const long long tokens = (long long)batch * S;
-  prof_begin(KC_NORMROPE, st);
-  rmsnorm_rope_out_kernel<<<(unsigned)((tokens + 7) / 8), 256, 0, st>>>(p);
-  prof_end(KC_NORMROPE, st, 0, 8.0 * tokens * H * 128);
-  B2F_LAUNCHED("rmsnorm_rope_out_kernel", 1);
   return B2F_OK;
 }
 

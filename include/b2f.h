@@ -646,9 +646,9 @@ int b2f_ln_modulate_bwd(const void* x, int64_t ldx, int64_t x_bs, const void* dy
                         const void* scale, const void* scale_b, int64_t mod_ld, const void* dres_in, int64_t ldr,
                         int64_t r_bs, void* dres_out, int64_t ldo, int64_t o_bs, float* partial, int batch, int rows,
                         int D, float eps, int split_row, int part_row0, b2f_stream_t stream);
-/* b2f_rmsnorm_rope out of place (training keeps the pre-norm projections), and its backward: in place on the Q / K
- * column blocks of the gradient buffer; partial[(batch*S + 7)/8, 512] receives per-block RMSNorm-weight gradient rows
- * [wq_a | wk_a | wq_b | wk_b] (NULL: none). */
+/* b2f_rmsnorm_rope out of place (training keeps the pre-norm projections); the output may alias the input when the
+ * pitches match.  Its backward: in place on the Q / K column blocks of the gradient buffer; partial[(batch*S + 7)/8,
+ * 512] receives per-block RMSNorm-weight gradient rows [wq_a | wk_a | wq_b | wk_b] (NULL: none). */
 int b2f_rmsnorm_rope_out(const void* xq, const void* xk, int64_t ldx, int64_t x_bs, void* oq, void* ok, int64_t ldo,
                          int64_t o_bs, const void* wq_a, const void* wk_a, const void* wq_b, const void* wk_b,
                          const float* cos, const float* sin, int batch, int S, int H, int n_a, float eps,
