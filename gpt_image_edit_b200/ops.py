@@ -69,7 +69,7 @@ def attention(q, k, v, *, out=None, causal: bool = False, scale: float | None = 
     bias [H,Sq,Skv] bf16 (shared by the batch; T5 relative position bias)."""
     for t, n in ((q, "q"), (k, "k"), (v, "v")):
         _req(t, n)
-        if t.dim() != 4 or t.stride(2) != t.shape[3] or (t.shape[0] > 1 and t.stride(0) != t.shape[1] * t.stride(1)):
+        if t.dim() != 4 or t.stride(2) != t.shape[3] or (t.shape[0] > 1 and t.stride(0) != t.shape[1] * _row_pitch(t)):
             raise _lib.B2FError(f"{n}: expected a [B,S,H,dh] view with contiguous heads and batch stride S*ld")
     B, Sq, H, dh = q.shape
     Skv, Hkv = k.shape[1], k.shape[2]
@@ -84,7 +84,7 @@ def attention(q, k, v, *, out=None, causal: bool = False, scale: float | None = 
             raise _lib.B2FError(f"bias: expected [H={H},Sq={Sq},Skv={Skv}] with unit inner stride, got {tuple(bias.shape)}")
         check(
             _lib.lib.b2f_attention_bias_fwd(
-                ptr(q), q.stride(1), ptr(k), k.stride(1), ptr(v), v.stride(1), ptr(out), out.stride(1),
+                ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v), ptr(out), _row_pitch(out),
                 B, H, Hkv, Sq, Skv, dh, float(scale), int(causal), ptr(bias), bias.stride(0), bias.stride(1), stream_ptr(),
             ),
             "b2f_attention_bias_fwd",
@@ -92,7 +92,7 @@ def attention(q, k, v, *, out=None, causal: bool = False, scale: float | None = 
         return out
     check(
         _lib.lib.b2f_attention_fwd(
-            ptr(q), q.stride(1), ptr(k), k.stride(1), ptr(v), v.stride(1), ptr(out), out.stride(1),
+            ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v), ptr(out), _row_pitch(out),
             B, H, Hkv, Sq, Skv, dh, float(scale), int(causal), stream_ptr(),
         ),
         "b2f_attention_fwd",
@@ -598,9 +598,10 @@ def linear_qkv_norm_rope_fp8_lora(xq, x_scale, wq, w_scale, bias, nq, nk, cos, s
 
 
 def _row_pitch(t: torch.Tensor) -> int:
-    """Token pitch of a [B,S,H,dh] view; with S = 1 the stride of that dimension is arbitrary and the batch pitch is it."""
+    """Token pitch of a [B,S,H,dh] (or [B,S,n]) view; with S = 1 the stride of that dimension is arbitrary and the batch
+    pitch is it."""
     B, S = t.shape[:2]
-    return t.stride(1) if S > 1 else t.stride(0) if B > 1 else t.shape[2] * t.shape[3]
+    return t.stride(1) if S > 1 else t.stride(0) if B > 1 else t[0, 0].numel()
 
 
 def _qkv_views(q, k, v):

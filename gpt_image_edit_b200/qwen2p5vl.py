@@ -149,7 +149,12 @@ def padding_spans(attention_mask):
 
 class B200Qwen2p5VL(torch.nn.Module):
     """Weights in kernel layout + the prefill forward.  `denoise_projector` (MLP2) is owned by the
-    denoise tower (univa.models.modeling_univa_denoise_tower)."""
+    denoise tower (univa.models.modeling_univa_denoise_tower).
+
+    The loops of `forward_visual`, `_decoder` and `generate` call their stages (`_vision_embed`, `_vision_block`,
+    `_vision_merge`, `_attn_buffer`, `_decoder_layer`, `_decode_step`) through the class, not through `self`: the
+    host-orchestration tests run these loops on a stand-in object that carries only the loops themselves, and a test can
+    drive one stage at a time through the same functions."""
 
     HP = 128  # head slot pitch (vision head_dim 80 is zero-padded to 128)
 
@@ -336,6 +341,14 @@ class B200Qwen2p5VL(torch.nn.Module):
     def forward_visual(self, pixel_values: torch.Tensor, grid_thw) -> torch.Tensor:
         """pixel_values [T, C*2*14*14] (processor order), grid_thw [[t,h,w]] -> merged image embeds
         [T/4, out_hidden] in the original (un-windowed) token order."""
+        x, ctx = B200Qwen2p5VL._vision_embed(self, pixel_values, grid_thw)
+        for i in range(self.vc.depth):
+            B200Qwen2p5VL._vision_block(self, i, x, ctx)
+        return B200Qwen2p5VL._vision_merge(self, x, ctx)
+
+    def _vision_embed(self, pixel_values, grid_thw):
+        """Patch embed, 2-D RoPE tables and the window gather -> (x [T, hidden] in window order, context of the blocks:
+        cos / sin, window_index, the window and full-attention cu_seqlens, the attention output buffer)."""
         vc, W, HP = self.vc, self.W, self.HP
         grid = [tuple(int(v) for v in g) for g in (grid_thw.tolist() if torch.is_tensor(grid_thw) else grid_thw)]
         T = pixel_values.shape[0]
@@ -358,26 +371,41 @@ class B200Qwen2p5VL(torch.nn.Module):
         for t, h, w in grid:
             for _ in range(t):
                 cu_full.append(cu_full[-1] + h * w)
+        attn_out = torch.empty((T, vc.num_heads * HP), device=self._dev, dtype=torch.bfloat16)
+        return x, SimpleNamespace(cos=cos, sin=sin, window_index=widx, cu_win=cu_win, cu_full=cu_full, attn_out=attn_out)
+
+    def _vision_block(self, i, x, ctx, keep=None):
+        """ViT block i on x [T, hidden] (window order), updated in place.  `keep` (a dict) receives views of the buffers
+        the block leaves behind: `qkv` after RoPE, `attn_out` and the SwiGLU output `a`."""
+        vc, W, HP = self.vc, self.W, self.HP
         nh = vc.num_heads
         HPv = nh * HP
-        scale = self.vhd ** -0.5
-        attn_out = torch.empty((T, HPv), device=self._dev, dtype=torch.bfloat16)
-        for i in range(vc.depth):
-            p = f"visual.blocks.{i}."
-            xn = ops.rmsnorm(x, W[p + "norm1"])
-            qkv = ops.linear(xn, W[p + "qkv.w"], W[p + "qkv.b"])
-            ops.rope_half_(qkv, 2 * nh, HP, cos, sin, fp32_math=True)         # q heads then k heads
-            cu = cu_full if i in vc.fullatt_block_indexes else cu_win
-            self._segment_attention(qkv, attn_out, cu, nh, nh, HPv, HPv, scale, causal=False)
-            ops.linear(attn_out, W[p + "proj.w"], W[p + "proj.b"], epilogue=ops.EPI_RESID, resid=x, out=x)
-            xn = ops.rmsnorm(x, W[p + "norm2"])
-            gu = ops.linear(xn, W[p + "gu.w"], W[p + "gu.b"])
-            a = ops.swiglu(gu, self.vi)
-            ops.linear(a, W[p + "down.w"], W[p + "down.b"], epilogue=ops.EPI_RESID, resid=x, out=x)
-        xn = ops.rmsnorm(x, W["visual.merger.ln_q"]).view(T // unit, unit * vc.hidden_size)
+        p = f"visual.blocks.{i}."
+        xn = ops.rmsnorm(x, W[p + "norm1"])
+        qkv = ops.linear(xn, W[p + "qkv.w"], W[p + "qkv.b"])
+        ops.rope_half_(qkv, 2 * nh, HP, ctx.cos, ctx.sin, fp32_math=True)     # q heads then k heads
+        cu = ctx.cu_full if i in vc.fullatt_block_indexes else ctx.cu_win
+        self._segment_attention(qkv, ctx.attn_out, cu, nh, nh, HPv, HPv, self.vhd ** -0.5, causal=False)
+        ops.linear(ctx.attn_out, W[p + "proj.w"], W[p + "proj.b"], epilogue=ops.EPI_RESID, resid=x, out=x)
+        xn = ops.rmsnorm(x, W[p + "norm2"])
+        gu = ops.linear(xn, W[p + "gu.w"], W[p + "gu.b"])
+        a = ops.swiglu(gu, self.vi)
+        ops.linear(a, W[p + "down.w"], W[p + "down.b"], epilogue=ops.EPI_RESID, resid=x, out=x)
+        if keep is not None:
+            keep.update(qkv=qkv, attn_out=ctx.attn_out, a=a)
+        return x
+
+    def _vision_merge(self, x, ctx, keep=None):
+        """The patch merger (ln_q, 2x2 concat, Linear · erf-GELU · Linear) and the un-windowing gather -> [T/4, out_hidden];
+        `keep` receives the merger output in window order as `merged`."""
+        vc, W = self.vc, self.W
+        unit = vc.spatial_merge_size ** 2
+        xn = ops.rmsnorm(x, W["visual.merger.ln_q"]).view(x.shape[0] // unit, unit * vc.hidden_size)
         h = ops.linear(xn, W["visual.merger.0.w"], W["visual.merger.0.b"], epilogue=ops.EPI_GELU_ERF)
         merged = ops.linear(h, W["visual.merger.2.w"], W["visual.merger.2.b"])
-        return ops.gather_rows(merged, torch.argsort(widx).to(self._dev))
+        if keep is not None:
+            keep.update(merged=merged)
+        return ops.gather_rows(merged, torch.argsort(ctx.window_index).to(self._dev))
 
     def _segment_attention(self, qkv, out, cu, H, Hkv, k_off, v_off_rel, scale, causal):
         """Block-diagonal attention over contiguous token segments cu[i]:cu[i+1]; runs of equal-length
@@ -422,43 +450,59 @@ class B200Qwen2p5VL(torch.nn.Module):
         own tokens only and the padding rows get a zero attention output — what transformers' flash_attention_2
         path does (unpad -> varlen attention -> pad_input), the backend the reference selects (cli.py:40,
         train_denoiser.py:1633)."""
-        tc, W, hd = self.tc, self.W, self.thd
-        nq, nkv = tc.num_attention_heads, tc.num_key_value_heads
-        # padded prefill: the rows no launch writes must read as zeros in every layer
-        o = (torch.zeros if (spans is not None and not past) else torch.empty)((B * L, nq * hd), device=self._dev, dtype=torch.bfloat16)
+        tc = self.tc
         if past and L != 1:
             raise _lib.B2FError("chunked prefill is not implemented: use past == 0 (prefill) or one new token (decode)")
+        o = B200Qwen2p5VL._attn_buffer(self, B, L, past, spans)
         for i in range(tc.num_hidden_layers):
-            p = f"model.layers.{i}."
-            xn = ops.rmsnorm(x, W[p + "ln1"], eps=tc.rms_norm_eps)
-            qkv = ops.linear(xn, W[p + "qkv.w"], W[p + "qkv.b"])
-            ops.rope_half_(qkv, nq + nkv, hd, cos, sin, fp32_math=False)
-            q = qkv[:, : nq * hd].unflatten(1, (nq, hd)).unflatten(0, (B, L))
-            k = qkv[:, nq * hd: (nq + nkv) * hd].unflatten(1, (nkv, hd)).unflatten(0, (B, L))
-            v = qkv[:, (nq + nkv) * hd:].unflatten(1, (nkv, hd)).unflatten(0, (B, L))
-            if kv_cache is not None:
-                kv_cache[i, 0, :, past:past + L].copy_(k)
-                kv_cache[i, 1, :, past:past + L].copy_(v)
-            if past:
-                # decode: the new token attends to every cached position of its own sequence (no mask needed: a left-padded
-                # prompt's padding slots lie before `lo`); one launch per sequence because the cache's batch pitch (Lmax
-                # rows) differs from the attended length
-                for b in range(B):
-                    lo = spans[b][0] if spans is not None else 0
-                    ops.attention(q[b:b + 1], kv_cache[i, 0, b:b + 1, lo:past + 1], kv_cache[i, 1, b:b + 1, lo:past + 1],
-                                  out=o.unflatten(0, (B, L))[b:b + 1])
-            elif spans is not None:                      # padded prefill
-                o3 = o.unflatten(0, (B, L))
-                for b, (lo, hi) in enumerate(spans):
-                    ops.attention(q[b:b + 1, lo:hi], k[b:b + 1, lo:hi], v[b:b + 1, lo:hi], out=o3[b:b + 1, lo:hi], causal=True)
-            else:
-                ops.attention(q, k, v, out=o.unflatten(0, (B, L)), causal=True)
-            ops.linear(o, W[p + "o.w"], None, epilogue=ops.EPI_RESID, resid=x, out=x)
-            xn = ops.rmsnorm(x, W[p + "ln2"], eps=tc.rms_norm_eps)
-            gu = ops.linear(xn, W[p + "gu.w"])
-            a = ops.swiglu(gu, tc.intermediate_size)
-            ops.linear(a, W[p + "down.w"], None, epilogue=ops.EPI_RESID, resid=x, out=x)
-        return ops.rmsnorm(x, W["model.norm"], eps=tc.rms_norm_eps)
+            B200Qwen2p5VL._decoder_layer(self, i, x, o, cos, sin, B, L, kv_cache, past, spans)
+        return ops.rmsnorm(x, self.W["model.norm"], eps=tc.rms_norm_eps)
+
+    def _attn_buffer(self, B, L, past=0, spans=None):
+        """The decoder's attention output [B*L, heads * head_dim], shared by its layers.  In a padded prefill the rows no
+        launch writes must read as zeros in every layer."""
+        n = self.tc.num_attention_heads * self.thd
+        return (torch.zeros if (spans is not None and not past) else torch.empty)((B * L, n), device=self._dev,
+                                                                                    dtype=torch.bfloat16)
+
+    def _decoder_layer(self, i, x, o, cos, sin, B, L, kv_cache=None, past: int = 0, spans=None, keep=None):
+        """Decoder layer i on x [B*L, hidden], updated in place; `o` is `_attn_buffer`'s, the rest as in `_decoder`.
+        `keep` (a dict) receives views of the buffers the layer leaves behind: `qkv` after RoPE, `attn_out` and the
+        SwiGLU output `a`."""
+        tc, W, hd = self.tc, self.W, self.thd
+        nq, nkv = tc.num_attention_heads, tc.num_key_value_heads
+        p = f"model.layers.{i}."
+        xn = ops.rmsnorm(x, W[p + "ln1"], eps=tc.rms_norm_eps)
+        qkv = ops.linear(xn, W[p + "qkv.w"], W[p + "qkv.b"])
+        ops.rope_half_(qkv, nq + nkv, hd, cos, sin, fp32_math=False)
+        q = qkv[:, : nq * hd].unflatten(1, (nq, hd)).unflatten(0, (B, L))
+        k = qkv[:, nq * hd: (nq + nkv) * hd].unflatten(1, (nkv, hd)).unflatten(0, (B, L))
+        v = qkv[:, (nq + nkv) * hd:].unflatten(1, (nkv, hd)).unflatten(0, (B, L))
+        if kv_cache is not None:
+            kv_cache[i, 0, :, past:past + L].copy_(k)
+            kv_cache[i, 1, :, past:past + L].copy_(v)
+        if past:
+            # decode: the new token attends to every cached position of its own sequence (no mask needed: a left-padded
+            # prompt's padding slots lie before `lo`); one launch per sequence because the cache's batch pitch (Lmax
+            # rows) differs from the attended length
+            for b in range(B):
+                lo = spans[b][0] if spans is not None else 0
+                ops.attention(q[b:b + 1], kv_cache[i, 0, b:b + 1, lo:past + 1], kv_cache[i, 1, b:b + 1, lo:past + 1],
+                              out=o.unflatten(0, (B, L))[b:b + 1])
+        elif spans is not None:                      # padded prefill
+            o3 = o.unflatten(0, (B, L))
+            for b, (lo, hi) in enumerate(spans):
+                ops.attention(q[b:b + 1, lo:hi], k[b:b + 1, lo:hi], v[b:b + 1, lo:hi], out=o3[b:b + 1, lo:hi], causal=True)
+        else:
+            ops.attention(q, k, v, out=o.unflatten(0, (B, L)), causal=True)
+        ops.linear(o, W[p + "o.w"], None, epilogue=ops.EPI_RESID, resid=x, out=x)
+        xn = ops.rmsnorm(x, W[p + "ln2"], eps=tc.rms_norm_eps)
+        gu = ops.linear(xn, W[p + "gu.w"])
+        a = ops.swiglu(gu, tc.intermediate_size)
+        ops.linear(a, W[p + "down.w"], None, epilogue=ops.EPI_RESID, resid=x, out=x)
+        if keep is not None:
+            keep.update(qkv=qkv, attn_out=o, a=a)
+        return x
 
     def lm_logits(self, hidden):
         """lm_head on [n, hidden] -> [n, vocab] bf16 (wgmma GEMM; vocab rows stream once from HBM)."""
@@ -505,13 +549,18 @@ class B200Qwen2p5VL(torch.nn.Module):
                 break
             if t == steps - 1:
                 break
-            # text continues on all three M-RoPE axes at (past length + delta)
-            pos = (torch.full((B, 1), L + t, dtype=torch.long) + deltas.cpu().view(B, 1))[None].expand(3, B, 1)
-            cos, sin = self._rope_tables(pos)
-            x = ops.gather_rows(self.W["model.embed_tokens"], nxt.contiguous())
-            last = self._decoder(x, cos, sin, B, 1, cache, past=L + t, spans=spans)
+            last = B200Qwen2p5VL._decode_step(self, nxt, cache, L + t, deltas, spans)
         seq = torch.cat(out, dim=1)
         return (seq, scores) if output_scores else seq
+
+    def _decode_step(self, nxt, cache, past, deltas, spans=None):
+        """One step of `generate`: the tokens nxt [B] at cache row `past` through every layer -> final-norm hidden [B, hidden]."""
+        B = nxt.shape[0]
+        # text continues on all three M-RoPE axes at (past length + delta)
+        pos = (torch.full((B, 1), past, dtype=torch.long) + deltas.cpu().view(B, 1))[None].expand(3, B, 1)
+        cos, sin = self._rope_tables(pos)
+        x = ops.gather_rows(self.W["model.embed_tokens"], nxt.contiguous())
+        return self._decoder(x, cos, sin, B, 1, cache, past=past, spans=spans)
 
     @torch.no_grad()
     def forward(self, input_ids: torch.Tensor, pixel_values=None, attention_mask=None, image_grid_thw=None,
