@@ -10,6 +10,9 @@
 // The two consumer warpgroups run independently, so one warpgroup's softmax overlaps the other's MMAs.
 // Causal calls (Sq == Skv) stop streaming at the tile's last query row; GQA maps head h to K/V head h / (H / Hkv);
 // the BIAS kernel adds a bf16 score bias (T5 relative positions) before the softmax.
+// The WIN kernel (b2f_attention_fwd_window) gives every batch item a text window: keys [lo, hi) of the first S_txt
+// and every key from S_txt on are valid, the rest are never loaded or, in a block that straddles them, get p = 0 and
+// zeroed V rows.
 //
 // Replaces F.scaled_dot_product_attention as reached by diffusers FluxAttnProcessor2_0
 // (SURVEY.md A.2; reference call site univa/utils/flux_pipeline.py:1067) and flash_attn as reached
@@ -26,7 +29,12 @@ namespace {
 
 // BIAS: additive bf16 score bias; the bias kernel folds the score scale into the bias step and runs with
 // scale_log2 = log2(e).
-template <bool BIAS>
+// WIN: per-item text window p.win[b] = (lo, hi) over the first p.S_txt keys (non-causal, no bias).  The K/V blocks
+// start at lo instead of 0: one run of blocks over [lo, end0) and, when the window stops short of the image rows
+// (hi < S_txt), a second run over [S_txt, Skv).  With end0 = Skv for hi == S_txt (left-padded text, the full window)
+// there is one run and no pad row is ever loaded; the full window (0, S_txt) streams exactly the blocks of the kernel
+// without WIN.
+template <bool BIAS, bool WIN>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
@@ -50,7 +58,17 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   // K/V blocks this CTA needs (causal: only up to its last query row; Sq == Skv then)
   int kv_len = p.Skv;
   if (p.causal) kv_len = min(p.Skv, q0 + BQ);
-  const int n_kv = (kv_len + BKV - 1) / BKV;
+  int n_kv = (kv_len + BKV - 1) / BKV;
+  // WIN: block j < n0 covers keys [lo + j BKV, ..) of the run ending at end0, block j >= n0 [S_txt + (j - n0) BKV, ..)
+  int lo = 0, hi = 0, end0 = 0, n0 = 0;
+  if (WIN) {
+    lo = min(max(p.win[2 * b], 0), p.S_txt);   // out-of-range windows are clamped, never read out of bounds
+    hi = min(max(p.win[2 * b + 1], lo), p.S_txt);
+    end0 = hi == p.S_txt ? p.Skv : hi;
+    n0 = (end0 - lo + BKV - 1) / BKV;
+    n_kv = n0 + (hi == p.S_txt ? 0 : (p.Skv - p.S_txt + BKV - 1) / BKV);
+  }
+  auto kv_start = [&](int j) { return !WIN ? j * BKV : j < n0 ? lo + j * BKV : p.S_txt + (j - n0) * BKV; };
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
@@ -80,11 +98,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         mbar_wait(&k_empty[slot], phase ^ 1);
         mbar_expect_tx(&k_full[slot], TILE_BYTES);
         for (int half = 0; half < 2; ++half)
-          tma_load_3d(k_smem + slot * TILE_BYTES + half * HALF_BYTES, &tmK, &k_full[slot], hk * DH + half * 64, j * BKV, b);
+          tma_load_3d(k_smem + slot * TILE_BYTES + half * HALF_BYTES, &tmK, &k_full[slot], hk * DH + half * 64,
+                      kv_start(j), b);
         mbar_wait(&v_empty[slot], phase ^ 1);
         mbar_expect_tx(&v_full[slot], TILE_BYTES);
         for (int half = 0; half < 2; ++half)
-          tma_load_3d(v_smem + slot * TILE_BYTES + half * HALF_BYTES, &tmV, &v_full[slot], hk * DH + half * 64, j * BKV, b);
+          tma_load_3d(v_smem + slot * TILE_BYTES + half * HALF_BYTES, &tmV, &v_full[slot], hk * DH + half * 64,
+                      kv_start(j), b);
       }
     }
     return;
@@ -121,7 +141,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     __syncwarp();
     if (lane == 0) mbar_arrive(&k_empty[slot]);
 
-    const int kv0 = j * BKV;
+    const int kv0 = kv_start(j);
     if (BIAS) {
 #pragma unroll
       for (int i = 0; i < 64; ++i) {
@@ -132,7 +152,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
                       __bfloat162float(p.bias[(long long)h * p.bias_h_stride + (long long)row * p.bias_row_stride + col]));
       }
     }
-    if (kv0 + BKV > p.Skv || p.causal) {
+    if (WIN) {
+      const int kv_end = j < n0 ? end0 : p.Skv;   // keys [kv_end, kv0 + BKV) of this block are masked
+      if (kv0 + BKV > kv_end) {
+#pragma unroll
+        for (int i = 0; i < 64; ++i)
+          if (kv0 + 8 * (i >> 2) + colq + (i & 1) >= kv_end) s[i] = -INFINITY;
+      }
+    } else if (kv0 + BKV > p.Skv || p.causal) {
 #pragma unroll
       for (int i = 0; i < 64; ++i) {
         const int row = row0 + 8 * ((i >> 1) & 1);
@@ -169,6 +196,19 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     uint32_t pa[BKV / 16][4];
 #pragma unroll
     for (int kk = 0; kk < BKV / 16; ++kk) pack_a_frag(s, kk, pa[kk]);
+    if (WIN && j == n0 - 1 && hi < p.S_txt && hi - kv0 < BKV) {
+      // The last block of the text run holds pad rows [hi, S_txt) (any content, NaN included): p = 0 there, but
+      // 0 * NaN is NaN in P.V, so both consumer warpgroups zero those V rows (all 128 channels, whole 128-byte rows
+      // of both swizzled halves) before either multiplies.  Rows from S_txt on are image rows (finite) and rows past
+      // Skv arrive as TMA zero fill.
+      const int z0 = hi - kv0, z1 = min(p.S_txt - kv0, BKV);
+      mbar_wait(&v_full[slot], phase);
+      uint8_t* vt = v_smem + slot * TILE_BYTES;
+      for (int i = z0 * 16 + (int(threadIdx.x) - 128); i < z1 * 16; i += 256)
+        *reinterpret_cast<uint4*>(vt + (i & 8) / 8 * HALF_BYTES + (i >> 4) * 128 + (i & 7) * 16) = make_uint4(0, 0, 0, 0);
+      fence_proxy_async_smem();
+      named_bar_sync(1, 256);
+    }
     mbar_wait(&v_full[slot], phase);
     reg_fence(o);
     wgmma_fence();
@@ -204,7 +244,8 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
 static int attention_impl(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
                           int64_t ldv, void* out, int64_t ldo, int B, int H, int Hkv, int Sq, int Skv,
                           int head_dim, float scale, int causal, const void* bias, int64_t bias_h_stride,
-                          int64_t bias_row_stride, float* lse, int64_t lse_stride, cudaStream_t stream) {
+                          int64_t bias_row_stride, float* lse, int64_t lse_stride, const int32_t* win, int S_txt,
+                          cudaStream_t stream) {
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (lse && lse_stride < Sq) return B2F_ERR_INVALID;
   if (!q || !k || !v || !out || B <= 0 || H <= 0 || Hkv <= 0 || Sq <= 0 || Skv <= 0)
@@ -218,9 +259,12 @@ static int attention_impl(const void* q, int64_t ldq, const void* k, int64_t ldk
     return B2F_ERR_ALIGN;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         ATTN_SMEM);
     if (e != cudaSuccess) return cuda_err(e, "attention smem attribute");
-    e = cudaFuncSetAttribute(attn_fwd_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM);
+    e = cudaFuncSetAttribute(attn_fwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM);
+    if (e != cudaSuccess) return cuda_err(e, "attention smem attribute");
+    e = cudaFuncSetAttribute(attn_fwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM);
     if (e != cudaSuccess) return cuda_err(e, "attention smem attribute");
     attr_set = true;
   }
@@ -252,15 +296,25 @@ static int attention_impl(const void* q, int64_t ldq, const void* k, int64_t ldk
     p.scale_log2 = 1.4426950408889634f;
     dim3 grid_b((Sq + BQ - 1) / BQ, H, B);
     prof_begin(KC_ATTN, stream);
-    attn_fwd_kernel<true><<<grid_b, ATTN_THREADS, ATTN_SMEM, stream>>>(tmQ, tmK, tmV, p);
+    attn_fwd_kernel<true, false><<<grid_b, ATTN_THREADS, ATTN_SMEM, stream>>>(tmQ, tmK, tmV, p);
     prof_end(KC_ATTN, stream, (causal ? 2.0 : 4.0) * B * H * (double)Sq * Skv * DH,
              2.0 * DH * B * (2.0 * H * Sq + 2.0 * Hkv * Skv) + 2.0 * H * (double)Sq * Skv);
     B2F_LAUNCHED("attn_fwd_kernel<bias>", 1);
     return B2F_OK;
   }
   dim3 grid((Sq + BQ - 1) / BQ, H, B);
+  if (win) {
+    p.win = win;
+    p.S_txt = S_txt;
+    prof_begin(KC_ATTN, stream);
+    attn_fwd_kernel<false, true><<<grid, ATTN_THREADS, ATTN_SMEM, stream>>>(tmQ, tmK, tmV, p);
+    // the full-window bound: blocks outside the windows are skipped
+    prof_end(KC_ATTN, stream, 4.0 * B * H * (double)Sq * Skv * DH, 2.0 * DH * B * (2.0 * H * Sq + 2.0 * Hkv * Skv));
+    B2F_LAUNCHED("attn_fwd_kernel<window>", 1);
+    return B2F_OK;
+  }
   prof_begin(KC_ATTN, stream);
-  attn_fwd_kernel<false><<<grid, ATTN_THREADS, ATTN_SMEM, stream>>>(tmQ, tmK, tmV, p);
+  attn_fwd_kernel<false, false><<<grid, ATTN_THREADS, ATTN_SMEM, stream>>>(tmQ, tmK, tmV, p);
   prof_end(KC_ATTN, stream, (causal ? 2.0 : 4.0) * B * H * (double)Sq * Skv * DH,
            2.0 * DH * B * (2.0 * H * Sq + 2.0 * Hkv * Skv));
   B2F_LAUNCHED("attn_fwd_kernel", 1);
@@ -272,7 +326,17 @@ extern "C" int b2f_attention_fwd(const void* q, int64_t ldq, const void* k, int6
                                  float scale, int causal, b2f_stream_t stream_) {
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   return attention_impl(q, ldq, k, ldk, v, ldv, out, ldo, B, H, Hkv, Sq, Skv, head_dim, scale, causal,
-                        nullptr, 0, 0, nullptr, 0, stream);
+                        nullptr, 0, 0, nullptr, 0, nullptr, 0, stream);
+}
+
+extern "C" int b2f_attention_fwd_window(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                                        int64_t ldv, void* out, int64_t ldo, int B, int H, int Hkv, int Sq, int Skv,
+                                        int head_dim, float scale, const int32_t* win, int S_txt,
+                                        b2f_stream_t stream_) {
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  if (!win || S_txt < 0 || S_txt > Skv) return B2F_ERR_INVALID;
+  return attention_impl(q, ldq, k, ldk, v, ldv, out, ldo, B, H, Hkv, Sq, Skv, head_dim, scale, 0, nullptr, 0, 0,
+                        nullptr, 0, win, S_txt, stream);
 }
 
 // forward that also emits the base-2 log-sum-exp rows the backward kernels need (attention_bwd.cu)
@@ -282,7 +346,7 @@ extern "C" int b2f_attention_fwd_lse(const void* q, int64_t ldq, const void* k, 
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!lse) return B2F_ERR_INVALID;
   return attention_impl(q, ldq, k, ldk, v, ldv, out, ldo, B, H, Hkv, Sq, Skv, head_dim, scale, causal, nullptr, 0, 0,
-                        lse, lse_stride, stream);
+                        lse, lse_stride, nullptr, 0, stream);
 }
 
 extern "C" int b2f_attention_bias_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
@@ -292,7 +356,7 @@ extern "C" int b2f_attention_bias_fwd(const void* q, int64_t ldq, const void* k,
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   if (!bias || bias_row_stride < Skv || bias_h_stride < 0) return B2F_ERR_INVALID;
   return attention_impl(q, ldq, k, ldk, v, ldv, out, ldo, B, H, Hkv, Sq, Skv, head_dim, scale, causal,
-                        bias, bias_h_stride, bias_row_stride, nullptr, 0, stream);
+                        bias, bias_h_stride, bias_row_stride, nullptr, 0, nullptr, 0, stream);
 }
 
 }  // namespace b2f

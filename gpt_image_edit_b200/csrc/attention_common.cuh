@@ -30,6 +30,9 @@ struct AttnParams {
   // are scale_log2 * q.k; element (b, h, q) at lse + (b*H + h)*lse_stride + q
   float* lse;
   long long lse_stride;
+  // per-item text window (WIN kernel only): int32 [B, 2] (lo, hi) on the device; keys k < S_txt valid iff lo <= k < hi
+  const int32_t* win;
+  int S_txt;
 };
 
 static __device__ __forceinline__ float ex2(float x) {

@@ -12,6 +12,10 @@
 // tokens through two slots, two consumer warpgroups own 64 query rows each.  V8t is K-major for the P.V product (FP8
 // wgmma takes no MN-major operand), and its token order within every 32-token group makes the m64n128 accumulator
 // layout of S the register A fragment of the k32 P.V wgmma, so P converts in place without shuffles.
+//
+// With a per-item text window (b2f_attn_quant_fp8_window / b2f_attention_fp8_window) the quantizer takes its amaxes
+// over the valid tokens only and writes masked tokens as +0 in q8, k8 and v8t; the attention kernel skips the 128-token
+// blocks that hold no valid key and masks the scores of the others, so p = 0 meets V = +0 there.
 #include <cmath>
 
 #include "attention_common.cuh"
@@ -40,7 +44,16 @@ struct QuantAttnParams {
   uint8_t *q8, *k8, *v8t;
   float *sq, *sk, *sv;
   int H, S, S_pad;
+  // optional per-item text window int32 [B, 2] (lo, hi): token t < S_txt is valid iff lo <= t < hi
+  const int32_t* win;
+  int S_txt;
 };
+
+// The text window of item b, clamped to [0, S_txt] so that out-of-range values never index out of bounds.
+__device__ __forceinline__ int2 text_window(const int32_t* win, int b, int S_txt) {
+  const int lo = min(max(win[2 * b], 0), S_txt);
+  return make_int2(lo, min(max(win[2 * b + 1], lo), S_txt));
+}
 
 // Thread t of a 256-thread CTA covers channels 8 (t % 16) .. + 7 of tokens t / 16 + 16 i (i < 8) of the CTA's block.
 __device__ __forceinline__ const __nv_bfloat16* head_row(const __nv_bfloat16* x, long long ld, int b, int S, int tok,
@@ -55,10 +68,12 @@ __global__ void __launch_bounds__(256) attn_amax_kernel(const QuantAttnParams p)
   const int h = blockIdx.y, b = blockIdx.z, t = threadIdx.x;
   const int cc = t & 15, r0 = t >> 4, warp = t >> 5;
   float mq = 0.f, mk = 0.f, mv[8] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
+  const int2 tw = p.win ? text_window(p.win, b, p.S_txt) : make_int2(0, 0);
 #pragma unroll 4
   for (int i = 0; i < QTOK / 16; ++i) {
     const int tok = blockIdx.x * QTOK + r0 + 16 * i;
     if (tok >= p.S) break;
+    if (p.win && tok < p.S_txt && (tok < tw.x || tok >= tw.y)) continue;   // masked text token
     mq = amax8(*reinterpret_cast<const uint4*>(head_row(p.q, p.ldq, b, p.S, tok, h) + 8 * cc), mq);
     mk = amax8(*reinterpret_cast<const uint4*>(head_row(p.k, p.ldk, b, p.S, tok, h) + 8 * cc), mk);
     const uint4 vv = *reinterpret_cast<const uint4*>(head_row(p.v, p.ldv, b, p.S, tok, h) + 8 * cc);
@@ -117,14 +132,21 @@ __global__ void __launch_bounds__(256) attn_quant_kernel(const QuantAttnParams p
   row_scale_of(p.sk[bh], s_, inv_k);
 #pragma unroll
   for (int j = 0; j < 8; ++j) row_scale_of(p.sv[bh * DH + 8 * cc + j], s_, inv_v[j]);
+  const int2 tw = p.win ? text_window(p.win, b, p.S_txt) : make_int2(0, 0);
 #pragma unroll 2
   for (int i = 0; i < QTOK / 16; ++i) {
     const int tl = r0 + 16 * i;
     const int tok = blockIdx.x * QTOK + tl;
     const int pos = (tl & ~31) + v8t_pos(tl & 31);
-    if (tok >= p.S) {   // padding tokens of v8t are +0
+    const bool masked = p.win && tok < p.S_txt && (tok < tw.x || tok >= tw.y);
+    if (tok >= p.S || masked) {   // padding and masked tokens of v8t are +0 (and masked ones of q8 / k8 too)
 #pragma unroll
       for (int j = 0; j < 8; ++j) vt[vt_off(8 * cc + j, pos)] = 0;
+      if (masked) {
+        const long long o8 = (((long long)b * p.S + tok) * p.H + h) * DH + 8 * cc;
+        *reinterpret_cast<uint2*>(p.q8 + o8) = make_uint2(0, 0);
+        *reinterpret_cast<uint2*>(p.k8 + o8) = make_uint2(0, 0);
+      }
       continue;
     }
     const long long o8 = (((long long)b * p.S + tok) * p.H + h) * DH + 8 * cc;
@@ -186,8 +208,15 @@ struct AttnFp8Params {
   float scale_log2;
   __nv_bfloat16* out;
   long long ldo;
+  const int32_t* win;   // WIN kernel: per-item text window over the first S_txt tokens
+  int S_txt;
 };
 
+// WIN: the kernel streams the 128-token blocks [lo / BKV, ceil(hi / BKV)) of the text window and then the blocks from
+// max(that end, S_txt / BKV) on, at the block positions of the kernel without WIN (v8t's token order lives in 32-token
+// groups from token 0, so blocks cannot start at lo); blocks that are not wholly valid mask their invalid scores.  The
+// full window (0, S_txt) streams every block and masks exactly the tail the kernel without WIN masks.
+template <bool WIN>
 __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnFp8Params p) {
@@ -207,7 +236,16 @@ attn_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   const int wg = __shfl_sync(0xffffffffu, int(threadIdx.x >> 7), 0);
   const int h = blockIdx.y, b = blockIdx.z;
   const int q0 = blockIdx.x * BQ;
-  const int n_kv = (p.S + BKV - 1) / BKV;
+  int n_kv = (p.S + BKV - 1) / BKV;
+  int2 tw = make_int2(0, 0);
+  int n_txt = 0, j_img = 0;   // WIN: blocks [lo / BKV, + n_txt), then [j_img, n_kv) of the unwindowed numbering
+  if (WIN) {
+    tw = text_window(p.win, b, p.S_txt);
+    n_txt = tw.y > tw.x ? (tw.y + BKV - 1) / BKV - tw.x / BKV : 0;
+    j_img = max(tw.x / BKV + n_txt, p.S_txt / BKV);
+    n_kv = n_txt + max(n_kv - j_img, 0);
+  }
+  auto kv_block = [&](int j) { return !WIN ? j : j < n_txt ? tw.x / BKV + j : j_img + (j - n_txt); };
 
   if (threadIdx.x == 0) {
     tma_prefetch_desc(&tmQ);
@@ -235,10 +273,10 @@ attn_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
         const uint32_t phase = (j / F8_SLOTS) & 1;
         mbar_wait(&k_empty[slot], phase ^ 1);
         mbar_expect_tx(&k_full[slot], F8_TILE);
-        tma_load_3d(k_smem + slot * F8_TILE, &tmK, &k_full[slot], h * DH, j * BKV, b);
+        tma_load_3d(k_smem + slot * F8_TILE, &tmK, &k_full[slot], h * DH, kv_block(j) * BKV, b);
         mbar_wait(&v_empty[slot], phase ^ 1);
         mbar_expect_tx(&v_full[slot], F8_TILE);
-        tma_load_3d(v_smem + slot * F8_TILE, &tmV, &v_full[slot], j * BKV, 0, b * p.H + h);
+        tma_load_3d(v_smem + slot * F8_TILE, &tmV, &v_full[slot], kv_block(j) * BKV, 0, b * p.H + h);
       }
     }
     return;
@@ -279,8 +317,18 @@ attn_fp8_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     __syncwarp();
     if (lane == 0) mbar_arrive(&k_empty[slot]);
 
-    const int kv0 = j * BKV;
-    if (kv0 + BKV > p.S) {   // masked tail columns give p = 0
+    const int kv0 = kv_block(j) * BKV;
+    if (WIN) {
+      const int kv1 = kv0 + BKV;
+      const bool whole = (kv0 >= tw.x && kv1 <= tw.y) || (kv0 >= (tw.y == p.S_txt ? tw.x : p.S_txt) && kv1 <= p.S);
+      if (!whole) {   // masked text columns and the tail give p = 0
+#pragma unroll
+        for (int i = 0; i < 64; ++i) {
+          const int col = kv0 + 8 * (i >> 2) + colq + (i & 1);
+          if (col >= p.S || (col < p.S_txt && (col < tw.x || col >= tw.y))) s[i] = -INFINITY;
+        }
+      }
+    } else if (kv0 + BKV > p.S) {   // masked tail columns give p = 0
 #pragma unroll
       for (int i = 0; i < 64; ++i)
         if (kv0 + 8 * (i >> 2) + colq + (i & 1) >= p.S) s[i] = -INFINITY;
@@ -365,10 +413,9 @@ bool misaligned16(const void* a) { return reinterpret_cast<uintptr_t>(a) & 15; }
 
 }  // namespace
 
-extern "C" int b2f_attn_quant_fp8(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
-                                  void* q8, void* k8, float* sq, float* sk, void* v8t, float* sv, int B, int H, int S,
-                                  int head_dim, b2f_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+static int attn_quant_fp8_impl(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                               void* q8, void* k8, float* sq, float* sk, void* v8t, float* sv, int B, int H, int S,
+                               int head_dim, const int32_t* win, int S_txt, cudaStream_t stream) {
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!q || !k || !v || !q8 || !k8 || !sq || !sk || !v8t || !sv || B <= 0 || H <= 0 || S <= 0) return B2F_ERR_INVALID;
   if (head_dim != DH) return B2F_ERR_UNSUPPORTED;
@@ -379,7 +426,7 @@ extern "C" int b2f_attn_quant_fp8(const void* q, int64_t ldq, const void* k, int
   const int nblk = (S + QTOK - 1) / QTOK;
   QuantAttnParams p{static_cast<const __nv_bfloat16*>(q), static_cast<const __nv_bfloat16*>(k),
                     static_cast<const __nv_bfloat16*>(v), ldq, ldk, ldv, static_cast<uint8_t*>(q8),
-                    static_cast<uint8_t*>(k8), static_cast<uint8_t*>(v8t), sq, sk, sv, H, S, nblk * QTOK};
+                    static_cast<uint8_t*>(k8), static_cast<uint8_t*>(v8t), sq, sk, sv, H, S, nblk * QTOK, win, S_txt};
   const size_t heads = (size_t)B * H;
   cudaError_t e = cudaMemsetAsync(sq, 0, heads * sizeof(float), stream);
   if (e == cudaSuccess) e = cudaMemsetAsync(sk, 0, heads * sizeof(float), stream);
@@ -398,10 +445,25 @@ extern "C" int b2f_attn_quant_fp8(const void* q, int64_t ldq, const void* k, int
   return B2F_OK;
 }
 
-extern "C" int b2f_attention_fp8(const void* q8, const void* k8, const float* sq, const float* sk, const void* v8t,
-                                 const float* sv, void* out, int64_t ldo, int B, int H, int S, int head_dim,
-                                 float scale, int causal, b2f_stream_t stream_) {
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+extern "C" int b2f_attn_quant_fp8(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                                  void* q8, void* k8, float* sq, float* sk, void* v8t, float* sv, int B, int H, int S,
+                                  int head_dim, b2f_stream_t stream) {
+  return attn_quant_fp8_impl(q, ldq, k, ldk, v, ldv, q8, k8, sq, sk, v8t, sv, B, H, S, head_dim, nullptr, 0,
+                             static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2f_attn_quant_fp8_window(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                                         int64_t ldv, void* q8, void* k8, float* sq, float* sk, void* v8t, float* sv,
+                                         int B, int H, int S, int head_dim, const int32_t* win, int S_txt,
+                                         b2f_stream_t stream) {
+  if (!win || S_txt < 0 || S_txt > S) return B2F_ERR_INVALID;
+  return attn_quant_fp8_impl(q, ldq, k, ldk, v, ldv, q8, k8, sq, sk, v8t, sv, B, H, S, head_dim, win, S_txt,
+                             static_cast<cudaStream_t>(stream));
+}
+
+static int attention_fp8_impl(const void* q8, const void* k8, const float* sq, const float* sk, const void* v8t,
+                              const float* sv, void* out, int64_t ldo, int B, int H, int S, int head_dim, float scale,
+                              int causal, const int32_t* win, int S_txt, cudaStream_t stream) {
   if (!device_info().ok) return B2F_ERR_NODEVICE;
   if (!q8 || !k8 || !sq || !sk || !v8t || !sv || !out || B <= 0 || H <= 0 || S <= 0) return B2F_ERR_INVALID;
   if (head_dim != DH || causal) return B2F_ERR_UNSUPPORTED;
@@ -409,7 +471,9 @@ extern "C" int b2f_attention_fp8(const void* q8, const void* k8, const float* sq
   if (misaligned16(q8) || misaligned16(k8) || misaligned16(v8t) || misaligned16(out)) return B2F_ERR_ALIGN;
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_fp8_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, F8_SMEM);
+    cudaError_t e = cudaFuncSetAttribute(attn_fp8_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, F8_SMEM);
+    if (e != cudaSuccess) return cuda_err(e, "attention fp8 smem attribute");
+    e = cudaFuncSetAttribute(attn_fp8_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, F8_SMEM);
     if (e != cudaSuccess) return cuda_err(e, "attention fp8 smem attribute");
     attr_set = true;
   }
@@ -424,16 +488,36 @@ extern "C" int b2f_attention_fp8(const void* q8, const void* k8, const float* sq
   rc = make_tmap_u8_rows(&tmV, v8t, 3, S_pad, DH, (uint64_t)B * H, S_pad, DH * S_pad);
   if (rc) return rc;
   // fp32(scale * log2 e) with the product of the fp32 scale taken in double
-  AttnFp8Params p{H, S, sq, sk, sv, float((double)scale * 1.4426950408889634), static_cast<__nv_bfloat16*>(out), ldo};
+  AttnFp8Params p{H, S, sq, sk, sv, float((double)scale * 1.4426950408889634), static_cast<__nv_bfloat16*>(out), ldo,
+                  win, S_txt};
   const dim3 grid((S + BQ - 1) / BQ, H, B);
   prof_begin(KC_ATTN, stream);
-  attn_fp8_kernel<<<grid, ATTN_THREADS, F8_SMEM, stream>>>(tmQ, tmK, tmV, p);
+  if (win)
+    attn_fp8_kernel<true><<<grid, ATTN_THREADS, F8_SMEM, stream>>>(tmQ, tmK, tmV, p);
+  else
+    attn_fp8_kernel<false><<<grid, ATTN_THREADS, F8_SMEM, stream>>>(tmQ, tmK, tmV, p);
   char tag[64];
   snprintf(tag, sizeof tag, "attn fp8 B%d H%d S%d", B, H, S);
   prof_end_tagged(KC_ATTN, stream, 4.0 * B * H * (double)S * S * DH,
                   (double)DH * B * H * (2.0 * S + S_pad) + 2.0 * DH * B * H * (double)S, tag);
-  B2F_LAUNCHED("attn_fp8_kernel", 1);
+  B2F_LAUNCHED(win ? "attn_fp8_kernel<window>" : "attn_fp8_kernel", 1);
   return B2F_OK;
+}
+
+extern "C" int b2f_attention_fp8(const void* q8, const void* k8, const float* sq, const float* sk, const void* v8t,
+                                 const float* sv, void* out, int64_t ldo, int B, int H, int S, int head_dim,
+                                 float scale, int causal, b2f_stream_t stream) {
+  return attention_fp8_impl(q8, k8, sq, sk, v8t, sv, out, ldo, B, H, S, head_dim, scale, causal, nullptr, 0,
+                            static_cast<cudaStream_t>(stream));
+}
+
+extern "C" int b2f_attention_fp8_window(const void* q8, const void* k8, const float* sq, const float* sk,
+                                        const void* v8t, const float* sv, void* out, int64_t ldo, int B, int H, int S,
+                                        int head_dim, float scale, const int32_t* win, int S_txt,
+                                        b2f_stream_t stream) {
+  if (!win || S_txt < 0 || S_txt > S) return B2F_ERR_INVALID;
+  return attention_fp8_impl(q8, k8, sq, sk, v8t, sv, out, ldo, B, H, S, head_dim, scale, 0, win, S_txt,
+                            static_cast<cudaStream_t>(stream));
 }
 
 }  // namespace b2f

@@ -63,6 +63,9 @@ struct FluxCtx {
   bool fp8_lora = false;
   // b2f_flux_set_fp8_attention: the blocks' attention runs in FP8 (b2f_attn_quant_fp8 + b2f_attention_fp8)
   bool fp8_attn = false;
+  // b2f_flux_set_text_window: per-item text windows int32 [text_win_B, 2] on the device (borrowed), or null
+  const int32_t* text_win = nullptr;
+  int text_win_B = 0;
   // fp32 gradient buffers of the trainable tensors, bound by name (flux_train.cu); an unbound name is frozen
   std::map<std::string, std::pair<float*, int64_t>> grads;
 };

@@ -272,6 +272,8 @@ int b2f_flux_finalize(b2f_flux* h) {
   c->fp8 = false;
   c->fp8_lora = false;
   c->fp8_attn = false;
+  c->text_win = nullptr;
+  c->text_win_B = 0;
   c->finalized = true;
   return B2F_OK;
 }
@@ -521,6 +523,16 @@ int b2f_flux_set_fp8_attention(b2f_flux* h, int on) {
   return B2F_OK;
 }
 
+int b2f_flux_set_text_window(b2f_flux* h, const int32_t* win_dev, int B) {
+  FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
+  if (!c || !c->finalized) return B2F_ERR_INVALID;
+  if (win_dev && B <= 0) return B2F_ERR_INVALID;
+  if (win_dev && (reinterpret_cast<uintptr_t>(win_dev) & 7)) return B2F_ERR_ALIGN;
+  c->text_win = win_dev;
+  c->text_win_B = win_dev ? B : 0;
+  return B2F_OK;
+}
+
 int b2f_flux_lora_rank(const b2f_flux* h) {
   const FluxCtx* c = reinterpret_cast<const FluxCtx*>(h);
   return c && c->finalized ? c->lora_rmax() : 0;
@@ -552,6 +564,10 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
     return B2F_ERR_INVALID;
   }
   if (ws_bytes < b2f_flux_workspace_bytes(h, B, S_img, S_txt)) return B2F_ERR_WORKSPACE;
+  if (c->text_win && c->text_win_B != B) {
+    fprintf(stderr, "[b2f] flux_forward: text windows set for B=%d, forward has B=%d\n", c->text_win_B, B);
+    return B2F_ERR_INVALID;
+  }
   const b2f_flux_cfg& g = c->cfg;
   const int64_t d = c->d;
   const int H = g.num_heads;
@@ -589,13 +605,24 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
   float* ask = asq + (int64_t)B * H;
   float* asv = ask + (int64_t)B * H;
   // joint attention of the qkv buffer into cat[:, :, :d]
+  // (with text windows set: the window entry points over the text rows [0, S_txt))
+  const int32_t* tw = c->text_win;
   auto attention = [&]() {
-    if (!c->fp8_attn)
+    if (!c->fp8_attn) {
+      if (tw)
+        return b2f_attention_fwd_window(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S,
+                                        g.head_dim, scale, tw, S_txt, st);
       return b2f_attention_fwd(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, cat, 5 * d, B, H, H, S, S, g.head_dim,
                                scale, 0, st);
-    const int r = b2f_attn_quant_fp8(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, aq8, ak8, asq, ask, av8, asv, B, H,
-                                     S, g.head_dim, st);
+    }
+    const int r = tw ? b2f_attn_quant_fp8_window(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, aq8, ak8, asq, ask, av8,
+                                                 asv, B, H, S, g.head_dim, tw, S_txt, st)
+                     : b2f_attn_quant_fp8(qkv, 3 * d, qkv + d, 3 * d, qkv + 2 * d, 3 * d, aq8, ak8, asq, ask, av8, asv,
+                                          B, H, S, g.head_dim, st);
     if (r) return r;
+    if (tw)
+      return b2f_attention_fp8_window(aq8, ak8, asq, ask, av8, asv, cat, 5 * d, B, H, S, g.head_dim, scale, tw, S_txt,
+                                      st);
     return b2f_attention_fp8(aq8, ak8, asq, ask, av8, asv, cat, 5 * d, B, H, S, g.head_dim, scale, 0, st);
   };
   const float ls = c->lora_scale;

@@ -133,6 +133,10 @@ int b2f_flux_train_forward(b2f_flux* h, const void* hidden, const void* enc, con
     fprintf(stderr, "[b2f] flux_train_forward: FP8 is on\n");
     return B2F_ERR_UNSUPPORTED;
   }
+  if (c->text_win) {   // the backward has no text windows
+    fprintf(stderr, "[b2f] flux_train_forward: text windows are set\n");
+    return B2F_ERR_UNSUPPORTED;
+  }
   if (ws_bytes < b2f_flux_train_workspace_bytes(h, B, S_img, S_txt)) return B2F_ERR_WORKSPACE;
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   const size_t infer = b2f_flux_workspace_bytes(h, B, S_img, S_txt);

@@ -146,6 +146,17 @@ def _norm_weights(cfg: FluxTransformerConfig):
     return out
 
 
+def text_windows(mask: torch.Tensor, B: int, S_txt: int) -> torch.Tensor:
+    """The per-item text windows of an encoder attention mask: [B, S_txt], each row one contiguous run of nonzeros
+    covering at least one token (left padding, as the Qwen processor pads, or right padding) -> int32 [B, 2] (lo, hi)
+    on the host.  Rows with holes, empty rows and shapes other than [B, S_txt] are refused."""
+    from .qwen2p5vl import padding_spans
+
+    if mask.dim() != 2 or tuple(mask.shape) != (B, S_txt):
+        raise _lib.B2FError(f"encoder_attention_mask: expected [{B}, {S_txt}], got {tuple(mask.shape)}")
+    return torch.tensor(padding_spans(mask), dtype=torch.int32)
+
+
 class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
     def __init__(self, config: FluxTransformerConfig | None = None, device="cuda", **kw):
         super().__init__()
@@ -197,6 +208,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         self._cache_cfg = None      # FirstBlockCacheConfig while the first-block cache is on
         self._cache_states = {}     # branch name -> _CacheState
         self._cache_epoch = 0       # bumped by every change of the weights or FP8 switches
+        self._text_wins = {}        # (mask identity) -> (mask, int32 [B, 2] device windows): validated once per mask
         self.cache_log = []         # one dict(branch, step, dist, hit) per cached forward since cache_reset()
         self._lora_init()
 
@@ -517,11 +529,28 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         _, cos, sin, _keep = self._rope
         check(_lib.lib.b2f_flux_set_rope(self._h, ptr(cos), ptr(sin), S_txt + S_img), "b2f_flux_set_rope")
 
+    def _text_window(self, mask: torch.Tensor, B: int, S_txt: int) -> torch.Tensor:
+        """Device windows of `mask` (text_windows), validated and uploaded once per mask tensor: a sampling loop that
+        passes the same mask every step pays one host round trip per call.  The entry keeps the mask alive, so its
+        address cannot be reused by another tensor while the entry exists, and an in-place write bumps _version."""
+        key = (mask.data_ptr(), mask._version, tuple(mask.shape), str(mask.device), B, S_txt)
+        hit = self._text_wins.get(key)
+        if hit is None:
+            win = text_windows(mask, B, S_txt).to(self.device)
+            if len(self._text_wins) >= 8:
+                self._text_wins.clear()
+            hit = self._text_wins[key] = (mask, win)
+        return hit[1]
+
     # ------------------------------------------------------------------ forward
     @torch.no_grad()
     def forward(self, hidden_states, encoder_hidden_states=None, pooled_projections=None, timestep=None,
                 img_ids=None, txt_ids=None, guidance=None, joint_attention_kwargs=None, return_dict=True,
-                **unused):
+                encoder_attention_mask=None, **unused):
+        """encoder_attention_mask: optional [B, S_txt] mask of the text tokens (1 = token, 0 = padding), each row one
+        contiguous run of ones (text_windows).  Batch item b then computes what it computes alone on its unpadded text:
+        masked text tokens are never keys for any query, and their content, NaN included, cannot reach an unmasked
+        output.  Image tokens are always valid."""
         cfg = self.config
         if self._fp8 is not None and self._lora_bound and not self._fp8_unfused:
             raise _lib.B2FError("FP8 is enabled and LoRA adapters are active unfused: fuse_lora() them first "
@@ -532,6 +561,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         B, S_img, _ = hidden_states.shape
         S_txt = encoder_hidden_states.shape[1]
         S = S_txt + S_img
+        win = None if encoder_attention_mask is None else self._text_window(encoder_attention_mask, B, S_txt)
         hs = hidden_states.to(torch.bfloat16).contiguous()
         enc = encoder_hidden_states.to(torch.bfloat16).contiguous()
         self._set_rope(txt_ids, img_ids, S_txt, S_img)
@@ -551,16 +581,22 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         out = torch.empty((B, n_out, cfg.out_channels), device=self.device, dtype=torch.bfloat16)
         nws = int(_lib.lib.b2f_flux_workspace_bytes(self._h, B, S_img, S_txt))
         ws = self._workspace(nws, "fwd")
-        if self._cache_cfg is not None:
-            if "_b2f_block_range" in jak:
-                raise _lib.B2FError("_b2f_block_range with the first-block cache on: the cache runs whole forwards only "
-                                    "(disable_cache() first)")
-            self._cache_forward(jak, lora_scale, hs, enc, mod, out, B, S_img, S_txt, n_out, ws, nws)
-            return (out,) if not return_dict else Transformer2DModelOutput(sample=out)
-        first, last = jak.get("_b2f_block_range", (0, -1))
-        check(_lib.lib.b2f_flux_forward(self._h, ptr(hs), ptr(enc), ptr(mod), mod.stride(0), ptr(out), B, S_img,
-                                        S_txt, n_out, ptr(ws), nws, int(first), int(last), stream_ptr()),
-              "b2f_flux_forward")
+        if self._cache_cfg is not None and "_b2f_block_range" in jak:
+            raise _lib.B2FError("_b2f_block_range with the first-block cache on: the cache runs whole forwards only "
+                                "(disable_cache() first)")
+        if win is not None:
+            check(_lib.lib.b2f_flux_set_text_window(self._h, ptr(win), B), "b2f_flux_set_text_window")
+        try:
+            if self._cache_cfg is not None:
+                self._cache_forward(jak, lora_scale, hs, enc, mod, out, B, S_img, S_txt, n_out, ws, nws)
+                return (out,) if not return_dict else Transformer2DModelOutput(sample=out)
+            first, last = jak.get("_b2f_block_range", (0, -1))
+            check(_lib.lib.b2f_flux_forward(self._h, ptr(hs), ptr(enc), ptr(mod), mod.stride(0), ptr(out), B, S_img,
+                                            S_txt, n_out, ptr(ws), nws, int(first), int(last), stream_ptr()),
+                  "b2f_flux_forward")
+        finally:
+            if win is not None:
+                check(_lib.lib.b2f_flux_set_text_window(self._h, None, 0), "b2f_flux_set_text_window")
         if not return_dict:
             return (out,)
         return Transformer2DModelOutput(sample=out)

@@ -63,10 +63,20 @@ def linear(x, weight, bias=None, *, epilogue: int = EPI_BIAS, out=None, resid=No
     return out
 
 
-def attention(q, k, v, *, out=None, causal: bool = False, scale: float | None = None, bias=None) -> torch.Tensor:
+def _text_window(win, S_txt, B: int, S: int):
+    _req(win, "win", torch.int32)
+    if tuple(win.shape) != (B, 2) or not win.is_contiguous():
+        raise _lib.B2FError(f"win: expected a contiguous int32 [B={B}, 2], got {tuple(win.shape)}")
+    if S_txt is None or not 0 <= S_txt <= S:
+        raise _lib.B2FError(f"S_txt: expected 0 <= S_txt <= {S}, got {S_txt}")
+
+
+def attention(q, k, v, *, out=None, causal: bool = False, scale: float | None = None, bias=None, win=None,
+              S_txt: int | None = None) -> torch.Tensor:
     """softmax(q k^T * scale [+ bias]) v via b2f_attention_fwd / b2f_attention_bias_fwd.  q [B,Sq,H,128],
     k/v [B,Skv,Hkv,128] as (possibly strided) views whose last two dims are contiguous; out [B,Sq,H*128];
-    bias [H,Sq,Skv] bf16 (shared by the batch; T5 relative position bias)."""
+    bias [H,Sq,Skv] bf16 (shared by the batch; T5 relative position bias).  win: per-item text windows int32 [B, 2]
+    (lo, hi) over the first S_txt keys (b2f_attention_fwd_window; non-causal, no bias)."""
     for t, n in ((q, "q"), (k, "k"), (v, "v")):
         _req(t, n)
         if t.dim() != 4 or t.stride(2) != t.shape[3] or (t.shape[0] > 1 and t.stride(0) != t.shape[1] * _row_pitch(t)):
@@ -89,6 +99,15 @@ def attention(q, k, v, *, out=None, causal: bool = False, scale: float | None = 
             ),
             "b2f_attention_bias_fwd",
         )
+        return out
+    if win is not None:
+        if causal or bias is not None:
+            raise _lib.B2FError("attention: text windows are non-causal and take no bias")
+        _text_window(win, S_txt, B, Skv)
+        check(_lib.lib.b2f_attention_fwd_window(ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v),
+                                                ptr(out), _row_pitch(out), B, H, Hkv, Sq, Skv, dh, float(scale), ptr(win),
+                                                int(S_txt), stream_ptr()),
+              "b2f_attention_fwd_window")
         return out
     check(
         _lib.lib.b2f_attention_fwd(
@@ -634,13 +653,22 @@ def _fp8_attn_buffers(B, S, H, dh, q8, k8, sq, sk, v8t, sv, device):
     return out
 
 
-def attn_quant_fp8(q, k, v, *, q8=None, k8=None, sq=None, sk=None, v8t=None, sv=None):
+def attn_quant_fp8(q, k, v, *, q8=None, k8=None, sq=None, sk=None, v8t=None, sv=None, win=None,
+                   S_txt: int | None = None):
     """(q8, k8, sq, sk, v8t, sv) of b2f_attn_quant_fp8: q, k, v bf16 [B,S,H,dh] views as attention() takes them ->
     q8 / k8 e4m3 [B,S,H,dh] with per-head scales sq / sk fp32 [B,H], v8t e4m3 [B,H,dh,S_pad] (tokens contiguous, in the
-    P-fragment order of include/b2f.h, padding +0) with per-channel scales sv fp32 [B,H,dh]."""
+    P-fragment order of include/b2f.h, padding +0) with per-channel scales sv fp32 [B,H,dh].  win / S_txt: per-item
+    text windows as attention() takes them (b2f_attn_quant_fp8_window)."""
     B, S, H, dh = _qkv_views(q, k, v)
     bufs = _fp8_attn_buffers(B, S, H, dh, q8, k8, sq, sk, v8t, sv, q.device)
     q8, k8, sq, sk, v8t, sv = bufs
+    if win is not None:
+        _text_window(win, S_txt, B, S)
+        check(_lib.lib.b2f_attn_quant_fp8_window(ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v),
+                                                 ptr(q8), ptr(k8), ptr(sq), ptr(sk), ptr(v8t), ptr(sv), B, H, S, dh,
+                                                 ptr(win), int(S_txt), stream_ptr()),
+              "b2f_attn_quant_fp8_window")
+        return tuple(bufs)
     check(_lib.lib.b2f_attn_quant_fp8(ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v), ptr(q8), ptr(k8),
                                       ptr(sq), ptr(sk), ptr(v8t), ptr(sv), B, H, S, dh, stream_ptr()),
           "b2f_attn_quant_fp8")
@@ -648,9 +676,10 @@ def attn_quant_fp8(q, k, v, *, q8=None, k8=None, sq=None, sk=None, v8t=None, sv=
 
 
 def attention_fp8(q8, k8, sq, sk, v8t, sv, *, out=None, scale: float | None = None, causal: bool = False,
-                  bias=None) -> torch.Tensor:
+                  bias=None, win=None, S_txt: int | None = None) -> torch.Tensor:
     """softmax(q k^T * scale) v via b2f_attention_fp8 from the buffers of attn_quant_fp8; out [B,S,H*dh] bf16 (any row
-    pitch).  Non-causal, without a bias: anything else raises."""
+    pitch).  Non-causal, without a bias: anything else raises.  win / S_txt: per-item text windows
+    (b2f_attention_fp8_window), the ones the buffers were quantized with."""
     if bias is not None:
         raise _lib.B2FError("attention_fp8: a score bias is not supported")
     _req(q8, "q8", FP8)
@@ -664,6 +693,15 @@ def attention_fp8(q8, k8, sq, sk, v8t, sv, *, out=None, scale: float | None = No
     _shape(out, "out", (B, S, H * dh))
     if B > 1 and out.stride(0) != S * out.stride(1):
         raise _lib.B2FError("out: expected batch stride S * row pitch")
+    if win is not None:
+        if causal:
+            raise _lib.B2FError("attention_fp8: text windows are non-causal")
+        _text_window(win, S_txt, B, S)
+        check(_lib.lib.b2f_attention_fp8_window(ptr(q8), ptr(k8), ptr(sq), ptr(sk), ptr(v8t), ptr(sv), ptr(out),
+                                                out.stride(1), B, H, S, dh, float(dh ** -0.5 if scale is None else scale),
+                                                ptr(win), int(S_txt), stream_ptr()),
+              "b2f_attention_fp8_window")
+        return out
     check(_lib.lib.b2f_attention_fp8(ptr(q8), ptr(k8), ptr(sq), ptr(sk), ptr(v8t), ptr(sv), ptr(out), out.stride(1), B,
                                      H, S, dh, float(dh ** -0.5 if scale is None else scale), int(causal), stream_ptr()),
           "b2f_attention_fp8")

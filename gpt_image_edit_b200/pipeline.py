@@ -30,6 +30,23 @@ PREFERRED_KONTEXT_RESOLUTIONS = [
 ]
 
 
+def stack_prompt_embeds(embeds):
+    """Batch prompt embeddings of different lengths: a list of [1, L_b, D] -> (embeds [B, max L_b, D], mask [B, max L_b]
+    int64), each item left-padded with zeros as the Qwen processor pads its prompts.  Pass the pair as prompt_embeds and
+    prompt_attention_mask: every item then samples what it samples alone on its own embeddings."""
+    if not embeds:
+        raise ValueError("stack_prompt_embeds: no embeddings")
+    if any(e.dim() != 3 or e.shape[0] != 1 or e.shape[1] < 1 or e.shape[2] != embeds[0].shape[2] for e in embeds):
+        raise ValueError(f"stack_prompt_embeds: expected [1, L, D] tensors of one D, got {[tuple(e.shape) for e in embeds]}")
+    L = max(e.shape[1] for e in embeds)
+    out = embeds[0].new_zeros((len(embeds), L, embeds[0].shape[2]))
+    mask = torch.zeros((len(embeds), L), dtype=torch.int64, device=embeds[0].device)
+    for b, e in enumerate(embeds):
+        out[b, L - e.shape[1]:] = e[0]
+        mask[b, L - e.shape[1]:] = 1
+    return out, mask
+
+
 def calculate_shift(image_seq_len, base_seq_len: int = 256, max_seq_len: int = 4096, base_shift: float = 0.5,
                     max_shift: float = 1.15):
     """mu is linear in the number of target tokens through (256, 0.5) and (4096, 1.15) (reference :106-116)."""
@@ -417,7 +434,11 @@ class FluxKontextPipeline:
                  callback_on_step_end: Optional[Callable] = None, callback_on_step_end_tensor_inputs=("latents",),
                  max_sequence_length: int = 512, max_area: int = 1024 ** 2, _auto_resize: bool = True,
                  ip_adapter_image=None, ip_adapter_image_embeds=None, negative_ip_adapter_image=None,
-                 negative_ip_adapter_image_embeds=None):
+                 negative_ip_adapter_image_embeds=None, prompt_attention_mask=None, negative_prompt_attention_mask=None):
+        """prompt_attention_mask / negative_prompt_attention_mask: optional [batch, L] masks of prompt_embeds /
+        negative_prompt_embeds (1 = token, 0 = padding; each row one contiguous run of ones, as stack_prompt_embeds
+        builds them) for batches of instructions of different lengths: every item samples what it samples alone on its
+        unpadded embeddings (B200FluxTransformer2DModel.forward, encoder_attention_mask)."""
         self._interrupt = False                    # reference :907-910: per-call state
         self._guidance_scale = guidance_scale
         self._joint_attention_kwargs = joint_attention_kwargs
@@ -459,12 +480,26 @@ class FluxKontextPipeline:
         batch_size = prompt_embeds.shape[0]
         device = self._execution_device
         dtype = prompt_embeds.dtype
+        if not do_true_cfg:
+            negative_prompt_attention_mask = None
+        for m, e, name in ((prompt_attention_mask, prompt_embeds, "prompt_attention_mask"),
+                           (negative_prompt_attention_mask, negative_prompt_embeds, "negative_prompt_attention_mask")):
+            if m is not None and tuple(m.shape) != tuple(e.shape[:2]):
+                raise ValueError(f"{name} has shape {tuple(m.shape)}; its embeddings have {tuple(e.shape[:2])}")
         if num_images_per_prompt != 1:
             prompt_embeds = prompt_embeds.repeat_interleave(num_images_per_prompt, dim=0)
             pooled_prompt_embeds = pooled_prompt_embeds.repeat_interleave(num_images_per_prompt, dim=0)
+            if prompt_attention_mask is not None:
+                prompt_attention_mask = prompt_attention_mask.repeat_interleave(num_images_per_prompt, dim=0)
             if do_true_cfg:
                 negative_prompt_embeds = negative_prompt_embeds.repeat_interleave(num_images_per_prompt, dim=0)
                 negative_pooled_prompt_embeds = negative_pooled_prompt_embeds.repeat_interleave(num_images_per_prompt, dim=0)
+                if negative_prompt_attention_mask is not None:
+                    negative_prompt_attention_mask = negative_prompt_attention_mask.repeat_interleave(
+                        num_images_per_prompt, dim=0)
+        # the masks go to the transformer as the same tensors every step: it validates and uploads each once per call
+        pos_kw = {} if prompt_attention_mask is None else {"encoder_attention_mask": prompt_attention_mask}
+        neg_kw = {} if negative_prompt_attention_mask is None else {"encoder_attention_mask": negative_prompt_attention_mask}
         text_ids = torch.zeros(prompt_embeds.shape[1], 3, device=device, dtype=dtype)
         negative_text_ids = torch.zeros(negative_prompt_embeds.shape[1], 3, device=device, dtype=dtype) if do_true_cfg else None
 
@@ -531,7 +566,7 @@ class FluxKontextPipeline:
             noise_pred = self.transformer(
                 hidden_states=x_in, timestep=timestep / 1000, guidance=guidance, pooled_projections=pooled_prompt_embeds,
                 encoder_hidden_states=prompt_embeds, txt_ids=text_ids, img_ids=latent_ids, joint_attention_kwargs=jak,
-                return_dict=False)[0]
+                return_dict=False, **pos_kw)[0]
             noise_pred = noise_pred[:, :n_tgt]
             if do_true_cfg:
                 # the hoisted modulation belongs to the positive pooled vector: the negative forward computes its own
@@ -541,7 +576,8 @@ class FluxKontextPipeline:
                 neg_noise_pred = self.transformer(
                     hidden_states=x_in, timestep=timestep / 1000, guidance=guidance,
                     pooled_projections=negative_pooled_prompt_embeds, encoder_hidden_states=negative_prompt_embeds,
-                    txt_ids=negative_text_ids, img_ids=latent_ids, joint_attention_kwargs=neg_jak, return_dict=False)[0]
+                    txt_ids=negative_text_ids, img_ids=latent_ids, joint_attention_kwargs=neg_jak, return_dict=False,
+                    **neg_kw)[0]
                 neg_noise_pred = neg_noise_pred[:, :n_tgt]
                 noise_pred = neg_noise_pred + true_cfg_scale * (noise_pred - neg_noise_pred)
             latents = self.scheduler.step(noise_pred, t, latents, return_dict=False)[0]

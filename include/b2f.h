@@ -35,7 +35,7 @@ typedef void* b2f_stream_t; /* cudaStream_t */
 const char* b2f_strerror(int code);
 /* ABI version; bumped on any signature change or addition (2: LoRA entry points, 3: FP8 entry points, 4: FP8
  * attention, 5: first-block cache, 6: GEMM tile override, 7: FP8 GEMMs with unfused LoRA, 8: VAE stop stage, ragged
- * and fp32-input softmax rows). */
+ * and fp32-input softmax rows, 9: per-item text windows in the joint attention). */
 int b2f_version(void);
 /* Device facts the host needs for grid sizing / reporting. Returns B2F_ERR_NODEVICE without GPU. */
 int b2f_device_info(int* num_sms, int* cc_major, int* cc_minor, size_t* smem_optin);
@@ -271,6 +271,19 @@ int b2f_attn_quant_fp8(const void* q, int64_t ldq, const void* k, int64_t ldk, c
 int b2f_attention_fp8(const void* q8, const void* k8, const float* sq, const float* sk, const void* v8t, const float* sv,
                       void* out, int64_t ldo, int B, int H, int S, int head_dim, float scale, int causal,
                       b2f_stream_t stream);
+/* The FP8 pair with the per-item text window of b2f_attention_fwd_window (win int32 DEVICE [B, 2], 0 <= S_txt <= S).
+ * The quantizer takes the Q / K amax of every head and the V amax of every channel over the valid tokens only, so an
+ * item's sq / sk / sv are bit-equal to those of its valid tokens quantized alone (the amax is order-independent); it
+ * writes masked tokens as +0 in q8, k8 and v8t.  The attention streams the 128-token blocks of the unwindowed kernel
+ * that hold a valid key, skips the others (no load, no MMA), and gives masked keys p = 0 (against V = +0).  The full
+ * window (0, S_txt) is bit-identical to b2f_attn_quant_fp8 + b2f_attention_fp8.  Masked query rows receive finite
+ * values that mean nothing. */
+int b2f_attn_quant_fp8_window(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v, int64_t ldv,
+                              void* q8, void* k8, float* sq, float* sk, void* v8t, float* sv, int B, int H, int S,
+                              int head_dim, const int32_t* win, int S_txt, b2f_stream_t stream);
+int b2f_attention_fp8_window(const void* q8, const void* k8, const float* sq, const float* sk, const void* v8t,
+                             const float* sv, void* out, int64_t ldo, int B, int H, int S, int head_dim, float scale,
+                             const int32_t* win, int S_txt, b2f_stream_t stream);
 
 /* ------------------------------------------------------------------------------------------
  * AdaLN modulate (HBM-bound): out = LayerNorm(x; eps, no affine) * (1 + scale[b]) + shift[b].
@@ -350,6 +363,19 @@ int b2f_temb_combine(const void* t, const void* g, const void* txt, void* temb, 
 int b2f_attention_fwd(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
                       int64_t ldv, void* out, int64_t ldo, int B, int H, int Hkv, int Sq, int Skv,
                       int head_dim, float scale, int causal, b2f_stream_t stream);
+
+/* Non-causal b2f_attention_fwd with a per-item text window: the first S_txt keys of every item are its text (0 <= S_txt
+ * <= Skv), win int32 DEVICE [B, 2] holds (lo, hi) per item, and key k of item b is valid iff k >= S_txt or
+ * lo <= k < hi (values outside 0 <= lo <= hi <= S_txt are clamped into that range).  Invalid keys never reach an
+ * output: the K/V blocks of 128 rows start at lo and cover [lo, Skv) when hi == S_txt, else [lo, hi) and then
+ * [S_txt, Skv), so blocks wholly outside the window are never loaded; within a block masked keys get p = 0, and pad
+ * V rows [hi, S_txt) sharing a block with valid keys are zeroed in shared memory first, so NaN or Inf there cannot
+ * reach P.V.  For hi == S_txt an item sees the blocks, in order and in the same positions, of its valid keys run alone
+ * (up to where its query rows sit); the full window (0, S_txt) is bit-identical to b2f_attention_fwd.  Rows of masked
+ * queries are computed like any other and mean nothing. */
+int b2f_attention_fwd_window(const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                             int64_t ldv, void* out, int64_t ldo, int B, int H, int Hkv, int Sq, int Skv,
+                             int head_dim, float scale, const int32_t* win, int S_txt, b2f_stream_t stream);
 
 /* Same kernel with an additive score bias: softmax(scale * q.k^T + bias[h]) v, bias bf16 with
  * element [h, s_q, s_kv] at bias + h*bias_h_stride + s_q*bias_row_stride + s_kv (shared by the
@@ -462,6 +488,16 @@ int b2f_flux_forward(b2f_flux* ctx, const void* hidden, const void* enc, const v
                      int64_t mod_ld, void* out, int B, int S_img, int S_txt, int n_out_rows,
                      void* ws, size_t ws_bytes, int first_block, int last_block,
                      b2f_stream_t stream);
+/* Per-item text windows for batches of instructions of different lengths: win_dev int32 DEVICE [B, 2] (borrowed, read
+ * when a forward runs) holds (lo, hi) per batch item; text token k of item b takes part iff lo <= k < hi, and each item
+ * then computes what it computes alone on its text rows [lo, hi).  b2f_flux_forward and b2f_flux_forward_cached run
+ * every block attention through b2f_attention_fwd_window (or the FP8 window pair) while it is set; the windows are not
+ * read on the host, so a forward stays graph-capturable.  Every other stage of a block works row by row, so pad rows
+ * need nothing else: their content, NaN included, stays in pad rows.  The first-block cache measures image rows
+ * only.  A forward whose B differs from the window's B returns B2F_ERR_INVALID; b2f_flux_train_forward returns
+ * B2F_ERR_UNSUPPORTED while a window is set.  win_dev NULL (or B <= 0 with NULL) switches windows off; b2f_flux_finalize
+ * does too. */
+int b2f_flux_set_text_window(b2f_flux* ctx, const int32_t* win_dev, int B);
 /* FP8 block linears (see b2f_gemm_fp8).  b2f_flux_bind_fp8 binds the e4m3 copy w8 [out, in] of one block linear and its
  * fp32 per-channel scales w_scale [out] (borrowed; made by b2f_quant_fp8_rows from the bf16 weight) under the linear's
  * bound name (transformer_blocks.{i}.attn.qkv / attn.add_qkv / attn.to_out.0 / attn.to_add_out / ff.net.0.proj /
