@@ -210,34 +210,55 @@ class B200T5Encoder(_Base):
         if b is None:
             c = self.config
             idx = t5_relative_position_bucket(L, c.relative_attention_num_buckets, c.relative_attention_max_distance)
-            # one-time table build per sequence length (like the RoPE tables), not on the per-call path
-            b = self.W["rel_bias"][idx.to(self._dev)].permute(2, 0, 1).contiguous()
+            # one-time table build per sequence length (like the RoPE tables), not on the per-call path.  Copied into a
+            # fresh [H, L, L] buffer: at L = 1 `.contiguous()` would keep the permuted view, whose innermost stride is H
+            b = torch.empty((c.num_heads, L, L), device=self._dev, dtype=torch.bfloat16)
+            b.copy_(self.W["rel_bias"][idx.to(self._dev)].permute(2, 0, 1))
             self._bias_cache[L] = b
         return b
+
+    def _t5_embed(self, input_ids):
+        """token embeddings [B*L, d] of ids [B, L]"""
+        ids = input_ids.to(self._dev, torch.int64).reshape(-1).contiguous()
+        return ops.embed(self.W["shared"], ids)
+
+    def _t5_layer(self, i, x, bias, attn, B, L, keep=None):
+        """Block i on x [B*L, d] -> the block's output (a new tensor); `bias` is `position_bias(L)`, `attn` the
+        [B, L, H*128] attention output buffer every block reuses.  `keep` (a dict) receives the buffers the block leaves
+        behind: `xn1`, `qkv` (heads in 128-wide slots), `attn_out`, `x_mid` (after o + residual), `xn2`, `gu`
+        ([wi_0 x | wi_1 x]) and `h` (gated GELU)."""
+        c, W = self.config, self.W
+        H = c.num_heads
+        p = f"block.{i}."
+        xn1 = ops.rmsnorm(x, W[p + "ln1"], eps=c.layer_norm_epsilon)
+        qkv = ops.linear(xn1, W[p + "qkv.w"])
+        q5 = qkv.view(B, L, 3, H, HP)
+        ops.attention(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], out=attn, scale=1.0, bias=bias)
+        x_mid = ops.linear(attn.view(B * L, H * HP), W[p + "o.w"], epilogue=ops.EPI_RESID, resid=x)
+        xn2 = ops.rmsnorm(x_mid, W[p + "ln2"], eps=c.layer_norm_epsilon)
+        gu = ops.linear(xn2, W[p + "wi.w"])
+        h = ops.geglu(gu, c.d_ff)
+        out = ops.linear(h, W[p + "wo.w"], epilogue=ops.EPI_RESID, resid=x_mid)
+        if keep is not None:
+            keep.update(xn1=xn1, qkv=qkv, attn_out=attn, x_mid=x_mid, xn2=xn2, gu=gu, h=h)
+        return out
+
+    def _t5_final(self, x):
+        return ops.rmsnorm(x, self.W["final_ln"], eps=self.config.layer_norm_epsilon)
 
     @torch.no_grad()
     def forward(self, input_ids: torch.Tensor, attention_mask=None, **kw) -> EncoderOutput:
         if attention_mask is not None and not bool(attention_mask.all()):
             raise _lib.B2FError("T5 padding masks are not implemented (the reference never passes one: "
                                 "denoiser_prompt_embedding_flux.py:44)")
-        c, W = self.config, self.W
+        c = self.config
         B, L = input_ids.shape
-        H, d = c.num_heads, c.d_model
-        ids = input_ids.to(self._dev, torch.int64).reshape(-1).contiguous()
-        x = ops.embed(W["shared"], ids)                                     # [B*L, d]
+        x = self._t5_embed(input_ids)                                       # [B*L, d]
         bias = self.position_bias(L)
-        attn = torch.empty((B, L, H * HP), device=self._dev, dtype=torch.bfloat16)
+        attn = torch.empty((B, L, c.num_heads * HP), device=self._dev, dtype=torch.bfloat16)
         for i in range(c.num_layers):
-            p = f"block.{i}."
-            xn = ops.rmsnorm(x, W[p + "ln1"], eps=c.layer_norm_epsilon)
-            qkv = ops.linear(xn, W[p + "qkv.w"]).view(B, L, 3, H, HP)
-            ops.attention(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], out=attn, scale=1.0, bias=bias)
-            x = ops.linear(attn.view(B * L, H * HP), W[p + "o.w"], epilogue=ops.EPI_RESID, resid=x)
-            xn = ops.rmsnorm(x, W[p + "ln2"], eps=c.layer_norm_epsilon)
-            h = ops.geglu(ops.linear(xn, W[p + "wi.w"]), c.d_ff)
-            x = ops.linear(h, W[p + "wo.w"], epilogue=ops.EPI_RESID, resid=x)
-        out = ops.rmsnorm(x, W["final_ln"], eps=c.layer_norm_epsilon)
-        return EncoderOutput(out.view(B, L, d))
+            x = self._t5_layer(i, x, bias, attn, B, L)
+        return EncoderOutput(self._t5_final(x).view(B, L, c.d_model))
 
 
 # ------------------------------------------------------------------------------------------------ CLIP
@@ -331,39 +352,59 @@ class B200CLIPTextModel(_Base):
                 _randn_into(t, g, std)
         return self
 
+    def _clip_embed(self, ids):
+        """token + position embeddings [B*L, d] of ids [B, L] on the device"""
+        return ops.embed(self.W["tok"], ids.reshape(-1).contiguous(), self.W["pos"], period=ids.shape[1])
+
+    def _clip_layer(self, i, x, attn, B, L, keep=None):
+        """Layer i on x [B*L, d] -> the layer's output (a new tensor); `attn` is the [B, L, H*128] attention output
+        buffer every layer reuses.  `keep` (a dict) receives `xn1`, `qkv` (heads in 128-wide slots), `attn_out`, `x_mid`
+        (after out_proj + residual), `xn2` and `fc1` (after quick-GELU)."""
+        c, W = self.config, self.W
+        H = c.num_attention_heads
+        p = f"layers.{i}."
+        xn1 = ops.layernorm(x, W[p + "ln1.w"], W[p + "ln1.b"], eps=c.layer_norm_eps)
+        qkv = ops.linear(xn1, W[p + "qkv.w"], W[p + "qkv.b"])
+        q5 = qkv.view(B, L, 3, H, HP)
+        ops.attention(q5[:, :, 0], q5[:, :, 1], q5[:, :, 2], out=attn, scale=self.hd ** -0.5, causal=True)
+        x_mid = ops.linear(attn.view(B * L, H * HP), W[p + "o.w"], W[p + "o.b"], epilogue=ops.EPI_RESID, resid=x)
+        xn2 = ops.layernorm(x_mid, W[p + "ln2.w"], W[p + "ln2.b"], eps=c.layer_norm_eps)
+        fc1 = ops.linear(xn2, W[p + "fc1.w"], W[p + "fc1.b"], epilogue=ops.EPI_QUICK_GELU)
+        out = ops.linear(fc1, W[p + "fc2.w"], W[p + "fc2.b"], epilogue=ops.EPI_RESID, resid=x_mid)
+        if keep is not None:
+            keep.update(xn1=xn1, qkv=qkv, attn_out=attn, x_mid=x_mid, xn2=xn2, fc1=fc1)
+        return out
+
+    def _clip_final(self, x, ids):
+        """final LayerNorm [B*L, d] and the pooled rows [B, d]: the hidden state at argmax(ids) under the
+        eos_token_id == 2 legacy rule, else at the first occurrence of eos_token_id (transformers
+        CLIPTextTransformer.forward)"""
+        c, W = self.config, self.W
+        B, L = ids.shape
+        last = ops.layernorm(x, W["final.w"], W["final.b"], eps=c.layer_norm_eps)
+        if c.eos_token_id == 2:
+            pos = ids.argmax(dim=-1)
+        else:
+            pos = (ids == c.eos_token_id).to(torch.int32).argmax(dim=-1)
+        rows = (torch.arange(B, device=self._dev) * L + pos).to(torch.int64)
+        return last, ops.gather_rows(last, rows)
+
     @torch.no_grad()
     def forward(self, input_ids: torch.Tensor, attention_mask=None, output_hidden_states: bool = False, **kw) -> EncoderOutput:
         if attention_mask is not None and not bool(attention_mask.all()):
             raise _lib.B2FError("CLIP padding masks are not implemented (the reference never passes one: "
                                 "denoiser_prompt_embedding_flux.py:91)")
-        c, W = self.config, self.W
+        c = self.config
         B, L = input_ids.shape
         if L > c.max_position_embeddings:
             raise ValueError(f"Sequence length must be less than max_position_embeddings (got {L} > {c.max_position_embeddings})")
-        d, H = c.hidden_size, c.num_attention_heads
-        ids2 = input_ids.to(self._dev, torch.int64)
-        x = ops.embed(W["tok"], ids2.reshape(-1).contiguous(), W["pos"], period=L)
-        attn = torch.empty((B, L, H * HP), device=self._dev, dtype=torch.bfloat16)
-        scale = self.hd ** -0.5
+        ids = input_ids.to(self._dev, torch.int64)
+        x = self._clip_embed(ids)
+        attn = torch.empty((B, L, c.num_attention_heads * HP), device=self._dev, dtype=torch.bfloat16)
         for i in range(c.num_hidden_layers):
-            p = f"layers.{i}."
-            xn = ops.layernorm(x, W[p + "ln1.w"], W[p + "ln1.b"], eps=c.layer_norm_eps)
-            qkv = ops.linear(xn, W[p + "qkv.w"], W[p + "qkv.b"]).view(B, L, 3, H, HP)
-            ops.attention(qkv[:, :, 0], qkv[:, :, 1], qkv[:, :, 2], out=attn, scale=scale, causal=True)
-            x = ops.linear(attn.view(B * L, H * HP), W[p + "o.w"], W[p + "o.b"], epilogue=ops.EPI_RESID, resid=x)
-            xn = ops.layernorm(x, W[p + "ln2.w"], W[p + "ln2.b"], eps=c.layer_norm_eps)
-            h = ops.linear(xn, W[p + "fc1.w"], W[p + "fc1.b"], epilogue=ops.EPI_QUICK_GELU)
-            x = ops.linear(h, W[p + "fc2.w"], W[p + "fc2.b"], epilogue=ops.EPI_RESID, resid=x)
-        last = ops.layernorm(x, W["final.w"], W["final.b"], eps=c.layer_norm_eps)
-        # pooled = hidden state at the EOS token: argmax(ids) under the eos_token_id == 2 legacy rule,
-        # else the first occurrence of eos_token_id (transformers CLIPTextTransformer.forward)
-        if c.eos_token_id == 2:
-            pos = ids2.argmax(dim=-1)
-        else:
-            pos = (ids2 == c.eos_token_id).to(torch.int32).argmax(dim=-1)
-        rows = (torch.arange(B, device=self._dev) * L + pos).to(torch.int64)
-        pooled = ops.gather_rows(last, rows)
-        return EncoderOutput(last.view(B, L, d), pooled)
+            x = self._clip_layer(i, x, attn, B, L)
+        last, pooled = self._clip_final(x, ids)
+        return EncoderOutput(last.view(B, L, c.hidden_size), pooled)
 
 
 # ------------------------------------------------------------------------------------------------ encode_prompt

@@ -41,6 +41,10 @@ WANT = [
                                       "test_stagewise_vae_matches_fp64[toy_64x96-decoder]"]),
     # the Qwen2.5-VL vision tower stage by stage at two blocks (80-wide heads in 128-wide slots, MLP 340 in 344)
     ("tests/test_qwen_stages_gpu.py", ["test_vit_stages_toy_width"]),
+    # the T5 / CLIP encoders stage by stage at d 256: the bias attention kernel (odd row stride 77, one-token rows),
+    # causal attention at 77 rows, 64-wide heads in 128-wide slots, gated GELU and the quick-GELU epilogue
+    ("tests/test_text_encoder_stages_gpu.py", ["test_stagewise_encoder_matches_fp64[toy_t5]",
+                                               "test_stagewise_encoder_matches_fp64[toy_clip]"]),
     ("tests/test_vae_gpu.py", ["test_conv3x3_matches_torch[1-8-16-64-128-1]", "test_conv3x3_matches_torch[1-33-50-64-256-1]",
                                "test_conv3x3_matches_torch[1-32-48-128-128-2]", "test_groupnorm_silu_matches_torch_chain[1-48-32-1]"]),
 ]
