@@ -1,11 +1,12 @@
 """Tensor-level wrappers over the C ABI (torch owns storage; libb2f does the work).
 
-Each function validates dtype/device/contiguity on the host, then passes raw device pointers and
+Each function validates dtype/device/contiguity and shapes on the host, then passes raw device pointers and
 the current CUDA stream to libb2f.  No function here computes anything in torch.
 """
 from __future__ import annotations
 
 import ctypes as C
+import math
 
 import torch
 
@@ -14,6 +15,7 @@ from ._lib import check, ptr, stream_ptr
 
 EPI_BIAS, EPI_GELU_TANH, EPI_SILU, EPI_GATE_RESID, EPI_RESID, EPI_GELU_ERF = 0, 1, 2, 3, 4, 5
 EPI_QUICK_GELU = 7
+FP8 = torch.float8_e4m3fn
 
 
 def _req(t: torch.Tensor, name: str, dtype=torch.bfloat16) -> None:
@@ -31,35 +33,129 @@ def _as3(t: torch.Tensor) -> torch.Tensor:
     return t if t.dim() == 3 else t.unsqueeze(0)
 
 
+def _shape(t: torch.Tensor, name: str, want) -> None:
+    if tuple(t.shape) != tuple(want):
+        raise _lib.B2FError(f"{name}: expected shape {tuple(want)}, got {tuple(t.shape)}")
+
+
+def _rows(t, name: str, B: int, M: int, n: int, dtype=torch.bfloat16) -> torch.Tensor:
+    """t as [B, M, n] rows (any row and batch pitch; a [M, n] view is one batch item), checked against that shape."""
+    _req(t, name, dtype)
+    t3 = _as3(t)
+    _shape(t3, name, (B, M, n))
+    return t3
+
+
+def _scales(s: torch.Tensor, name: str, B: int, rows: int) -> torch.Tensor:
+    """a per-row fp32 scale vector as [B, rows] (any batch pitch, unit row pitch); [rows] when B == 1."""
+    _req(s, name, torch.float32)
+    s2 = s if s.dim() == 2 else s.unsqueeze(0)
+    _shape(s2, name, (B, rows))
+    return s2
+
+
+# The forward GEMM entry points of include/b2f.h take the same operand groups in the same order: A rows [+ per-token
+# scales], weight [+ per-channel scales], bias, output rows and sizes, then the plain epilogue's or the fused QKV
+# epilogue's operands, then the LoRA k-extension.  libb2f sees pointers and pitches only, so each group is checked
+# against the launch's sizes here and returned as its arguments; alignment and pitch rules stay libb2f's.
+def _a_group(x, fp8: bool = False, x_scale=None):
+    """(B, M, K, args) of the A rows x [M, K] / [B, M, K]: bf16, or e4m3 with per-token fp32 scales [M] / [B, M]."""
+    _req(x, "xq" if fp8 else "x", FP8 if fp8 else torch.bfloat16)
+    x3 = _as3(x)
+    B, M, K = x3.shape
+    if not fp8:
+        return B, M, K, (ptr(x3), x3.stride(1), x3.stride(0))
+    s2 = _scales(x_scale, "x_scale", B, M)
+    return B, M, K, (ptr(x3), x3.stride(1), x3.stride(0), ptr(s2), s2.stride(0))
+
+
+def _w_group(w, name: str, K: int, fp8: bool = False, w_scale=None):
+    """(N, args) of the weight w [N, K]: bf16, or e4m3 with per-channel fp32 scales w_scale [N]."""
+    _req(w, name, FP8 if fp8 else torch.bfloat16)
+    N = w.shape[0]
+    _shape(w, name, (N, K))
+    if not fp8:
+        return N, (ptr(w), w.stride(0))
+    _req(w_scale, "w_scale", torch.float32)
+    _shape(w_scale, "w_scale", (N,))
+    return N, (ptr(w), w.stride(0), ptr(w_scale))
+
+
+def _bias_group(bias, N: int):
+    if bias is not None:
+        _req(bias, "bias")
+        _shape(bias, "bias", (N,))
+    return (ptr(bias),)
+
+
+def _out_group(x, out, B: int, M: int, N: int, n_arg: int, K: int):
+    """(out, args): the output rows out [B, M, N] (new, shaped like x's rows, when None) and the launch sizes
+    batch, M, n_arg (N, or d_model for the QKV epilogue), K."""
+    if out is None:
+        out = torch.empty((*x.shape[:-1], N), device=x.device, dtype=torch.bfloat16)
+    o3 = _rows(out, "out", B, M, N)
+    return out, (ptr(o3), o3.stride(1), o3.stride(0), B, M, n_arg, K)
+
+
+def _epi_group(epilogue: int, resid, gate, B: int, M: int, N: int):
+    """The plain epilogue: resid [B, M, N] for EPI_RESID / EPI_GATE_RESID, gate [B, N] (or [N], shared by the batch)
+    for EPI_GATE_RESID."""
+    ldr = rbs = gld = 0
+    if epilogue in (EPI_GATE_RESID, EPI_RESID):
+        r3 = _rows(resid, "resid", B, M, N)
+        ldr, rbs = r3.stride(1), r3.stride(0)
+        if epilogue == EPI_GATE_RESID:
+            _req(gate, "gate")
+            _shape(gate, "gate", (B, N) if gate.dim() == 2 else (N,))
+            gld = gate.stride(0) if gate.dim() == 2 else 0
+    return (epilogue, ptr(resid), ldr, rbs, ptr(gate), gld)
+
+
+def _qkv_group(n_w: int, B: int, M: int, nw_q, nw_k, cos, sin, rope_row0: int, eps: float, out_extra, epi_extra: int,
+               fp8: bool = False):
+    """(d_model, args) of the fused QKV epilogue on a weight of n_w = 3 d_model + n_extra rows: RMSNorm weights [128],
+    RoPE tables fp32 [>= rope_row0 + M, 128], and out_extra [B, M, n_extra] for the columns after [Q|K|V]."""
+    for t, n in zip((nw_q, nw_k), ("nq", "nk") if fp8 else ("wq", "wk")):
+        _req(t, n)
+        _shape(t, n, (128,))
+    _req(cos, "cos", torch.float32)
+    _req(sin, "sin", torch.float32)
+    if cos.dim() != 2 or cos.shape[0] < rope_row0 + M or cos.shape[1] != 128 or cos.shape != sin.shape:
+        raise _lib.B2FError(f"cos/sin: expected [>= {rope_row0 + M}, 128] tables, got {tuple(cos.shape)} / "
+                            f"{tuple(sin.shape)}")
+    n_extra, extra = 0, (None, 0, 0)
+    if out_extra is not None:
+        _req(out_extra, "out_extra")
+        n_extra = out_extra.shape[-1]
+        e3 = _rows(out_extra, "out_extra", B, M, n_extra)
+        extra = (ptr(e3), e3.stride(1), e3.stride(0))
+    if (n_w - n_extra) % 3:
+        raise _lib.B2FError(f"weight: {n_w} rows less n_extra = {n_extra} do not split into Q, K and V")
+    return (n_w - n_extra) // 3, (ptr(nw_q), ptr(nw_k), ptr(cos), ptr(sin), rope_row0, eps, n_extra, *extra, epi_extra)
+
+
+def _lora_group(t, bcat, B: int, M: int, N: int):
+    """The LoRA k-extension: t [B, M, r_pad] (rows as x's) and bcat [N, r_pad]."""
+    _req(bcat, "bcat")
+    r_pad = bcat.shape[-1]
+    _shape(bcat, "bcat", (N, r_pad))
+    t3 = _rows(t, "t", B, M, r_pad)
+    return (ptr(t3), t3.stride(1), t3.stride(0), ptr(bcat), bcat.stride(0), r_pad)
+
+
+def _gemm(name: str, *groups) -> None:
+    """Launch libb2f's `name` on the joined argument groups and the current stream."""
+    check(getattr(_lib.lib, name)(*(a for g in groups for a in g), stream_ptr()), name)
+
+
 def linear(x, weight, bias=None, *, epilogue: int = EPI_BIAS, out=None, resid=None, gate=None) -> torch.Tensor:
     """out = epilogue(x @ weight^T + bias) via b2f_gemm_bf16 (wgmma).
 
     x: [M,K] or [B,M,K] (any batch/row pitch); weight [N,K]; gate [B,N] for EPI_GATE_RESID."""
-    _req(x, "x")
-    _req(weight, "weight")
-    x3 = _as3(x)
-    B, M, K = x3.shape
-    N = weight.shape[0]
-    if out is None:
-        out = torch.empty((*x.shape[:-1], N), device=x.device, dtype=torch.bfloat16)
-    _req(out, "out")
-    o3 = _as3(out)
-    ldr = rbs = gld = 0
-    if epilogue in (EPI_GATE_RESID, EPI_RESID):
-        _req(resid, "resid")
-        r3 = _as3(resid)
-        ldr, rbs = r3.stride(1), r3.stride(0)
-        if epilogue == EPI_GATE_RESID:
-            _req(gate, "gate")
-            gld = gate.stride(0) if gate.dim() == 2 else 0
-    check(
-        _lib.lib.b2f_gemm_bf16(
-            ptr(x3), x3.stride(1), x3.stride(0), ptr(weight), weight.stride(0), ptr(bias),
-            ptr(o3), o3.stride(1), o3.stride(0), B, M, N, K, epilogue,
-            ptr(resid), ldr, rbs, ptr(gate), gld, stream_ptr(),
-        ),
-        "b2f_gemm_bf16",
-    )
+    B, M, K, a = _a_group(x)
+    N, w = _w_group(weight, "weight", K)
+    out, o = _out_group(x, out, B, M, N, N, K)
+    _gemm("b2f_gemm_bf16", a, w, _bias_group(bias, N), o, _epi_group(epilogue, resid, gate, B, M, N))
     return out
 
 
@@ -77,15 +173,11 @@ def attention(q, k, v, *, out=None, causal: bool = False, scale: float | None = 
     k/v [B,Skv,Hkv,128] as (possibly strided) views whose last two dims are contiguous; out [B,Sq,H*128];
     bias [H,Sq,Skv] bf16 (shared by the batch; T5 relative position bias).  win: per-item text windows int32 [B, 2]
     (lo, hi) over the first S_txt keys (b2f_attention_fwd_window; non-causal, no bias)."""
-    for t, n in ((q, "q"), (k, "k"), (v, "v")):
-        _req(t, n)
-        if t.dim() != 4 or t.stride(2) != t.shape[3] or (t.shape[0] > 1 and t.stride(0) != t.shape[1] * _row_pitch(t)):
-            raise _lib.B2FError(f"{n}: expected a [B,S,H,dh] view with contiguous heads and batch stride S*ld")
-    B, Sq, H, dh = q.shape
+    B, Sq, H, dh = _qkv_views(q, k, v)
     Skv, Hkv = k.shape[1], k.shape[2]
     if out is None:
         out = torch.empty((B, Sq, H * dh), device=q.device, dtype=torch.bfloat16)
-    _req(out, "out")
+    ldo = _token_rows(out, "out", B, Sq, H * dh)
     if scale is None:
         scale = dh ** -0.5
     if bias is not None:
@@ -94,7 +186,7 @@ def attention(q, k, v, *, out=None, causal: bool = False, scale: float | None = 
             raise _lib.B2FError(f"bias: expected [H={H},Sq={Sq},Skv={Skv}] with unit inner stride, got {tuple(bias.shape)}")
         check(
             _lib.lib.b2f_attention_bias_fwd(
-                ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v), ptr(out), _row_pitch(out),
+                ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v), ptr(out), ldo,
                 B, H, Hkv, Sq, Skv, dh, float(scale), int(causal), ptr(bias), bias.stride(0), bias.stride(1), stream_ptr(),
             ),
             "b2f_attention_bias_fwd",
@@ -105,13 +197,13 @@ def attention(q, k, v, *, out=None, causal: bool = False, scale: float | None = 
             raise _lib.B2FError("attention: text windows are non-causal and take no bias")
         _text_window(win, S_txt, B, Skv)
         check(_lib.lib.b2f_attention_fwd_window(ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v),
-                                                ptr(out), _row_pitch(out), B, H, Hkv, Sq, Skv, dh, float(scale), ptr(win),
+                                                ptr(out), ldo, B, H, Hkv, Sq, Skv, dh, float(scale), ptr(win),
                                                 int(S_txt), stream_ptr()),
               "b2f_attention_fwd_window")
         return out
     check(
         _lib.lib.b2f_attention_fwd(
-            ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v), ptr(out), _row_pitch(out),
+            ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v), ptr(out), ldo,
             B, H, Hkv, Sq, Skv, dh, float(scale), int(causal), stream_ptr(),
         ),
         "b2f_attention_fwd",
@@ -282,23 +374,11 @@ def linear_qkv_norm_rope(x, weight, bias, wq, wk, cos, sin, *, rope_row0: int = 
                          out_extra=None, epi_extra: int = EPI_BIAS):
     """[Q|K|V] = x @ weight^T + bias with per-head RMSNorm + RoPE on Q, K fused in the GEMM epilogue.
     With `out_extra` [.., n_extra]: weight has 3d + n_extra rows, the extra columns go there via epi_extra."""
-    _req(x, "x")
-    _req(weight, "weight")
-    _req(cos, "cos", torch.float32)
-    _req(sin, "sin", torch.float32)
-    x3 = _as3(x)
-    B, M, K = x3.shape
-    n_extra = 0 if out_extra is None else out_extra.shape[-1]
-    N = weight.shape[0] - n_extra
-    if out is None:
-        out = torch.empty((*x.shape[:-1], N), device=x.device, dtype=torch.bfloat16)
-    o3 = _as3(out)
-    e3 = None if out_extra is None else _as3(out_extra)
-    check(_lib.lib.b2f_gemm_qkv_norm_rope(ptr(x3), x3.stride(1), x3.stride(0), ptr(weight), weight.stride(0), ptr(bias),
-                                          ptr(o3), o3.stride(1), o3.stride(0), B, M, N // 3, K, ptr(wq), ptr(wk),
-                                          ptr(cos), ptr(sin), rope_row0, eps, n_extra, ptr(e3),
-                                          0 if e3 is None else e3.stride(1), 0 if e3 is None else e3.stride(0),
-                                          epi_extra, stream_ptr()), "b2f_gemm_qkv_norm_rope")
+    B, M, K, a = _a_group(x)
+    n_w, w = _w_group(weight, "weight", K)
+    d, qkv = _qkv_group(n_w, B, M, wq, wk, cos, sin, rope_row0, eps, out_extra, epi_extra)
+    out, o = _out_group(x, out, B, M, 3 * d, d, K)
+    _gemm("b2f_gemm_qkv_norm_rope", a, w, _bias_group(bias, n_w), o, qkv)
     return out
 
 
@@ -318,66 +398,34 @@ def blend(a, b, wa: float, wb: float, *, out=None) -> torch.Tensor:
 def lora_down(x, acat, colscale, *, cs_mul: float = 1.0, out=None) -> torch.Tensor:
     """T = bf16(fp32(x @ acat^T) * fp32(colscale * cs_mul)) via b2f_gemm_colscale.  x [.., K], acat [r_pad, K],
     colscale fp32 [r_pad]."""
-    _req(x, "x")
-    _req(acat, "acat")
+    B, M, K, a = _a_group(x)
+    N, w = _w_group(acat, "acat", K)
     _req(colscale, "colscale", torch.float32)
-    x3 = _as3(x)
-    B, M, K = x3.shape
-    N = acat.shape[0]
-    if out is None:
-        out = torch.empty((*x.shape[:-1], N), device=x.device, dtype=torch.bfloat16)
-    o3 = _as3(out)
-    check(_lib.lib.b2f_gemm_colscale(ptr(x3), x3.stride(1), x3.stride(0), ptr(acat), acat.stride(0), ptr(o3),
-                                     o3.stride(1), o3.stride(0), B, M, N, K, ptr(colscale), float(cs_mul), stream_ptr()),
-          "b2f_gemm_colscale")
+    _shape(colscale, "colscale", (N,))
+    out, o = _out_group(x, out, B, M, N, N, K)
+    _gemm("b2f_gemm_colscale", a, w, o, (ptr(colscale), float(cs_mul)))
     return out
 
 
 def linear_lora(x, weight, bias, t, bcat, *, epilogue: int = EPI_BIAS, out=None, resid=None, gate=None) -> torch.Tensor:
     """out = epilogue(x @ weight^T + t @ bcat^T + bias) via b2f_gemm_bf16_lora (one fp32 accumulation).
     t [.., r_pad] (rows as x), bcat [N, r_pad]."""
-    _req(x, "x")
-    _req(weight, "weight")
-    _req(t, "t")
-    _req(bcat, "bcat")
-    x3, t3 = _as3(x), _as3(t)
-    B, M, K = x3.shape
-    N = weight.shape[0]
-    if out is None:
-        out = torch.empty((*x.shape[:-1], N), device=x.device, dtype=torch.bfloat16)
-    o3 = _as3(out)
-    ldr = rbs = gld = 0
-    if epilogue in (EPI_GATE_RESID, EPI_RESID):
-        r3 = _as3(resid)
-        ldr, rbs = r3.stride(1), r3.stride(0)
-        if epilogue == EPI_GATE_RESID:
-            gld = gate.stride(0) if gate.dim() == 2 else 0
-    check(_lib.lib.b2f_gemm_bf16_lora(ptr(x3), x3.stride(1), x3.stride(0), ptr(weight), weight.stride(0), ptr(bias),
-                                      ptr(o3), o3.stride(1), o3.stride(0), B, M, N, K, epilogue, ptr(resid), ldr, rbs,
-                                      ptr(gate), gld, ptr(t3), t3.stride(1), t3.stride(0), ptr(bcat), bcat.stride(0),
-                                      bcat.shape[1], stream_ptr()), "b2f_gemm_bf16_lora")
+    B, M, K, a = _a_group(x)
+    N, w = _w_group(weight, "weight", K)
+    out, o = _out_group(x, out, B, M, N, N, K)
+    _gemm("b2f_gemm_bf16_lora", a, w, _bias_group(bias, N), o, _epi_group(epilogue, resid, gate, B, M, N),
+          _lora_group(t, bcat, B, M, N))
     return out
 
 
 def linear_qkv_norm_rope_lora(x, weight, bias, wq, wk, cos, sin, t, bcat, *, rope_row0: int = 0, out=None,
                               eps: float = 1e-6, out_extra=None, epi_extra: int = EPI_BIAS):
     """linear_qkv_norm_rope with the LoRA K-extension (t, bcat) of linear_lora."""
-    _req(x, "x")
-    _req(t, "t")
-    _req(bcat, "bcat")
-    x3, t3 = _as3(x), _as3(t)
-    B, M, K = x3.shape
-    n_extra = 0 if out_extra is None else out_extra.shape[-1]
-    N = weight.shape[0] - n_extra
-    if out is None:
-        out = torch.empty((*x.shape[:-1], N), device=x.device, dtype=torch.bfloat16)
-    o3 = _as3(out)
-    e3 = None if out_extra is None else _as3(out_extra)
-    check(_lib.lib.b2f_gemm_qkv_norm_rope_lora(
-        ptr(x3), x3.stride(1), x3.stride(0), ptr(weight), weight.stride(0), ptr(bias), ptr(o3), o3.stride(1),
-        o3.stride(0), B, M, N // 3, K, ptr(wq), ptr(wk), ptr(cos), ptr(sin), rope_row0, eps, n_extra, ptr(e3),
-        0 if e3 is None else e3.stride(1), 0 if e3 is None else e3.stride(0), epi_extra, ptr(t3), t3.stride(1),
-        t3.stride(0), ptr(bcat), bcat.stride(0), bcat.shape[1], stream_ptr()), "b2f_gemm_qkv_norm_rope_lora")
+    B, M, K, a = _a_group(x)
+    n_w, w = _w_group(weight, "weight", K)
+    d, qkv = _qkv_group(n_w, B, M, wq, wk, cos, sin, rope_row0, eps, out_extra, epi_extra)
+    out, o = _out_group(x, out, B, M, 3 * d, d, K)
+    _gemm("b2f_gemm_qkv_norm_rope_lora", a, w, _bias_group(bias, n_w), o, qkv, _lora_group(t, bcat, B, M, n_w))
     return out
 
 
@@ -393,22 +441,6 @@ def lora_fuse_(weight, bcat, acat, colscale, *, cs_mul: float = 1.0) -> torch.Te
 
 
 # ---------------------------------------------------------------------------------------------------- FP8 (e4m3)
-FP8 = torch.float8_e4m3fn
-
-
-def _shape(t: torch.Tensor, name: str, want) -> None:
-    if tuple(t.shape) != tuple(want):
-        raise _lib.B2FError(f"{name}: expected shape {tuple(want)}, got {tuple(t.shape)}")
-
-
-def _scales(s: torch.Tensor, name: str, B: int, rows: int) -> torch.Tensor:
-    """a per-row fp32 scale vector as [B, rows] (any batch pitch, unit row pitch); [rows] when B == 1."""
-    _req(s, name, torch.float32)
-    s2 = s if s.dim() == 2 else s.unsqueeze(0)
-    _shape(s2, name, (B, rows))
-    return s2
-
-
 def quant_fp8_rows(x, *, out=None, scale=None):
     """(q, scale): the FP8 row rule of include/b2f.h (b2f_quant_fp8_rows) on every row of x [rows, K] or [B, rows, K]
     (any pitches): q e4m3 like x, scale fp32 [rows] / [B, rows]."""
@@ -419,9 +451,7 @@ def quant_fp8_rows(x, *, out=None, scale=None):
         out = torch.empty(x.shape, device=x.device, dtype=FP8)
     if scale is None:
         scale = torch.empty(x.shape[:-1], device=x.device, dtype=torch.float32)
-    _req(out, "out", FP8)
-    q3, s2 = _as3(out), _scales(scale, "scale", B, rows)
-    _shape(q3, "out", (B, rows, K))
+    q3, s2 = _rows(out, "out", B, rows, K, FP8), _scales(scale, "scale", B, rows)
     check(_lib.lib.b2f_quant_fp8_rows(ptr(x3), x3.stride(1), x3.stride(0), ptr(q3), q3.stride(1), q3.stride(0), ptr(s2),
                                       s2.stride(0), B, rows, K, stream_ptr()), "b2f_quant_fp8_rows")
     return out, scale
@@ -439,9 +469,7 @@ def ln_modulate_fp8(x, scale, shift, *, out=None, row_scale=None, eps: float = 1
         out = torch.empty(x.shape, device=x.device, dtype=FP8)
     if row_scale is None:
         row_scale = torch.empty(x.shape[:-1], device=x.device, dtype=torch.float32)
-    _req(out, "out", FP8)
-    o3, s2 = _as3(out), _scales(row_scale, "row_scale", B, rows)
-    _shape(o3, "out", (B, rows, D))
+    o3, s2 = _rows(out, "out", B, rows, D, FP8), _scales(row_scale, "row_scale", B, rows)
     if scale.dim() != 2 or shift.stride(0) != scale.stride(0):
         raise _lib.B2FError("scale/shift must be [B,D] views with equal pitch")
     for t, n in ((scale, "scale"), (shift, "shift"), (scale_b, "scale_b"), (shift_b, "shift_b")):
@@ -453,166 +481,48 @@ def ln_modulate_fp8(x, scale, shift, *, out=None, row_scale=None, eps: float = 1
     return out, row_scale
 
 
-def _fp8_weight_checks(wq, w_scale, bias, N, K):
-    _shape(wq, "wq", (N, K))
-    _shape(w_scale, "w_scale", (N,))
-    if bias is not None:
-        _req(bias, "bias")
-        _shape(bias, "bias", (N,))
-
-
 def linear_fp8(xq, x_scale, wq, w_scale, bias=None, *, epilogue: int = EPI_BIAS, out=None, resid=None,
                gate=None) -> torch.Tensor:
     """out = epilogue(fp32(x_scale[m] * w_scale[n]) * (xq @ wq^T) + bias) via b2f_gemm_fp8.  xq e4m3 [M,K] / [B,M,K],
     x_scale fp32 [M] / [B,M], wq e4m3 [N,K], w_scale fp32 [N]."""
-    _req(xq, "xq", FP8)
-    _req(wq, "wq", FP8)
-    _req(w_scale, "w_scale", torch.float32)
-    x3 = _as3(xq)
-    B, M, K = x3.shape
-    s2 = _scales(x_scale, "x_scale", B, M)
-    N = wq.shape[0]
-    _fp8_weight_checks(wq, w_scale, bias, N, K)
-    if out is None:
-        out = torch.empty((*xq.shape[:-1], N), device=xq.device, dtype=torch.bfloat16)
-    _req(out, "out")
-    o3 = _as3(out)
-    _shape(o3, "out", (B, M, N))
-    ldr = rbs = gld = 0
-    if epilogue in (EPI_GATE_RESID, EPI_RESID):
-        _req(resid, "resid")
-        r3 = _as3(resid)
-        _shape(r3, "resid", (B, M, N))
-        ldr, rbs = r3.stride(1), r3.stride(0)
-        if epilogue == EPI_GATE_RESID:
-            _req(gate, "gate")
-            _shape(gate, "gate", (B, N) if gate.dim() == 2 else (N,))
-            gld = gate.stride(0) if gate.dim() == 2 else 0
-    check(_lib.lib.b2f_gemm_fp8(ptr(x3), x3.stride(1), x3.stride(0), ptr(s2), s2.stride(0), ptr(wq), wq.stride(0),
-                                ptr(w_scale), ptr(bias), ptr(o3), o3.stride(1), o3.stride(0), B, M, N, K, epilogue,
-                                ptr(resid), ldr, rbs, ptr(gate), gld, stream_ptr()), "b2f_gemm_fp8")
+    B, M, K, a = _a_group(xq, True, x_scale)
+    N, w = _w_group(wq, "wq", K, True, w_scale)
+    out, o = _out_group(xq, out, B, M, N, N, K)
+    _gemm("b2f_gemm_fp8", a, w, _bias_group(bias, N), o, _epi_group(epilogue, resid, gate, B, M, N))
     return out
 
 
 def linear_qkv_norm_rope_fp8(xq, x_scale, wq, w_scale, bias, nq, nk, cos, sin, *, rope_row0: int = 0, out=None,
                              eps: float = 1e-6, out_extra=None, epi_extra: int = EPI_BIAS):
     """linear_qkv_norm_rope with the FP8 operands of linear_fp8 (b2f_gemm_qkv_norm_rope_fp8)."""
-    _req(xq, "xq", FP8)
-    _req(wq, "wq", FP8)
-    _req(w_scale, "w_scale", torch.float32)
-    _req(cos, "cos", torch.float32)
-    _req(sin, "sin", torch.float32)
-    x3 = _as3(xq)
-    B, M, K = x3.shape
-    s2 = _scales(x_scale, "x_scale", B, M)
-    n_extra = 0 if out_extra is None else out_extra.shape[-1]
-    N = wq.shape[0] - n_extra
-    _fp8_weight_checks(wq, w_scale, bias, N + n_extra, K)
-    _shape(nq, "nq", (128,))
-    _shape(nk, "nk", (128,))
-    if cos.dim() != 2 or cos.shape[0] < rope_row0 + M or cos.shape[1] != 128 or cos.shape != sin.shape:
-        raise _lib.B2FError(f"cos/sin: expected [>= {rope_row0 + M}, 128] tables, got {tuple(cos.shape)} / "
-                            f"{tuple(sin.shape)}")
-    if out is None:
-        out = torch.empty((*xq.shape[:-1], N), device=xq.device, dtype=torch.bfloat16)
-    _req(out, "out")
-    o3 = _as3(out)
-    _shape(o3, "out", (B, M, N))
-    e3 = None
-    if out_extra is not None:
-        _req(out_extra, "out_extra")
-        e3 = _as3(out_extra)
-        _shape(e3, "out_extra", (B, M, n_extra))
-    check(_lib.lib.b2f_gemm_qkv_norm_rope_fp8(ptr(x3), x3.stride(1), x3.stride(0), ptr(s2), s2.stride(0), ptr(wq),
-                                              wq.stride(0), ptr(w_scale), ptr(bias), ptr(o3), o3.stride(1), o3.stride(0),
-                                              B, M, N // 3, K, ptr(nq), ptr(nk), ptr(cos), ptr(sin), rope_row0, eps,
-                                              n_extra, ptr(e3), 0 if e3 is None else e3.stride(1),
-                                              0 if e3 is None else e3.stride(0), epi_extra, stream_ptr()),
-          "b2f_gemm_qkv_norm_rope_fp8")
+    B, M, K, a = _a_group(xq, True, x_scale)
+    n_w, w = _w_group(wq, "wq", K, True, w_scale)
+    d, qkv = _qkv_group(n_w, B, M, nq, nk, cos, sin, rope_row0, eps, out_extra, epi_extra, fp8=True)
+    out, o = _out_group(xq, out, B, M, 3 * d, d, K)
+    _gemm("b2f_gemm_qkv_norm_rope_fp8", a, w, _bias_group(bias, n_w), o, qkv)
     return out
-
-
-def _lora_ext(t, bcat, B, M, N):
-    """(t3, r_pad) of a LoRA K-extension t [.., M, r_pad] / bcat [N, r_pad] checked against the launch."""
-    _req(t, "t")
-    _req(bcat, "bcat")
-    t3 = _as3(t)
-    r_pad = bcat.shape[1]
-    _shape(t3, "t", (B, M, r_pad))
-    _shape(bcat, "bcat", (N, r_pad))
-    return t3, r_pad
 
 
 def linear_fp8_lora(xq, x_scale, wq, w_scale, bias, t, bcat, *, epilogue: int = EPI_BIAS, out=None, resid=None,
                     gate=None) -> torch.Tensor:
     """out = epilogue(fp32(x_scale[m] * w_scale[n]) * (xq @ wq^T) + t @ bcat^T + bias) via b2f_gemm_fp8_lora: linear_fp8
     with the bf16 LoRA K-extension (t, bcat) of linear_lora accumulated onto the scaled FP8 accumulators."""
-    _req(xq, "xq", FP8)
-    _req(wq, "wq", FP8)
-    _req(w_scale, "w_scale", torch.float32)
-    x3 = _as3(xq)
-    B, M, K = x3.shape
-    s2 = _scales(x_scale, "x_scale", B, M)
-    N = wq.shape[0]
-    _fp8_weight_checks(wq, w_scale, bias, N, K)
-    t3, r_pad = _lora_ext(t, bcat, B, M, N)
-    if out is None:
-        out = torch.empty((*xq.shape[:-1], N), device=xq.device, dtype=torch.bfloat16)
-    _req(out, "out")
-    o3 = _as3(out)
-    _shape(o3, "out", (B, M, N))
-    ldr = rbs = gld = 0
-    if epilogue in (EPI_GATE_RESID, EPI_RESID):
-        _req(resid, "resid")
-        r3 = _as3(resid)
-        _shape(r3, "resid", (B, M, N))
-        ldr, rbs = r3.stride(1), r3.stride(0)
-        if epilogue == EPI_GATE_RESID:
-            _req(gate, "gate")
-            _shape(gate, "gate", (B, N) if gate.dim() == 2 else (N,))
-            gld = gate.stride(0) if gate.dim() == 2 else 0
-    check(_lib.lib.b2f_gemm_fp8_lora(ptr(x3), x3.stride(1), x3.stride(0), ptr(s2), s2.stride(0), ptr(wq), wq.stride(0),
-                                     ptr(w_scale), ptr(bias), ptr(o3), o3.stride(1), o3.stride(0), B, M, N, K, epilogue,
-                                     ptr(resid), ldr, rbs, ptr(gate), gld, ptr(t3), t3.stride(1), t3.stride(0),
-                                     ptr(bcat), bcat.stride(0), r_pad, stream_ptr()), "b2f_gemm_fp8_lora")
+    B, M, K, a = _a_group(xq, True, x_scale)
+    N, w = _w_group(wq, "wq", K, True, w_scale)
+    out, o = _out_group(xq, out, B, M, N, N, K)
+    _gemm("b2f_gemm_fp8_lora", a, w, _bias_group(bias, N), o, _epi_group(epilogue, resid, gate, B, M, N),
+          _lora_group(t, bcat, B, M, N))
     return out
 
 
 def linear_qkv_norm_rope_fp8_lora(xq, x_scale, wq, w_scale, bias, nq, nk, cos, sin, t, bcat, *, rope_row0: int = 0,
                                   out=None, eps: float = 1e-6, out_extra=None, epi_extra: int = EPI_BIAS):
     """linear_qkv_norm_rope_fp8 with the LoRA K-extension of linear_fp8_lora (b2f_gemm_qkv_norm_rope_fp8_lora)."""
-    _req(xq, "xq", FP8)
-    _req(wq, "wq", FP8)
-    _req(w_scale, "w_scale", torch.float32)
-    _req(cos, "cos", torch.float32)
-    _req(sin, "sin", torch.float32)
-    x3 = _as3(xq)
-    B, M, K = x3.shape
-    s2 = _scales(x_scale, "x_scale", B, M)
-    n_extra = 0 if out_extra is None else out_extra.shape[-1]
-    N = wq.shape[0] - n_extra
-    _fp8_weight_checks(wq, w_scale, bias, N + n_extra, K)
-    t3, r_pad = _lora_ext(t, bcat, B, M, N + n_extra)
-    _shape(nq, "nq", (128,))
-    _shape(nk, "nk", (128,))
-    if cos.dim() != 2 or cos.shape[0] < rope_row0 + M or cos.shape[1] != 128 or cos.shape != sin.shape:
-        raise _lib.B2FError(f"cos/sin: expected [>= {rope_row0 + M}, 128] tables, got {tuple(cos.shape)} / "
-                            f"{tuple(sin.shape)}")
-    if out is None:
-        out = torch.empty((*xq.shape[:-1], N), device=xq.device, dtype=torch.bfloat16)
-    _req(out, "out")
-    o3 = _as3(out)
-    _shape(o3, "out", (B, M, N))
-    e3 = None
-    if out_extra is not None:
-        _req(out_extra, "out_extra")
-        e3 = _as3(out_extra)
-        _shape(e3, "out_extra", (B, M, n_extra))
-    check(_lib.lib.b2f_gemm_qkv_norm_rope_fp8_lora(
-        ptr(x3), x3.stride(1), x3.stride(0), ptr(s2), s2.stride(0), ptr(wq), wq.stride(0), ptr(w_scale), ptr(bias),
-        ptr(o3), o3.stride(1), o3.stride(0), B, M, N // 3, K, ptr(nq), ptr(nk), ptr(cos), ptr(sin), rope_row0, eps,
-        n_extra, ptr(e3), 0 if e3 is None else e3.stride(1), 0 if e3 is None else e3.stride(0), epi_extra, ptr(t3),
-        t3.stride(1), t3.stride(0), ptr(bcat), bcat.stride(0), r_pad, stream_ptr()), "b2f_gemm_qkv_norm_rope_fp8_lora")
+    B, M, K, a = _a_group(xq, True, x_scale)
+    n_w, w = _w_group(wq, "wq", K, True, w_scale)
+    d, qkv = _qkv_group(n_w, B, M, nq, nk, cos, sin, rope_row0, eps, out_extra, epi_extra, fp8=True)
+    out, o = _out_group(xq, out, B, M, 3 * d, d, K)
+    _gemm("b2f_gemm_qkv_norm_rope_fp8_lora", a, w, _bias_group(bias, n_w), o, qkv, _lora_group(t, bcat, B, M, n_w))
     return out
 
 
@@ -623,15 +533,28 @@ def _row_pitch(t: torch.Tensor) -> int:
     return t.stride(1) if S > 1 else t.stride(0) if B > 1 else t[0, 0].numel()
 
 
-def _qkv_views(q, k, v):
-    """(B, S, H, dh) of bf16 [B,S,H,dh] views as attention() takes them, with one shape for all three."""
+def _qkv_views(q, k, v, prefix: str = ""):
+    """(B, Sq, H, dh) of q: q, k, v bf16 [B,S,H,dh] views as attention() takes them, k and v of one shape with q's B and
+    dh.  `prefix` goes before the operands' names in errors (the gradients "dq", "dk", "dv")."""
     for t, n in ((q, "q"), (k, "k"), (v, "v")):
-        _req(t, n)
+        _req(t, prefix + n)
         if t.dim() != 4 or t.stride(2) != t.shape[3] or (t.shape[0] > 1 and t.stride(0) != t.shape[1] * _row_pitch(t)):
-            raise _lib.B2FError(f"{n}: expected a [B,S,H,dh] view with contiguous heads and batch stride S*ld")
-    if not (q.shape == k.shape == v.shape):
-        raise _lib.B2FError(f"q, k, v: expected one shape, got {tuple(q.shape)}, {tuple(k.shape)}, {tuple(v.shape)}")
+            raise _lib.B2FError(f"{prefix}{n}: expected a [B,S,H,dh] view with contiguous heads and batch stride S*ld")
+    if k.shape != v.shape or k.shape[0] != q.shape[0] or k.shape[3] != q.shape[3]:
+        raise _lib.B2FError(f"{prefix}q, {prefix}k, {prefix}v: expected k and v of one shape with q's batch and head dim, "
+                            f"got {tuple(q.shape)}, {tuple(k.shape)}, {tuple(v.shape)}")
     return tuple(q.shape)
+
+
+def _token_rows(t, name: str, B: int, S: int, n: int) -> int:
+    """Row pitch of t, B * S token rows of n contiguous bf16 elements at one pitch: a [B, S, n] view, or [B, S, H, dh]
+    with contiguous heads and H * dh = n, whose batch stride is S rows."""
+    _req(t, name)
+    if (t.dim() not in (3, 4) or tuple(t.shape[:2]) != (B, S) or math.prod(t.shape[2:]) != n
+            or (t.dim() == 4 and t.stride(2) != t.shape[3]) or (B > 1 and t.stride(0) != S * _row_pitch(t))):
+        raise _lib.B2FError(f"{name}: expected {B} x {S} rows of {n} contiguous elements at one pitch ([B, S, {n}] or "
+                            f"[B, S, H, dh]), got shape {tuple(t.shape)}, strides {t.stride()}")
+    return _row_pitch(t)
 
 
 def _fp8_attn_buffers(B, S, H, dh, q8, k8, sq, sk, v8t, sv, device):
@@ -660,6 +583,8 @@ def attn_quant_fp8(q, k, v, *, q8=None, k8=None, sq=None, sk=None, v8t=None, sv=
     P-fragment order of include/b2f.h, padding +0) with per-channel scales sv fp32 [B,H,dh].  win / S_txt: per-item
     text windows as attention() takes them (b2f_attn_quant_fp8_window)."""
     B, S, H, dh = _qkv_views(q, k, v)
+    if k.shape != q.shape:
+        raise _lib.B2FError(f"q, k, v: expected one shape, got {tuple(q.shape)}, {tuple(k.shape)}, {tuple(v.shape)}")
     bufs = _fp8_attn_buffers(B, S, H, dh, q8, k8, sq, sk, v8t, sv, q.device)
     q8, k8, sq, sk, v8t, sv = bufs
     if win is not None:
@@ -689,20 +614,17 @@ def attention_fp8(q8, k8, sq, sk, v8t, sv, *, out=None, scale: float | None = No
     q8, k8, sq, sk, v8t, sv = _fp8_attn_buffers(B, S, H, dh, q8, k8, sq, sk, v8t, sv, q8.device)
     if out is None:
         out = torch.empty((B, S, H * dh), device=q8.device, dtype=torch.bfloat16)
-    _req(out, "out")
-    _shape(out, "out", (B, S, H * dh))
-    if B > 1 and out.stride(0) != S * out.stride(1):
-        raise _lib.B2FError("out: expected batch stride S * row pitch")
+    ldo = _token_rows(out, "out", B, S, H * dh)
     if win is not None:
         if causal:
             raise _lib.B2FError("attention_fp8: text windows are non-causal")
         _text_window(win, S_txt, B, S)
         check(_lib.lib.b2f_attention_fp8_window(ptr(q8), ptr(k8), ptr(sq), ptr(sk), ptr(v8t), ptr(sv), ptr(out),
-                                                out.stride(1), B, H, S, dh, float(dh ** -0.5 if scale is None else scale),
+                                                ldo, B, H, S, dh, float(dh ** -0.5 if scale is None else scale),
                                                 ptr(win), int(S_txt), stream_ptr()),
               "b2f_attention_fp8_window")
         return out
-    check(_lib.lib.b2f_attention_fp8(ptr(q8), ptr(k8), ptr(sq), ptr(sk), ptr(v8t), ptr(sv), ptr(out), out.stride(1), B,
+    check(_lib.lib.b2f_attention_fp8(ptr(q8), ptr(k8), ptr(sq), ptr(sk), ptr(v8t), ptr(sv), ptr(out), ldo, B,
                                      H, S, dh, float(dh ** -0.5 if scale is None else scale), int(causal), stream_ptr()),
           "b2f_attention_fp8")
     return out

@@ -11,7 +11,7 @@ import torch
 
 from . import _lib
 from ._lib import check, ptr, stream_ptr
-from .ops import _as3, _req
+from .ops import _as3, _qkv_views, _req, _row_pitch, _rows, _shape, _token_rows
 
 EPI_STORE, EPI_RESID, EPI_DGELU, EPI_DSILU = 0, 4, 8, 9
 
@@ -32,12 +32,10 @@ def linear_dgrad(dy, weight, *, epilogue: int = EPI_STORE, aux=None, out=None) -
     N = weight.shape[1]
     if out is None:
         out = torch.empty((*dy.shape[:-1], N), device=dy.device, dtype=torch.bfloat16)
-    _req(out, "out")
-    o3 = _as3(out)
+    o3 = _rows(out, "out", B, M, N)
     ld_aux = aux_bs = 0
     if epilogue != EPI_STORE:
-        _req(aux, "aux")
-        a3 = _as3(aux)
+        a3 = _rows(aux, "aux", B, M, N)
         ld_aux, aux_bs = a3.stride(1), a3.stride(0)
     check(_lib.lib.b2f_gemm_dgrad(ptr(d3), d3.stride(1), d3.stride(0), ptr(weight), weight.stride(0), ptr(o3),
                                   o3.stride(1), o3.stride(0), B, M, N, K, epilogue, ptr(aux), ld_aux, aux_bs, stream_ptr()),
@@ -59,15 +57,10 @@ def linear_wgrad(dy, x, *, out=None, accumulate: bool = False) -> torch.Tensor:
             raise _lib.B2FError("linear_wgrad: accumulate needs an existing gradient tensor")
         out = torch.empty((M, N), device=dy.device, dtype=torch.float32)
     _f32(out, "out")
+    _shape(out, "out", (M, N))
     check(_lib.lib.b2f_gemm_wgrad(ptr(d3), d3.stride(1), d3.stride(0), ptr(x3), x3.stride(1), x3.stride(0), ptr(out),
                                   out.stride(0), B, rows, M, N, int(accumulate), stream_ptr()), "b2f_gemm_wgrad")
     return out
-
-
-def _qkv_check(t, n):
-    _req(t, n)
-    if t.dim() != 4 or t.stride(2) != t.shape[3] or (t.shape[0] > 1 and t.stride(0) != t.shape[1] * t.stride(1)):
-        raise _lib.B2FError(f"{n}: expected a [B,S,H,128] view with contiguous heads and batch stride S*ld")
 
 
 def s_pad(S: int) -> int:
@@ -76,46 +69,45 @@ def s_pad(S: int) -> int:
 
 def attention_fwd_lse(q, k, v, *, out=None, scale: float | None = None):
     """(out [B,S,H*128], lse2 fp32 [B,H,S_pad]) — forward that keeps the base-2 log-sum-exp rows."""
-    for t, n in ((q, "q"), (k, "k"), (v, "v")):
-        _qkv_check(t, n)
-    B, Sq, H, dh = q.shape
+    B, Sq, H, dh = _qkv_views(q, k, v)
     Skv, Hkv = k.shape[1], k.shape[2]
     if out is None:
         out = torch.empty((B, Sq, H * dh), device=q.device, dtype=torch.bfloat16)
+    ldo = _token_rows(out, "out", B, Sq, H * dh)
     lse = torch.empty((B, H, s_pad(Sq)), device=q.device, dtype=torch.float32)
     if scale is None:
         scale = dh ** -0.5
-    check(_lib.lib.b2f_attention_fwd_lse(ptr(q), q.stride(1), ptr(k), k.stride(1), ptr(v), v.stride(1), ptr(out),
-                                         out.stride(1), B, H, Hkv, Sq, Skv, dh, float(scale), 0, ptr(lse), lse.stride(1),
+    check(_lib.lib.b2f_attention_fwd_lse(ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v), ptr(out),
+                                         ldo, B, H, Hkv, Sq, Skv, dh, float(scale), 0, ptr(lse), lse.stride(1),
                                          stream_ptr()), "b2f_attention_fwd_lse")
     return out, lse
 
 
 def attention_bwd(q, k, v, o, dout, lse, *, dq=None, dk=None, dv=None, scale: float | None = None):
     """dq, dk, dv ([B,S,H,128] views or new tensors) of softmax attention; o / dout: [B,S,H*128] views."""
-    for t, n in ((q, "q"), (k, "k"), (v, "v")):
-        _qkv_check(t, n)
-    _req(o, "o")
-    _req(dout, "dout")
-    _f32(lse, "lse")
-    B, S, H, dh = q.shape
-    if k.shape != q.shape or v.shape != q.shape:
+    B, S, H, dh = _qkv_views(q, k, v)
+    if k.shape != q.shape:
         raise _lib.B2FError("attention_bwd: the joint FLUX attention only (Sq == Skv, H == Hkv)")
+    ldo, lddo = _token_rows(o, "o", B, S, H * dh), _token_rows(dout, "dout", B, S, H * dh)
+    _f32(lse, "lse")
     sp = lse.shape[-1]
+    if lse.dim() != 3 or tuple(lse.shape[:2]) != (B, H) or sp < S or sp % 128 or not lse.is_contiguous():
+        raise _lib.B2FError(f"lse: expected a contiguous [B={B}, H={H}, S_pad] with S_pad >= {S} a multiple of 128, "
+                            f"got {tuple(lse.shape)}")
     mk = lambda: torch.empty((B, S, H, dh), device=q.device, dtype=torch.bfloat16)
     dq = mk() if dq is None else dq
     dk = mk() if dk is None else dk
     dv = mk() if dv is None else dv
-    for t, n in ((dq, "dq"), (dk, "dk"), (dv, "dv")):
-        _qkv_check(t, n)
+    if _qkv_views(dq, dk, dv, "d") != q.shape or dk.shape != q.shape:
+        raise _lib.B2FError(f"dq, dk, dv: expected q's shape {tuple(q.shape)}, got {tuple(dq.shape)}, {tuple(dk.shape)}")
     delta = torch.empty((B, H, sp), device=q.device, dtype=torch.float32)
     if scale is None:
         scale = dh ** -0.5
-    check(_lib.lib.b2f_attn_delta(ptr(o), o.stride(1), ptr(dout), dout.stride(1), ptr(delta), ptr(lse), B, H, S, sp,
+    check(_lib.lib.b2f_attn_delta(ptr(o), ldo, ptr(dout), lddo, ptr(delta), ptr(lse), B, H, S, sp,
                                   stream_ptr()), "b2f_attn_delta")
-    check(_lib.lib.b2f_attention_bwd(ptr(q), q.stride(1), ptr(k), k.stride(1), ptr(v), v.stride(1), ptr(dout),
-                                     dout.stride(1), ptr(lse), ptr(delta), sp, ptr(dq), dq.stride(1), ptr(dk), dk.stride(1),
-                                     ptr(dv), dv.stride(1), B, H, S, dh, float(scale), stream_ptr()), "b2f_attention_bwd")
+    check(_lib.lib.b2f_attention_bwd(ptr(q), _row_pitch(q), ptr(k), _row_pitch(k), ptr(v), _row_pitch(v), ptr(dout),
+                                     lddo, ptr(lse), ptr(delta), sp, ptr(dq), _row_pitch(dq), ptr(dk), _row_pitch(dk),
+                                     ptr(dv), _row_pitch(dv), B, H, S, dh, float(scale), stream_ptr()), "b2f_attention_bwd")
     return dq, dk, dv
 
 
