@@ -161,8 +161,6 @@ __global__ void __launch_bounds__(kThreads) cache_capture_kernel(const __nv_bflo
   }
 }
 
-inline size_t align256(size_t n) { return (n + 255) & ~size_t(255); }
-
 // The regions of a cache's memory for one shape, in the order include/b2f.h documents.
 struct Layout {
   size_t r[2], R, partials, dec, xy, end;
@@ -173,12 +171,12 @@ Layout layout_of(int64_t d, int B, int S_img, int n_out) {
   const size_t N = (size_t)B * S_img * d;
   L.ctas = (int)(((int64_t)B * S_img + kRowsPerCta - 1) / kRowsPerCta);
   L.r[0] = 0;
-  L.r[1] = align256(N * 4);
-  L.R = L.r[1] + align256(N * 4);
-  L.partials = L.R + align256((size_t)B * n_out * d * 4);
-  L.dec = L.partials + align256((size_t)L.ctas * 16);
+  L.r[1] = al256(N * 4);
+  L.R = L.r[1] + al256(N * 4);
+  L.partials = L.R + al256((size_t)B * n_out * d * 4);
+  L.dec = L.partials + al256((size_t)L.ctas * 16);
   L.xy = L.dec + 256;
-  L.end = L.xy + align256(N * 2);
+  L.end = L.xy + al256(N * 2);
   return L;
 }
 
@@ -210,7 +208,7 @@ size_t b2f_flux_cache_bytes(const b2f_flux* h, int B, int S_img, int S_txt, int 
 
 int b2f_flux_cache_create(b2f_flux_cache** out, void* mem, size_t bytes) {
   if (!out || !mem) return B2F_ERR_INVALID;
-  const uintptr_t p = reinterpret_cast<uintptr_t>(mem), a = (p + 255) & ~uintptr_t(255);
+  const uintptr_t p = reinterpret_cast<uintptr_t>(mem), a = al256(p);
   if (bytes < a - p + 256) return B2F_ERR_WORKSPACE;
   FluxCache* c = new (std::nothrow) FluxCache();
   if (!c) return B2F_ERR_INVALID;
@@ -272,9 +270,8 @@ int b2f_flux_forward_cached(b2f_flux* h, b2f_flux_cache* cache, float threshold,
   double* partials = reinterpret_cast<double*>(k->mem + L.partials);
   Decision* dec = reinterpret_cast<Decision*>(k->mem + L.dec);
   bf16_t* xy = reinterpret_cast<bf16_t*>(k->mem + L.xy);
-  // h[B, S, d] starts at the workspace's first 256-aligned byte (b2f_flux_forward's layout); its image rows at S_txt
-  __nv_bfloat16* h_img = reinterpret_cast<__nv_bfloat16*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255)) +
-                         (int64_t)S_txt * d;
+  // the image rows of b2f_flux_forward's h[B, S, d]
+  __nv_bfloat16* h_img = reinterpret_cast<__nv_bfloat16*>(fwd_ws(c, ws, B, S_img, S_txt).h + (int64_t)S_txt * d);
   const int64_t h_bs = (int64_t)S * d;
 
   const bool valid = k->valid && k->ctx == c && k->B == B && k->S_img == S_img && k->S_txt == S_txt &&

@@ -56,7 +56,6 @@ struct FluxCtx {
   // colscale (the per-call `scale` of joint_attention_kwargs).
   std::map<std::string, AdalnLora> adaln_lora;
   float lora_scale = 1.f;
-  int lora_count = 0;
   int lora_rmax() const;
   // b2f_flux_set_fp8: the block linears of b2f_flux_forward run in FP8; fp8_lora (mode 2): with unfused adapters
   bool fp8 = false;
@@ -69,6 +68,21 @@ struct FluxCtx {
   // fp32 gradient buffers of the trainable tensors, bound by name (flux_train.cu); an unbound name is frozen
   std::map<std::string, std::pair<float*, int64_t>> grads;
 };
+
+// The regions of b2f_flux_forward's workspace for one shape (flux_model.cu); with a null ws only `bytes` is meaningful.
+//   h [B,S,d] | xn [B,S,d] | qkv [B,S,3d] | cat [B,S,5d] | tb, the LoRA T [B,S,r_pad] (with adapters bound)
+//     packed in this order from the workspace's first 256-aligned byte;
+//   with FP8 on, one aligned region: e4m3 rows q8 [B,S,5d] and their scales qs [B,S];
+//   with FP8 attention on, one aligned region: e4m3 aq8 / ak8 [B,S,d], av8 [B,H,128,S_pad], fp32 asq / ask [B,H], asv [B,d].
+struct FwdWs {
+  bf16_t *h, *xn, *qkv, *cat, *tb;
+  uint8_t* q8;
+  float* qs;
+  uint8_t *aq8, *ak8, *av8;
+  float *asq, *ask, *asv;
+  size_t bytes;   // b2f_flux_workspace_bytes
+};
+FwdWs fwd_ws(const FluxCtx* c, void* ws, int B, int S_img, int S_txt);
 
 // b2f_flux_forward (flux_model.cu) after the handle cast.  x0, when set, receives the image rows of h right after the
 // embedders ([B, S_img, d] contiguous): the first-block cache (flux_cache.cu) compares block 0's output with them.

@@ -48,10 +48,11 @@ static int expect_lin(FluxCtx* c, const std::string& name, int64_t out_f, int64_
   return expect(c, name + ".bias", out_f, &l->b);
 }
 
-// Every linear a LoRA can target, by its bound name (the fused ones: attn.qkv, attn.add_qkv, qkv_mlp) or, for the
-// AdaLN linears, by its diffusers name (rows of the fused adaln weight).  f(name, lin or nullptr, row0, out, in).
-template <class F>
-static void for_each_linear(FluxCtx* c, F&& f) {
+// The model's linears: every one a LoRA can target, by its bound name (the fused ones: attn.qkv, attn.add_qkv,
+// qkv_mlp) or, for the AdaLN linears, by its diffusers name (rows of the fused adaln weight, which is not a target).
+// f(name, lin or nullptr, row0, out, in); the lin is const when the context is.
+template <class Ctx, class F>
+static void for_each_linear(Ctx* c, F&& f) {
   const b2f_flux_cfg& g = c->cfg;
   const int64_t d = c->d;
   f(std::string("x_embedder"), &c->x_embedder, 0, d, (int64_t)g.in_channels);
@@ -67,7 +68,7 @@ static void for_each_linear(FluxCtx* c, F&& f) {
   f(std::string("proj_out"), &c->proj_out, 0, (int64_t)g.out_channels, d);
   for (int i = 0; i < g.num_double; ++i) {
     const std::string p = "transformer_blocks." + std::to_string(i) + ".";
-    DoubleW& w = c->dbl[i];
+    auto& w = c->dbl[i];
     f(p + "attn.qkv", &w.qkv, 0, 3 * d, d);
     f(p + "attn.add_qkv", &w.add_qkv, 0, 3 * d, d);
     f(p + "attn.to_out.0", &w.to_out, 0, d, d);
@@ -81,7 +82,7 @@ static void for_each_linear(FluxCtx* c, F&& f) {
   }
   for (int i = 0; i < g.num_single; ++i) {
     const std::string p = "single_transformer_blocks." + std::to_string(i) + ".";
-    SingleW& w = c->sgl[i];
+    auto& w = c->sgl[i];
     f(p + "qkv_mlp", &w.qkv_mlp, 0, 7 * d, d);
     f(p + "proj_out", &w.proj_out, 0, d, 5 * d);
     f(p + "norm.linear", nullptr, (int64_t)g.num_double * 12 * d + (int64_t)i * 3 * d, 3 * d, d);
@@ -165,15 +166,73 @@ static void for_each_block_linear(FluxCtx* c, F&& f) {
 
 int FluxCtx::lora_rmax() const {
   int r = adaln_rmax(this);
-  auto upd = [&](const Lin& l) { r = std::max(r, l.lora.r_pad); };
-  for (const Lin* l : {&x_embedder, &context_embedder, &proj_out, &t1, &t2, &g1, &g2, &p1, &p2}) upd(*l);
-  for (const DoubleW& w : dbl)
-    for (const Lin* l : {&w.qkv, &w.add_qkv, &w.to_out, &w.to_add_out, &w.ff1, &w.ff2, &w.ffc1, &w.ffc2}) upd(*l);
-  for (const SingleW& w : sgl) {
-    upd(w.qkv_mlp);
-    upd(w.proj_out);
-  }
+  for_each_linear(this, [&](const std::string&, const Lin* l, int64_t, int64_t, int64_t) {
+    if (l) r = std::max(r, l->lora.r_pad);
+  });
   return r;
+}
+
+namespace {
+// Regions of a caller's workspace, each starting at the next 256-byte boundary and counted with 256 bytes of room for
+// that, so `bytes` suffices wherever the workspace starts.
+struct Regions {
+  uintptr_t end;   // the workspace, then the end of the last region
+  size_t bytes = 0;
+  template <class T>
+  T* take(size_t n) {
+    const uintptr_t p = al256(end);
+    end = p + n;
+    bytes += n + 256;
+    return reinterpret_cast<T*>(p);
+  }
+};
+
+// b2f_flux_temb's workspace, one region: 2 sinusoid tables [rows,256] + 6 activations [rows,d] (+ LoRA T [rows, r_pad]
+// with adapters bound)
+struct TembWs {
+  bf16_t *sin_t, *sin_g, *a1, *et, *eg, *ep, *tb;
+  size_t bytes;
+};
+TembWs temb_ws(const FluxCtx* c, void* ws, int rows) {
+  const size_t n = rows, d = c->d;
+  Regions r{reinterpret_cast<uintptr_t>(ws)};
+  TembWs w;
+  w.sin_t = r.take<bf16_t>((n * 256 * 2 + n * d * 6 + n * c->lora_rmax()) * 2);
+  w.sin_g = w.sin_t + n * 256;
+  w.a1 = w.sin_g + n * 256;   // hidden
+  w.et = w.a1 + n * d;
+  w.eg = w.et + n * d;
+  w.ep = w.eg + n * d;
+  w.tb = w.ep + n * d;
+  w.bytes = r.bytes;
+  return w;
+}
+}  // namespace
+
+FwdWs fwd_ws(const FluxCtx* c, void* ws, int B, int S_img, int S_txt) {
+  const size_t d = c->d, S = (size_t)S_img + S_txt, BS = (size_t)B * S, H = c->cfg.num_heads;
+  const size_t S_pad = (S + 127) / 128 * 128;
+  Regions r{reinterpret_cast<uintptr_t>(ws)};
+  FwdWs w{};
+  w.h = r.take<bf16_t>(BS * (10 * d + c->lora_rmax()) * 2);
+  w.xn = w.h + BS * d;
+  w.qkv = w.xn + BS * d;
+  w.cat = w.qkv + BS * 3 * d;
+  w.tb = w.cat + BS * 5 * d;
+  if (c->fp8) {
+    w.q8 = r.take<uint8_t>(BS * (5 * d + 4));
+    w.qs = reinterpret_cast<float*>(w.q8 + BS * 5 * d);
+  }
+  if (c->fp8_attn) {
+    w.aq8 = r.take<uint8_t>(B * d * (2 * S + S_pad) + B * (2 * H + d) * 4);
+    w.ak8 = w.aq8 + BS * d;
+    w.av8 = w.ak8 + BS * d;
+    w.asq = reinterpret_cast<float*>(w.av8 + B * d * S_pad);
+    w.ask = w.asq + B * H;
+    w.asv = w.ask + B * H;
+  }
+  w.bytes = r.bytes;
+  return w;
 }
 
 }  // namespace b2f
@@ -217,53 +276,31 @@ int64_t b2f_flux_mod_width(const b2f_flux* h) {
 int b2f_flux_finalize(b2f_flux* h) {
   FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
   if (!c) return B2F_ERR_INVALID;
-  const int64_t d = c->d, d4 = 4 * d;
   const b2f_flux_cfg& g = c->cfg;
-  int rc;
-#define EL(name, o, i, dst) \
-  if ((rc = expect_lin(c, name, o, i, dst)) != 0) return rc
-#define EW(name, n, dst) \
-  if ((rc = expect(c, name, n, dst)) != 0) return rc
-  EL("x_embedder", d, g.in_channels, &c->x_embedder);
-  EL("context_embedder", d, g.joint_dim, &c->context_embedder);
-  EL("time_text_embed.timestep_embedder.linear_1", d, 256, &c->t1);
-  EL("time_text_embed.timestep_embedder.linear_2", d, d, &c->t2);
-  if (g.guidance_embeds) {
-    EL("time_text_embed.guidance_embedder.linear_1", d, 256, &c->g1);
-    EL("time_text_embed.guidance_embedder.linear_2", d, d, &c->g2);
-  }
-  EL("time_text_embed.text_embedder.linear_1", d, g.pooled_dim, &c->p1);
-  EL("time_text_embed.text_embedder.linear_2", d, d, &c->p2);
-  EL("adaln", c->mod_width, d, &c->adaln);
-  EL("proj_out", g.out_channels, d, &c->proj_out);
   c->dbl.assign(g.num_double, DoubleW());
-  for (int i = 0; i < g.num_double; ++i) {
-    const std::string p = "transformer_blocks." + std::to_string(i) + ".";
-    DoubleW& w = c->dbl[i];
-    EL(p + "attn.qkv", 3 * d, d, &w.qkv);
-    EL(p + "attn.add_qkv", 3 * d, d, &w.add_qkv);
-    EL(p + "attn.to_out.0", d, d, &w.to_out);
-    EL(p + "attn.to_add_out", d, d, &w.to_add_out);
-    EL(p + "ff.net.0.proj", d4, d, &w.ff1);
-    EL(p + "ff.net.2", d, d4, &w.ff2);
-    EL(p + "ff_context.net.0.proj", d4, d, &w.ffc1);
-    EL(p + "ff_context.net.2", d, d4, &w.ffc2);
-    EW(p + "attn.norm_q.weight", g.head_dim, &w.norm_q);
-    EW(p + "attn.norm_k.weight", g.head_dim, &w.norm_k);
-    EW(p + "attn.norm_added_q.weight", g.head_dim, &w.norm_added_q);
-    EW(p + "attn.norm_added_k.weight", g.head_dim, &w.norm_added_k);
-  }
   c->sgl.assign(g.num_single, SingleW());
-  for (int i = 0; i < g.num_single; ++i) {
-    const std::string p = "single_transformer_blocks." + std::to_string(i) + ".";
-    SingleW& w = c->sgl[i];
-    EL(p + "qkv_mlp", 7 * d, d, &w.qkv_mlp);
-    EL(p + "proj_out", d, 5 * d, &w.proj_out);
-    EW(p + "attn.norm_q.weight", g.head_dim, &w.norm_q);
-    EW(p + "attn.norm_k.weight", g.head_dim, &w.norm_k);
+  // the fused AdaLN weight, every other linear of the inventory, the blocks' per-head RMSNorm weights
+  int rc = expect_lin(c, "adaln", c->mod_width, c->d, &c->adaln);
+  for_each_linear(c, [&](const std::string& name, Lin* l, int64_t, int64_t out_f, int64_t in_f) {
+    if (!rc && l) rc = expect_lin(c, name, out_f, in_f, l);
+  });
+  auto norm = [&](const std::string& name, const bf16_t** dst) {
+    if (!rc) rc = expect(c, name, g.head_dim, dst);
+  };
+  for (int i = 0; i < g.num_double; ++i) {
+    const std::string p = "transformer_blocks." + std::to_string(i) + ".attn.norm_";
+    DoubleW& w = c->dbl[i];
+    norm(p + "q.weight", &w.norm_q);
+    norm(p + "k.weight", &w.norm_k);
+    norm(p + "added_q.weight", &w.norm_added_q);
+    norm(p + "added_k.weight", &w.norm_added_k);
   }
-#undef EL
-#undef EW
+  for (int i = 0; i < g.num_single; ++i) {
+    const std::string p = "single_transformer_blocks." + std::to_string(i) + ".attn.norm_";
+    norm(p + "q.weight", &c->sgl[i].norm_q);
+    norm(p + "k.weight", &c->sgl[i].norm_k);
+  }
+  if (rc) return rc;
   // (re)binding weights drops every LoRA binding (the FP8 ones went with the reassigned block weights)
   for_each_linear(c, [](const std::string&, Lin* l, int64_t, int64_t, int64_t) {
     if (l) l->lora = LoraBind();
@@ -291,20 +328,13 @@ int b2f_flux_set_rope(b2f_flux* h, const float* cos, const float* sin, int S) {
 size_t b2f_flux_workspace_bytes(const b2f_flux* h, int B, int S_img, int S_txt) {
   const FluxCtx* c = reinterpret_cast<const FluxCtx*>(h);
   if (!c || B <= 0 || S_img <= 0 || S_txt < 0) return 0;
-  const size_t S = (size_t)S_img + S_txt;
-  // h[d] + xn[d] + qkv[3d] + cat[5d] per token, bf16; with unfused LoRA adapters bound, T[r_pad] per token; with FP8
-  // on, e4m3 q8[5d] and an fp32 scale per token; with FP8 attention on, the buffers of b2f_attn_quant_fp8
-  const size_t fp8 = c->fp8 ? (size_t)B * S * ((size_t)c->d * 5 + 4) + 256 : 0;
-  const size_t S_pad = (S + 127) / 128 * 128, H = (size_t)c->cfg.num_heads;
-  const size_t fa = c->fp8_attn ? (size_t)B * c->d * (2 * S + S_pad) + (size_t)B * (2 * H + c->d) * 4 + 256 : 0;
-  return (size_t)B * S * ((size_t)c->d * 10 + (size_t)c->lora_rmax()) * 2 + 1024 + fp8 + fa;
+  return fwd_ws(c, nullptr, B, S_img, S_txt).bytes;
 }
 
 size_t b2f_flux_temb_workspace_bytes(const b2f_flux* h, int rows) {
   const FluxCtx* c = reinterpret_cast<const FluxCtx*>(h);
   if (!c || rows <= 0) return 0;
-  // 2 sinusoid tables [rows,256] + 6 activations [rows,d] (+ LoRA T [rows, r_pad] with adapters bound)
-  return ((size_t)rows * 256 * 2 + (size_t)rows * c->d * 6 + (size_t)rows * c->lora_rmax()) * 2 + 1024;
+  return temb_ws(c, nullptr, rows).bytes;
 }
 
 int b2f_flux_temb(b2f_flux* h, const float* timestep, const float* guidance, const void* pooled,
@@ -314,17 +344,11 @@ int b2f_flux_temb(b2f_flux* h, const float* timestep, const float* guidance, con
   if (!c || !c->finalized || !timestep || !pooled || !temb || !silu_temb || rows <= 0 || !ws)
     return B2F_ERR_INVALID;
   if (c->cfg.guidance_embeds && !guidance) return B2F_ERR_INVALID;
-  if (ws_bytes < b2f_flux_temb_workspace_bytes(h, rows)) return B2F_ERR_WORKSPACE;
+  const TembWs w = temb_ws(c, ws, rows);
+  if (ws_bytes < w.bytes) return B2F_ERR_WORKSPACE;
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
   const int d = c->d;
-  bf16_t* w = reinterpret_cast<bf16_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255));
-  bf16_t* sin_t = w;
-  bf16_t* sin_g = sin_t + (size_t)rows * 256;
-  bf16_t* a1 = sin_g + (size_t)rows * 256;  // hidden
-  bf16_t* et = a1 + (size_t)rows * d;
-  bf16_t* eg = et + (size_t)rows * d;
-  bf16_t* ep = eg + (size_t)rows * d;
-  bf16_t* tb = ep + (size_t)rows * d;   // LoRA T
+  bf16_t *sin_t = w.sin_t, *sin_g = w.sin_g, *a1 = w.a1, *et = w.et, *eg = w.eg, *ep = w.ep, *tb = w.tb;
   const float ls = c->lora_scale;
   int rc;
   if ((rc = b2f_temb_sinusoid(timestep, sin_t, rows, st))) return rc;
@@ -383,7 +407,7 @@ int b2f_flux_modulation_ws(b2f_flux* h, const void* silu_temb, int rows, void* m
                          (int)d, B2F_EPI_BIAS, nullptr, 0, 0, nullptr, 0, st);
   if (rc) return rc;
   // each AdaLN linear with an adapter: its own K-extended launch over its rows of adaln, overwriting its columns of mod
-  bf16_t* tb = reinterpret_cast<bf16_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255));
+  bf16_t* tb = al256<bf16_t>(ws);
   bf16_t* m = static_cast<bf16_t*>(mod);
   for (const auto& kv : c->adaln_lora) {
     const AdalnLora& a = kv.second;
@@ -553,7 +577,6 @@ namespace b2f {
 int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mod, int64_t mod_ld, void* out, int B,
                  int S_img, int S_txt, int n_out_rows, void* ws, size_t ws_bytes, int first_block, int last_block,
                  bf16_t* x0, cudaStream_t st) {
-  b2f_flux* h = reinterpret_cast<b2f_flux*>(c);
   if (!c || !c->finalized) return B2F_ERR_INVALID;
   if (!hidden || !enc || !mod || !out || !ws || B <= 0 || S_img <= 0 || S_txt <= 0)
     return B2F_ERR_INVALID;
@@ -563,7 +586,8 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
     fprintf(stderr, "[b2f] flux_forward: RoPE tables not set for S=%d (have %d)\n", S, c->rope_S);
     return B2F_ERR_INVALID;
   }
-  if (ws_bytes < b2f_flux_workspace_bytes(h, B, S_img, S_txt)) return B2F_ERR_WORKSPACE;
+  const FwdWs L = fwd_ws(c, ws, B, S_img, S_txt);
+  if (ws_bytes < L.bytes) return B2F_ERR_WORKSPACE;
   if (c->text_win && c->text_win_B != B) {
     fprintf(stderr, "[b2f] flux_forward: text windows set for B=%d, forward has B=%d\n", c->text_win_B, B);
     return B2F_ERR_INVALID;
@@ -574,17 +598,10 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
   const float eps = 1e-6f;
   const float scale = 1.0f / sqrtf((float)g.head_dim);
 
-  bf16_t* base = reinterpret_cast<bf16_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255));
-  const int64_t BS = (int64_t)B * S;
-  bf16_t* hb = base;               // [B,S,d]
-  bf16_t* xn = hb + BS * d;        // [B,S,d]
-  bf16_t* qkv = xn + BS * d;       // [B,S,3d]
-  bf16_t* cat = qkv + BS * 3 * d;  // [B,S,5d]
-  bf16_t* tb = cat + BS * 5 * d;   // LoRA T [B,S,r_pad] (only with adapters bound)
+  bf16_t *hb = L.h, *xn = L.xn, *qkv = L.qkv, *cat = L.cat, *tb = L.tb;
   // FP8 on: e4m3 rows q8 [B,S,5d] (pitch 5d bytes) and their scales qs [B,S], rewritten before each block linear
-  uint8_t* q8 = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(tb + BS * c->lora_rmax()) + 255) &
-                                           ~uintptr_t(255));
-  float* qs = reinterpret_cast<float*>(q8 + BS * 5 * d);
+  uint8_t* q8 = L.q8;
+  float* qs = L.qs;
   const bool f8 = c->fp8;
   const int64_t q8_bs = (int64_t)S * 5 * d;
   const Q8 q_txt{q8, 5 * d, q8_bs, qs, S};
@@ -596,14 +613,8 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
     return b2f_quant_fp8_rows(cat + c0, 5 * d, (int64_t)S * 5 * d, q8, 5 * d, q8_bs, qs, S, B, S, K, st);
   };
   // FP8 attention on: q8 / k8 [B,S,d], v8t [B,H,128,S_pad] e4m3 and their scales sq / sk [B,H], sv [B,d] fp32
-  const int64_t S_pad = ((int64_t)S + 127) / 128 * 128;
-  uint8_t* aq8 = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(f8 ? reinterpret_cast<uint8_t*>(qs + BS) : q8) +
-                                             255) & ~uintptr_t(255));
-  uint8_t* ak8 = aq8 + BS * d;
-  uint8_t* av8 = ak8 + BS * d;
-  float* asq = reinterpret_cast<float*>(av8 + (int64_t)B * d * S_pad);
-  float* ask = asq + (int64_t)B * H;
-  float* asv = ask + (int64_t)B * H;
+  uint8_t *aq8 = L.aq8, *ak8 = L.ak8, *av8 = L.av8;
+  float *asq = L.asq, *ask = L.ask, *asv = L.asv;
   // joint attention of the qkv buffer into cat[:, :, :d]
   // (with text windows set: the window entry points over the text rows [0, S_txt))
   const int32_t* tw = c->text_win;
@@ -636,6 +647,19 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
   bf16_t* cat_img = cat + (int64_t)S_txt * 5 * d;
   bf16_t* cat_txt = cat;
   const bf16_t* modp = static_cast<const bf16_t*>(mod);
+  // the modulated LayerNorm of h before a step's linears (the first split_row rows of each item take scale / shift,
+  // the others scale_b / shift_b): e4m3 rows into q8 while FP8 is on, bf16 rows into xn when FP8 is off or an adapter
+  // on one of those linears reads them (FP8 mode 2)
+  auto ln_modulate = [&](const bf16_t* scale, const bf16_t* shift, int split_row, const bf16_t* scale_b,
+                         const bf16_t* shift_b, bool adapted) {
+    if (f8) {
+      const int r = b2f_ln_modulate_fp8(hb, d, h_bs, scale, shift, mod_ld, q8, 5 * d, q8_bs, qs, S, B, S, (int)d, eps,
+                                        split_row, scale_b, shift_b, st);
+      if (r || !adapted) return r;
+    }
+    return b2f_ln_modulate(hb, d, h_bs, scale, shift, mod_ld, xn, d, h_bs, B, S, (int)d, eps, split_row, scale_b,
+                           shift_b, st);
+  };
   int rc;
 #define RUN(expr) \
   if ((rc = (expr)) != 0) return rc
@@ -662,13 +686,7 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
       const bf16_t* mi = modp + (int64_t)blk * 12 * d;
       const bf16_t* mt = mi + 6 * d;
       // both streams in one launch over the joint buffer: text rows use the context modulation
-      if (f8) {
-        RUN(b2f_ln_modulate_fp8(hb, d, h_bs, mt + d, mt, mod_ld, q8, 5 * d, q8_bs, qs, S, B, S, (int)d, eps, S_txt,
-                                mi + d, mi, st));
-      }
-      if (!f8 || w.qkv.lora.A || w.add_qkv.lora.A) {   // FP8 mode 2: the bf16 rows an adapter's down projection reads
-        RUN(b2f_ln_modulate(hb, d, h_bs, mt + d, mt, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt, mi + d, mi, st));
-      }
+      RUN(ln_modulate(mt + d, mt, S_txt, mi + d, mi, w.qkv.lora.A || w.add_qkv.lora.A));
       // QKV projections with per-head RMSNorm + RoPE fused into the GEMM epilogue; both streams write
       // straight into the joint [txt; img] qkv buffer
       RUN(qkv_fwd(w.qkv, tb, ls, xn_img, d, h_bs, d, qkv_img, 3 * d, qkv_bs, B, S_img, (int)d,
@@ -683,14 +701,7 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
                     (int)d, (int)d, B2F_EPI_GATE_RESID, h_img, d, h_bs, mi + 2 * d, mod_ld, st, qi));
       RUN(lin_fwd(w.to_add_out, tb, ls, cat_txt, 5 * d, cat_bs, d, h_txt, d, h_bs, B,
                     S_txt, (int)d, (int)d, B2F_EPI_GATE_RESID, h_txt, d, h_bs, mt + 2 * d, mod_ld, st, qt));
-      if (f8) {
-        RUN(b2f_ln_modulate_fp8(hb, d, h_bs, mt + 4 * d, mt + 3 * d, mod_ld, q8, 5 * d, q8_bs, qs, S, B, S, (int)d, eps,
-                                S_txt, mi + 4 * d, mi + 3 * d, st));
-      }
-      if (!f8 || w.ff1.lora.A || w.ffc1.lora.A) {
-        RUN(b2f_ln_modulate(hb, d, h_bs, mt + 4 * d, mt + 3 * d, mod_ld, xn, d, h_bs, B, S, (int)d, eps, S_txt,
-                            mi + 4 * d, mi + 3 * d, st));
-      }
+      RUN(ln_modulate(mt + 4 * d, mt + 3 * d, S_txt, mi + 4 * d, mi + 3 * d, w.ff1.lora.A || w.ffc1.lora.A));
       RUN(lin_fwd(w.ff1, tb, ls, xn_img, d, h_bs, d, cat_img + d, 5 * d, cat_bs, B, S_img,
                     (int)(4 * d), (int)d, B2F_EPI_GELU_TANH, nullptr, 0, 0, nullptr, 0, st, qi));
       RUN(lin_fwd(w.ffc1, tb, ls, xn_txt, d, h_bs, d, cat_txt + d, 5 * d, cat_bs, B, S_txt,
@@ -705,13 +716,7 @@ int flux_forward(FluxCtx* c, const void* hidden, const void* enc, const void* mo
       const SingleW& w = c->sgl[si];
       // mod columns: [shift, scale, gate]
       const bf16_t* ms = modp + (int64_t)g.num_double * 12 * d + (int64_t)si * 3 * d;
-      if (f8) {
-        RUN(b2f_ln_modulate_fp8(hb, d, h_bs, ms + d, ms, mod_ld, q8, 5 * d, q8_bs, qs, S, B, S, (int)d, eps, 0, nullptr,
-                                nullptr, st));
-      }
-      if (!f8 || w.qkv_mlp.lora.A) {
-        RUN(b2f_ln_modulate(hb, d, h_bs, ms + d, ms, mod_ld, xn, d, h_bs, B, S, (int)d, eps, 0, nullptr, nullptr, st));
-      }
+      RUN(ln_modulate(ms + d, ms, 0, nullptr, nullptr, w.qkv_mlp.lora.A));
       // ONE launch for [to_q;to_k;to_v;proj_mlp] (N = 7d): Q/K get RMSNorm+RoPE, V passes through into
       // qkv, the MLP columns are GELU'd straight into cat[:, :, d:5d]
       RUN(qkv_fwd(w.qkv_mlp, tb, ls, xn, d, h_bs, d, qkv, 3 * d, qkv_bs, B, S, (int)d, (int)d,

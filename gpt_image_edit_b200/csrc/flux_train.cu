@@ -25,11 +25,9 @@ namespace b2f {
 
 namespace {
 
-inline size_t al256(size_t n) { return (n + 255) & ~size_t(255); }
-
 // carve-up of the training workspace (all offsets 256-byte aligned)
 struct TrainWs {
-  size_t infer_bytes;      // workspace of b2f_flux_forward (h | xn | qkv | cat), at offset 0
+  FwdWs fwd;               // workspace of b2f_flux_forward, at offset 0
   bf16_t *ckpt;            // [(nblocks + 1), B, S, d]
   bf16_t *hin, *xn, *pre, *qkv, *cat, *y1, *h1, *xn2, *y2;   // recompute buffers (pre: [B,S,7d], qkv: [B,S,3d], cat: [B,S,5d])
   bf16_t *dh, *dy, *dxn, *dpre, *dattn;                      // gradients (dpre: [B,S,7d])
@@ -37,14 +35,14 @@ struct TrainWs {
   size_t total;
 };
 
-TrainWs carve(const FluxCtx* c, void* ws, int B, int S_img, int S_txt, size_t infer_bytes) {
+TrainWs carve(const FluxCtx* c, void* ws, int B, int S_img, int S_txt) {
   const size_t S = (size_t)S_img + S_txt, d = c->d, BS = (size_t)B * S;
   const size_t nblk = (size_t)c->cfg.num_double + c->cfg.num_single;
   const size_t S_pad = (S + 127) / 128 * 128;
   TrainWs w{};
-  uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255));
-  size_t off = al256(infer_bytes);
-  w.infer_bytes = infer_bytes;
+  uint8_t* base = al256(ws);
+  w.fwd = fwd_ws(c, ws, B, S_img, S_txt);
+  size_t off = al256(w.fwd.bytes);
   auto take = [&](size_t elems, size_t esz) {
     uint8_t* p = base ? base + off : nullptr;
     off += al256(elems * esz);
@@ -117,8 +115,7 @@ int b2f_flux_bind_grad(b2f_flux* h, const char* key, float* dptr, int64_t numel)
 size_t b2f_flux_train_workspace_bytes(const b2f_flux* h, int B, int S_img, int S_txt) {
   const FluxCtx* c = reinterpret_cast<const FluxCtx*>(h);
   if (!c || B <= 0 || S_img <= 0 || S_txt <= 0) return 0;
-  const size_t infer = b2f_flux_workspace_bytes(h, B, S_img, S_txt);
-  return carve(c, nullptr, B, S_img, S_txt, infer).total;
+  return carve(c, nullptr, B, S_img, S_txt).total;
 }
 
 int b2f_flux_train_forward(b2f_flux* h, const void* hidden, const void* enc, const void* mod, int64_t mod_ld, void* out,
@@ -139,12 +136,10 @@ int b2f_flux_train_forward(b2f_flux* h, const void* hidden, const void* enc, con
   }
   if (ws_bytes < b2f_flux_train_workspace_bytes(h, B, S_img, S_txt)) return B2F_ERR_WORKSPACE;
   cudaStream_t st = static_cast<cudaStream_t>(stream_);
-  const size_t infer = b2f_flux_workspace_bytes(h, B, S_img, S_txt);
-  TrainWs w = carve(c, ws, B, S_img, S_txt, infer);
+  TrainWs w = carve(c, ws, B, S_img, S_txt);
   const int nblk = c->cfg.num_double + c->cfg.num_single;
-  const size_t S = (size_t)S_img + S_txt, hbytes = (size_t)B * S * c->d * 2;
-  // the inference workspace starts with h[B,S,d] (flux_model.cu); same 256-byte alignment rule as there
-  bf16_t* hb = reinterpret_cast<bf16_t*>((reinterpret_cast<uintptr_t>(ws) + 255) & ~uintptr_t(255));
+  const size_t S = (size_t)S_img + S_txt, hbytes = (size_t)B * S * c->d * 2, infer = w.fwd.bytes;
+  bf16_t* hb = w.fwd.h;
   int rc = b2f_flux_forward(h, hidden, enc, mod, mod_ld, out, B, S_img, S_txt, n_out_rows, ws, infer, 0, 0, stream_);
   if (rc) return rc;
   for (int blk = 0; blk < nblk; ++blk) {
@@ -182,7 +177,7 @@ int b2f_flux_train_backward(b2f_flux* h, const void* dout, const void* mod, int6
   if (last_block == nblk && !dout) return B2F_ERR_INVALID;
   const float eps = 1e-6f, scale = 1.0f / sqrtf((float)g.head_dim);
   const int64_t S_pad = (S + 127) / 128 * 128;
-  TrainWs w = carve(c, ws, B, S_img, S_txt, b2f_flux_workspace_bytes(h, B, S_img, S_txt));
+  TrainWs w = carve(c, ws, B, S_img, S_txt);
   const int64_t BS = (int64_t)B * S;
   const int64_t bs1 = (int64_t)S * d, bs3 = 3 * bs1, bs5 = 5 * bs1, bs7 = 7 * bs1;
   const bf16_t* modp = static_cast<const bf16_t*>(mod);
@@ -419,7 +414,7 @@ int b2f_flux_train_backward(b2f_flux* h, const void* dout, const void* mod, int6
 int b2f_flux_train_debug_dh(b2f_flux* h, void* dst, int B, int S_img, int S_txt, void* ws, b2f_stream_t stream_) {
   FluxCtx* c = reinterpret_cast<FluxCtx*>(h);
   if (!c || !dst || !ws) return B2F_ERR_INVALID;
-  TrainWs w = carve(c, ws, B, S_img, S_txt, b2f_flux_workspace_bytes(h, B, S_img, S_txt));
+  TrainWs w = carve(c, ws, B, S_img, S_txt);
   const size_t n = (size_t)B * (S_img + S_txt) * c->d * 2;
   return cuda_err(cudaMemcpyAsync(dst, w.dh, n, cudaMemcpyDeviceToDevice, static_cast<cudaStream_t>(stream_)), "dh copy");
 }

@@ -51,6 +51,13 @@ inline int cuda_err(cudaError_t e, const char* what) {
   return B2F_ERR_CUDA;
 }
 
+// Workspace carving: sizes and pointers rounded up to 256 bytes (a null pointer stays null).
+inline size_t al256(size_t n) { return (n + 255) & ~size_t(255); }
+template <class T = uint8_t>
+inline T* al256(void* p) {
+  return reinterpret_cast<T*>(al256(reinterpret_cast<uintptr_t>(p)));
+}
+
 // Kernels launched since load (b2f_launch_count).
 extern std::atomic<uint64_t> g_launch_count;
 

@@ -18,7 +18,7 @@ from types import SimpleNamespace
 
 import torch
 
-from . import _lib
+from . import _lib, flux_layout
 from ._lib import check, ptr, stream_ptr
 from .lora import FluxLoraMixin
 
@@ -87,63 +87,20 @@ class _CacheState:
         self.mem = None
 
 
-def _fused_layout(cfg: FluxTransformerConfig):
-    """fused name -> list of (diffusers linear name, out_features); plus plain names."""
-    d = cfg.num_attention_heads * cfg.attention_head_dim
-    fused: "OrderedDict[str, list]" = OrderedDict()
-    adaln = []
-    for i in range(cfg.num_layers):
-        p = f"transformer_blocks.{i}."
-        adaln += [(p + "norm1.linear", 6 * d), (p + "norm1_context.linear", 6 * d)]
-        fused[p + "attn.qkv"] = [(p + "attn.to_q", d), (p + "attn.to_k", d), (p + "attn.to_v", d)]
-        fused[p + "attn.add_qkv"] = [(p + "attn.add_q_proj", d), (p + "attn.add_k_proj", d), (p + "attn.add_v_proj", d)]
-    for i in range(cfg.num_single_layers):
-        p = f"single_transformer_blocks.{i}."
-        adaln += [(p + "norm.linear", 3 * d)]
-        fused[p + "qkv_mlp"] = [(p + "attn.to_q", d), (p + "attn.to_k", d), (p + "attn.to_v", d), (p + "proj_mlp", 4 * d)]
-    adaln += [("norm_out.linear", 2 * d)]
-    fused["adaln"] = adaln
-    return fused
-
-
-def _plain_linears(cfg: FluxTransformerConfig):
-    d = cfg.num_attention_heads * cfg.attention_head_dim
-    out = [("x_embedder", d, cfg.in_channels), ("context_embedder", d, cfg.joint_attention_dim),
-           ("time_text_embed.timestep_embedder.linear_1", d, 256), ("time_text_embed.timestep_embedder.linear_2", d, d)]
-    if cfg.guidance_embeds:
-        out += [("time_text_embed.guidance_embedder.linear_1", d, 256), ("time_text_embed.guidance_embedder.linear_2", d, d)]
-    out += [("time_text_embed.text_embedder.linear_1", d, cfg.pooled_projection_dim),
-            ("time_text_embed.text_embedder.linear_2", d, d), ("proj_out", cfg.out_channels, d)]
-    for i in range(cfg.num_layers):
-        p = f"transformer_blocks.{i}."
-        out += [(p + "attn.to_out.0", d, d), (p + "attn.to_add_out", d, d), (p + "ff.net.0.proj", 4 * d, d),
-                (p + "ff.net.2", d, 4 * d), (p + "ff_context.net.0.proj", 4 * d, d), (p + "ff_context.net.2", d, 4 * d)]
-    for i in range(cfg.num_single_layers):
-        out += [(f"single_transformer_blocks.{i}.proj_out", d, 5 * d)]
-    return out
-
-
-def _fp8_linears(cfg: FluxTransformerConfig):
-    """bound names of the block linears that run in FP8 once enable_fp8() is called (b2f_flux_bind_fp8)."""
-    out = []
-    for i in range(cfg.num_layers):
-        p = f"transformer_blocks.{i}."
-        out += [p + n for n in ("attn.qkv", "attn.add_qkv", "attn.to_out.0", "attn.to_add_out", "ff.net.0.proj",
-                                "ff.net.2", "ff_context.net.0.proj", "ff_context.net.2")]
-    for i in range(cfg.num_single_layers):
-        out += [f"single_transformer_blocks.{i}.qkv_mlp", f"single_transformer_blocks.{i}.proj_out"]
-    return out
-
-
-def _norm_weights(cfg: FluxTransformerConfig):
-    out = []
-    for i in range(cfg.num_layers):
-        p = f"transformer_blocks.{i}.attn."
-        out += [p + "norm_q.weight", p + "norm_k.weight", p + "norm_added_q.weight", p + "norm_added_k.weight"]
-    for i in range(cfg.num_single_layers):
-        p = f"single_transformer_blocks.{i}.attn."
-        out += [p + "norm_q.weight", p + "norm_k.weight"]
-    return out
+def _storage(cfg: FluxTransformerConfig):
+    """Every stored linear as (bound name, out, in, views) in allocation order, which is the order randomize_ draws
+    them in; views: (diffusers name, row0, rows).  The fused block linears, the fused AdaLN weight, the embedders and
+    proj_out, the other block linears."""
+    lay = flux_layout.layout(cfg)
+    adaln = [t for t in lay if t.kind == "adaln"]
+    row0 = [sum(t.out for t in adaln[:j]) for j in range(len(adaln))]
+    # the embedders are allocated with guidance before text, proj_out last
+    emb = sorted((t for t in lay if t.kind == "embedder"),
+                 key=lambda t: (".text_embedder." in t.name) + 2 * (t.name == "proj_out"))
+    return ([(t.name, t.out, t.inp, t.parts) for t in lay if len(t.parts) > 1]
+            + [("adaln", sum(t.out for t in adaln), adaln[0].inp, tuple((t.name, r, t.out) for t, r in zip(adaln, row0)))]
+            + [(t.name, t.out, t.inp, t.parts) for t in emb]
+            + [(t.name, t.out, t.inp, t.parts) for t in lay if t.kind == "block" and len(t.parts) == 1])
 
 
 def text_windows(mask: torch.Tensor, B: int, S_txt: int) -> torch.Tensor:
@@ -165,23 +122,17 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         dev = torch.device(device)
         if dev.type != "cuda":
             raise _lib.B2FError("B200FluxTransformer2DModel lives on a CUDA device; there is no CPU path")
-        self.inner_dim = d = cfg.num_attention_heads * cfg.attention_head_dim
+        self.inner_dim = cfg.num_attention_heads * cfg.attention_head_dim
         self._store: "OrderedDict[str, torch.Tensor]" = OrderedDict()   # bound name -> storage tensor
         self._views: "OrderedDict[str, torch.Tensor]" = OrderedDict()   # diffusers name -> view
         mk = lambda *shape: torch.zeros(shape, device=dev, dtype=torch.bfloat16)
-        for fname, parts in _fused_layout(cfg).items():
-            rows = sum(n for _, n in parts)
-            w, b = mk(rows, d), mk(rows)
-            self._store[fname + ".weight"], self._store[fname + ".bias"] = w, b
-            r = 0
-            for name, n in parts:
-                self._views[name + ".weight"], self._views[name + ".bias"] = w[r:r + n], b[r:r + n]
-                r += n
-        for name, o, i in _plain_linears(cfg):
+        for name, o, i, views in _storage(cfg):
             w, b = mk(o, i), mk(o)
             self._store[name + ".weight"], self._store[name + ".bias"] = w, b
-            self._views[name + ".weight"], self._views[name + ".bias"] = w, b
-        for name in _norm_weights(cfg):
+            for v, r, n in views:
+                self._views[v + ".weight"], self._views[v + ".bias"] = (w, b) if len(views) == 1 else (w[r:r + n],
+                                                                                                    b[r:r + n])
+        for name in flux_layout.norm_weights(cfg):
             w = torch.ones(cfg.attention_head_dim, device=dev, dtype=torch.bfloat16)
             self._store[name] = w
             self._views[name] = w
@@ -339,7 +290,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
         if self._lora_bound and mode != 2:
             raise _lib.B2FError("enable_fp8: unfused LoRA adapters are active; fuse_lora() them first")
         fp8 = OrderedDict()
-        for name in _fp8_linears(self.config):
+        for name in (t.name for t in flux_layout.layout(self.config) if t.kind == "block"):
             w = self._store[name + ".weight"]
             fp8[name] = (torch.empty(w.shape, device=w.device, dtype=torch.float8_e4m3fn),
                          torch.empty(w.shape[0], device=w.device, dtype=torch.float32))
@@ -604,10 +555,7 @@ class B200FluxTransformer2DModel(FluxLoraMixin, torch.nn.Module):
     def debug_hidden(self, B: int, S_img: int, S_txt: int) -> torch.Tensor:
         """View of the joint activation buffer h[B, S_txt+S_img, d] inside the workspace (block-level
         parity tests read it after a partial-range forward)."""
-        ws = self._ws["fwd"]
-        off = (-ws.data_ptr()) % 256
-        n = B * (S_img + S_txt) * self.inner_dim
-        return ws[off:off + 2 * n].view(torch.bfloat16).view(B, S_img + S_txt, self.inner_dim)
+        return self.debug_buffers(B, S_img, S_txt).h
 
     def debug_buffers(self, B: int, S_img: int, S_txt: int) -> SimpleNamespace:
         """Views of the whole forward workspace in b2f_flux_forward's layout (text rows first): h and xn [B, S, d],

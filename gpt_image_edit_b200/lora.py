@@ -34,6 +34,7 @@ from dataclasses import dataclass
 import torch
 
 from ._lib import B2FError
+from .flux_layout import layout
 
 
 # ------------------------------------------------------------------------------------------------ targets
@@ -49,55 +50,18 @@ class Part:
 
 def targets(cfg) -> "OrderedDict[str, tuple[int, int]]":
     """engine target name -> (out_features, in_features), in the engine's order."""
-    d = cfg.num_attention_heads * cfg.attention_head_dim
-    t: "OrderedDict[str, tuple[int, int]]" = OrderedDict()
-    t["x_embedder"] = (d, cfg.in_channels)
-    t["context_embedder"] = (d, cfg.joint_attention_dim)
-    embs = ["timestep_embedder", "text_embedder"] + (["guidance_embedder"] if cfg.guidance_embeds else [])
-    for e in embs:
-        t[f"time_text_embed.{e}.linear_1"] = (d, cfg.pooled_projection_dim if e == "text_embedder" else 256)
-        t[f"time_text_embed.{e}.linear_2"] = (d, d)
-    for i in range(cfg.num_layers):
-        p = f"transformer_blocks.{i}."
-        for n, o, k in (("attn.qkv", 3 * d, d), ("attn.add_qkv", 3 * d, d), ("attn.to_out.0", d, d),
-                        ("attn.to_add_out", d, d), ("ff.net.0.proj", 4 * d, d), ("ff.net.2", d, 4 * d),
-                        ("ff_context.net.0.proj", 4 * d, d), ("ff_context.net.2", d, 4 * d),
-                        ("norm1.linear", 6 * d, d), ("norm1_context.linear", 6 * d, d)):
-            t[p + n] = (o, k)
-    for i in range(cfg.num_single_layers):
-        p = f"single_transformer_blocks.{i}."
-        t[p + "qkv_mlp"] = (7 * d, d)
-        t[p + "proj_out"] = (d, 5 * d)
-        t[p + "norm.linear"] = (3 * d, d)
-    t["norm_out.linear"] = (2 * d, d)
-    t["proj_out"] = (cfg.out_channels, d)
-    return t
+    return OrderedDict((t.name, (t.out, t.inp)) for t in layout(cfg))
 
 
 def adaln_targets(cfg) -> set:
-    return {n for n in targets(cfg) if n.endswith("norm1.linear") or n.endswith("norm1_context.linear")
-            or n.endswith(".norm.linear") or n == "norm_out.linear"}
+    return {t.name for t in layout(cfg) if t.kind == "adaln"}
 
 
 def diffusers_parts(cfg) -> "dict[str, Part]":
-    """diffusers module name -> Part (every nn.Linear of FluxTransformer2DModel)."""
-    d = cfg.num_attention_heads * cfg.attention_head_dim
-    out = {}
-    for name, (o, k) in targets(cfg).items():
-        if not name.endswith(("attn.qkv", "attn.add_qkv", "qkv_mlp")):
-            out[name] = Part(name, 0, o, k)
-    for i in range(cfg.num_layers):
-        p = f"transformer_blocks.{i}."
-        for j, n in enumerate(("to_q", "to_k", "to_v")):
-            out[p + "attn." + n] = Part(p + "attn.qkv", j * d, d, d)
-        for j, n in enumerate(("add_q_proj", "add_k_proj", "add_v_proj")):
-            out[p + "attn." + n] = Part(p + "attn.add_qkv", j * d, d, d)
-    for i in range(cfg.num_single_layers):
-        p = f"single_transformer_blocks.{i}."
-        for j, n in enumerate(("to_q", "to_k", "to_v")):
-            out[p + "attn." + n] = Part(p + "qkv_mlp", j * d, d, d)
-        out[p + "proj_mlp"] = Part(p + "qkv_mlp", 3 * d, 4 * d, d)
-    return out
+    """diffusers module name -> Part (every nn.Linear of FluxTransformer2DModel): the targets that are one linear,
+    then the parts of the fused ones."""
+    return {p: Part(t.name, r0, n, t.inp) for t in sorted(layout(cfg), key=lambda t: len(t.parts) > 1)
+            for p, r0, n in t.parts}
 
 
 def bfl_parts(cfg) -> "dict[str, Part]":
