@@ -27,6 +27,8 @@ using namespace attn;
 
 namespace {
 
+constexpr int ATTN_SMEM = FwdSmem<TILE_BYTES>::BYTES;
+
 // BIAS: additive bf16 score bias; the bias kernel folds the score scale into the bias step and runs with
 // scale_log2 = log2(e).
 // WIN: per-item text window p.win[b] = (lo, hi) over the first p.S_txt keys (non-causal, no bias).  The K/V blocks
@@ -39,17 +41,7 @@ __global__ void __launch_bounds__(ATTN_THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                 const __grid_constant__ CUtensorMap tmV, const AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
-  uint8_t* q_smem = smem;
-  uint8_t* k_smem = smem + TILE_BYTES;                      // KV_SLOTS tiles
-  uint8_t* v_smem = k_smem + KV_SLOTS * TILE_BYTES;         // KV_SLOTS tiles
-  uint64_t* bars = reinterpret_cast<uint64_t*>(v_smem + KV_SLOTS * TILE_BYTES);
-  uint64_t* q_full = bars;                 // 1
-  uint64_t* k_full = bars + 1;             // KV_SLOTS
-  uint64_t* k_empty = k_full + KV_SLOTS;
-  uint64_t* v_full = k_empty + KV_SLOTS;
-  uint64_t* v_empty = v_full + KV_SLOTS;
+  const FwdSmem<TILE_BYTES> sm(smem_raw);
 
   const int wg = __shfl_sync(0xffffffffu, int(threadIdx.x >> 7), 0);   // warp-uniform for the compiler
   const int h = blockIdx.y, b = blockIdx.z;
@@ -62,8 +54,9 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   // WIN: block j < n0 covers keys [lo + j BKV, ..) of the run ending at end0, block j >= n0 [S_txt + (j - n0) BKV, ..)
   int lo = 0, hi = 0, end0 = 0, n0 = 0;
   if (WIN) {
-    lo = min(max(p.win[2 * b], 0), p.S_txt);   // out-of-range windows are clamped, never read out of bounds
-    hi = min(max(p.win[2 * b + 1], lo), p.S_txt);
+    const int2 tw = text_window(p.win, b, p.S_txt);
+    lo = tw.x;
+    hi = tw.y;
     end0 = hi == p.S_txt ? p.Skv : hi;
     n0 = (end0 - lo + BKV - 1) / BKV;
     n_kv = n0 + (hi == p.S_txt ? 0 : (p.Skv - p.S_txt + BKV - 1) / BKV);
@@ -74,61 +67,48 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     tma_prefetch_desc(&tmQ);
     tma_prefetch_desc(&tmK);
     tma_prefetch_desc(&tmV);
-    mbar_init(q_full, 1);
-    for (int i = 0; i < KV_SLOTS; ++i) {
-      mbar_init(&k_full[i], 1);
-      mbar_init(&v_full[i], 1);
-      mbar_init(&k_empty[i], 8);   // one arrive per consumer warp
-      mbar_init(&v_empty[i], 8);
-    }
-    fence_mbar_init();
+    sm.init_barriers();
   }
   __syncthreads();
 
   if (wg == 0) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       // ---------------------------------------------------------------- TMA producer
-      mbar_expect_tx(q_full, TILE_BYTES);
+      mbar_expect_tx(sm.q_full, TILE_BYTES);
       for (int half = 0; half < 2; ++half)
-        tma_load_3d(q_smem + half * HALF_BYTES, &tmQ, q_full, h * DH + half * 64, q0, b);
-      for (int j = 0; j < n_kv; ++j) {
-        const int slot = j % KV_SLOTS;
-        const uint32_t phase = (j / KV_SLOTS) & 1;
-        mbar_wait(&k_empty[slot], phase ^ 1);
-        mbar_expect_tx(&k_full[slot], TILE_BYTES);
-        for (int half = 0; half < 2; ++half)
-          tma_load_3d(k_smem + slot * TILE_BYTES + half * HALF_BYTES, &tmK, &k_full[slot], hk * DH + half * 64,
-                      kv_start(j), b);
-        mbar_wait(&v_empty[slot], phase ^ 1);
-        mbar_expect_tx(&v_full[slot], TILE_BYTES);
-        for (int half = 0; half < 2; ++half)
-          tma_load_3d(v_smem + slot * TILE_BYTES + half * HALF_BYTES, &tmV, &v_full[slot], hk * DH + half * 64,
-                      kv_start(j), b);
-      }
+        tma_load_3d(sm.q + half * HALF_BYTES, &tmQ, sm.q_full, h * DH + half * 64, q0, b);
+      // K / V block j: two 64-column halves of the 128 rows from kv_start(j)
+      sm.produce_kv(
+          n_kv,
+          [&](int j, uint8_t* dst, uint64_t* bar) {
+            for (int half = 0; half < 2; ++half)
+              tma_load_3d(dst + half * HALF_BYTES, &tmK, bar, hk * DH + half * 64, kv_start(j), b);
+          },
+          [&](int j, uint8_t* dst, uint64_t* bar) {
+            for (int half = 0; half < 2; ++half)
+              tma_load_3d(dst + half * HALF_BYTES, &tmV, bar, hk * DH + half * 64, kv_start(j), b);
+          });
     }
     return;
   }
 
   // ------------------------------------------------------------------ consumer warpgroups
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
-  const int c = wg - 1;
-  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  const int row0 = q0 + c * 64 + w * 16 + (lane >> 2);   // this thread's rows: row0 and row0 + 8
-  const int colq = 2 * (lane & 3);                       // first of its two columns in every 8-column group
-  const uint64_t dq0 = make_sdesc_sw128(smem_u32(q_smem) + c * 8192, 16, 1024);
-  const uint64_t dk0 = make_sdesc_sw128(smem_u32(k_smem), 16, 1024);
-  const uint64_t dv0 = make_sdesc_sw128(smem_u32(v_smem), HALF_BYTES, 1024);
+  setmaxnreg_inc<CONSUMER_REGS>();
+  const auto [c, w, lane, row0, colq] = consumer_pos(wg, q0);
+  const uint64_t dq0 = make_sdesc_sw128(smem_u32(sm.q) + c * 8192, 16, 1024);
+  const uint64_t dk0 = make_sdesc_sw128(smem_u32(sm.k), 16, 1024);
+  const uint64_t dv0 = make_sdesc_sw128(smem_u32(sm.v), HALF_BYTES, 1024);
   float o[64];
 #pragma unroll
   for (int i = 0; i < 64; ++i) o[i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};   // l: this thread's partial row sums
-  mbar_wait(q_full, 0);
+  mbar_wait(sm.q_full, 0);
   for (int j = 0; j < n_kv; ++j) {
     const int slot = j % KV_SLOTS;
     const uint32_t phase = (j / KV_SLOTS) & 1;
     float s[64];
-    mbar_wait(&k_full[slot], phase);
+    mbar_wait(&sm.k_full[slot], phase);
     wgmma_fence();
 #pragma unroll
     for (int k = 0; k < DH / 16; ++k) {
@@ -138,15 +118,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(s);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&k_empty[slot]);
+    consumer_release(&sm.k_empty[slot], lane);
 
     const int kv0 = kv_start(j);
     if (BIAS) {
 #pragma unroll
       for (int i = 0; i < 64; ++i) {
-        const int row = row0 + 8 * ((i >> 1) & 1);
-        const int col = kv0 + 8 * (i >> 2) + colq + (i & 1);
+        const int row = row0 + acc_row(i);
+        const int col = kv0 + acc_col(i, colq);
         if (row < p.Sq && col < p.Skv)
           s[i] = fmaf(s[i], p.bias_scale,
                       __bfloat162float(p.bias[(long long)h * p.bias_h_stride + (long long)row * p.bias_row_stride + col]));
@@ -157,41 +136,19 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       if (kv0 + BKV > kv_end) {
 #pragma unroll
         for (int i = 0; i < 64; ++i)
-          if (kv0 + 8 * (i >> 2) + colq + (i & 1) >= kv_end) s[i] = -INFINITY;
+          if (kv0 + acc_col(i, colq) >= kv_end) s[i] = -INFINITY;
       }
     } else if (kv0 + BKV > p.Skv || p.causal) {
 #pragma unroll
       for (int i = 0; i < 64; ++i) {
-        const int row = row0 + 8 * ((i >> 1) & 1);
-        const int col = kv0 + 8 * (i >> 2) + colq + (i & 1);
-        const int limit = p.causal ? min(p.Skv, row + 1) : p.Skv;
-        if (col >= limit) s[i] = -INFINITY;
+        const int limit = p.causal ? min(p.Skv, row0 + acc_row(i) + 1) : p.Skv;
+        if (kv0 + acc_col(i, colq) >= limit) s[i] = -INFINITY;
       }
     }
-    float alpha[2], neg_m[2];
+    float alpha[2];
+    softmax_step<0>(s, m, l, p.scale_log2, alpha);
 #pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      float mx = -INFINITY;
-#pragma unroll
-      for (int i = 0; i < 64; ++i)
-        if (((i >> 1) & 1) == r) mx = fmaxf(mx, s[i]);
-      mx = quad_max(mx);
-      const float m_new = fmaxf(m[r], mx * p.scale_log2);
-      alpha[r] = m[r] == -INFINITY ? 0.f : ex2(m[r] - m_new);
-      neg_m[r] = m_new == -INFINITY ? 0.f : -m_new;   // fully masked row so far
-      m[r] = m_new;
-    }
-    float sum[2] = {0.f, 0.f};
-#pragma unroll
-    for (int i = 0; i < 64; ++i) {
-      const int r = (i >> 1) & 1;
-      s[i] = ex2(fmaf(s[i], p.scale_log2, neg_m[r]));
-      sum[r] += s[i];
-    }
-#pragma unroll
-    for (int r = 0; r < 2; ++r) l[r] = l[r] * alpha[r] + sum[r];
-#pragma unroll
-    for (int i = 0; i < 64; ++i) o[i] *= alpha[(i >> 1) & 1];
+    for (int i = 0; i < 64; ++i) o[i] *= alpha[acc_row(i) / 8];
 
     uint32_t pa[BKV / 16][4];
 #pragma unroll
@@ -202,14 +159,14 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
       // of both swizzled halves) before either multiplies.  Rows from S_txt on are image rows (finite) and rows past
       // Skv arrive as TMA zero fill.
       const int z0 = hi - kv0, z1 = min(p.S_txt - kv0, BKV);
-      mbar_wait(&v_full[slot], phase);
-      uint8_t* vt = v_smem + slot * TILE_BYTES;
+      mbar_wait(&sm.v_full[slot], phase);
+      uint8_t* vt = sm.v + slot * TILE_BYTES;
       for (int i = z0 * 16 + (int(threadIdx.x) - 128); i < z1 * 16; i += 256)
         *reinterpret_cast<uint4*>(vt + (i & 8) / 8 * HALF_BYTES + (i >> 4) * 128 + (i & 7) * 16) = make_uint4(0, 0, 0, 0);
       fence_proxy_async_smem();
       named_bar_sync(1, 256);
     }
-    mbar_wait(&v_full[slot], phase);
+    mbar_wait(&sm.v_full[slot], phase);
     reg_fence(o);
     wgmma_fence();
 #pragma unroll
@@ -218,8 +175,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     wgmma_commit();
     wgmma_wait<0>();
     reg_fence(o);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&v_empty[slot]);
+    consumer_release(&sm.v_empty[slot], lane);
   }
 
   // ---------------------------------------------------------------- epilogue: O / l -> bf16
@@ -230,12 +186,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     const float inv_l = 1.0f / lt;
     if (row >= p.Sq) continue;
     if (p.lse && (lane & 3) == 0) p.lse[((long long)b * p.H + h) * p.lse_stride + row] = m[r] + log2f(lt);
-    __nv_bfloat16* out_row = p.out + ((long long)b * p.Sq + row) * p.ldo + (long long)h * DH;
-#pragma unroll
-    for (int jj = 0; jj < 16; ++jj) {
-      const int i = 4 * jj + 2 * r;
-      *reinterpret_cast<uint32_t*>(out_row + 8 * jj + colq) = pack_bf16x2(o[i] * inv_l, o[i + 1] * inv_l);
-    }
+    store_row_bf16(p.out + ((long long)b * p.Sq + row) * p.ldo + (long long)h * DH, o, r, colq, inv_l);
   }
 }
 
@@ -258,16 +209,9 @@ static int attention_impl(const void* q, int64_t ldq, const void* k, int64_t ldk
        reinterpret_cast<uintptr_t>(v) | reinterpret_cast<uintptr_t>(out)) & 15)
     return B2F_ERR_ALIGN;
   static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_fwd_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         ATTN_SMEM);
-    if (e != cudaSuccess) return cuda_err(e, "attention smem attribute");
-    e = cudaFuncSetAttribute(attn_fwd_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM);
-    if (e != cudaSuccess) return cuda_err(e, "attention smem attribute");
-    e = cudaFuncSetAttribute(attn_fwd_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, ATTN_SMEM);
-    if (e != cudaSuccess) return cuda_err(e, "attention smem attribute");
-    attr_set = true;
-  }
+  if (int rc = set_max_smem_once(attr_set, ATTN_SMEM, "attention smem attribute", attn_fwd_kernel<false, false>,
+                                 attn_fwd_kernel<true, false>, attn_fwd_kernel<false, true>))
+    return rc;
   CUtensorMap tmQ, tmK, tmV;
   int rc = make_tmap_3d_rows(&tmQ, q, (uint64_t)H * DH, Sq, B, ldq, (uint64_t)Sq * ldq);
   if (rc) return rc;

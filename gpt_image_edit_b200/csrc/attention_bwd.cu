@@ -84,7 +84,7 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_constant_
   __syncthreads();
 
   if (wg == 0) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;");
+    setmaxnreg_dec<PRODUCER_REGS>();
     if (threadIdx.x == 0) {
       // ---------------------------------------------------------------- TMA producer
       mbar_expect_tx(x_full, 2 * TILE_BYTES);
@@ -115,11 +115,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_constant_
   }
 
   // ------------------------------------------------------------------ consumer warpgroups
-  asm volatile("setmaxnreg.inc.sync.aligned.u32 240;");
-  const int c = wg - 1;
-  const int w = (threadIdx.x >> 5) & 3, lane = threadIdx.x & 31;
-  const int row0 = row0_cta + c * 64 + w * 16 + (lane >> 2);   // this thread's stationary rows: row0, row0 + 8
-  const int colq = 2 * (lane & 3);
+  setmaxnreg_inc<CONSUMER_REGS>();
+  const auto [c, w, lane, row0, colq] = consumer_pos(wg, row0_cta);   // stationary rows row0, row0 + 8
   const uint64_t dx0 = make_sdesc_sw128(smem_u32(x_smem) + c * 8192, 16, 1024);
   const uint64_t dx1 = dx0 + uint64_t(TILE_BYTES >> 4);
   const uint64_t dyk = make_sdesc_sw128(smem_u32(y_smem), 16, 1024);        // K-major view of a Y block
@@ -161,8 +158,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_constant_
     const float* dl_s = lse_s + BS;
 #pragma unroll
     for (int i = 0; i < 32; ++i) {
-      const int r = (i >> 1) & 1;
-      const int lc = 8 * (i >> 2) + colq + (i & 1);   // streamed index inside the block
+      const int r = acc_row(i) / 8;
+      const int lc = acc_col(i, colq);   // streamed index inside the block
       float l, d;
       if (MODE == 0) {
         l = lse_s[lc];
@@ -203,29 +200,16 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmX0, const __grid_constant_
     wgmma_wait<0>();
     reg_fence(g0);
     if (MODE == 0) reg_fence(g1);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&y_empty[stage]);
+    consumer_release(&y_empty[stage], lane);
   }
 
   // ---------------------------------------------------------------- epilogue: accumulators -> bf16 -> global
 #pragma unroll
-  for (int g = 0; g < (MODE == 0 ? 2 : 1); ++g) {
-    __nv_bfloat16* base = g == 0 ? p.g0 : p.g1;
-    const long long ld = g == 0 ? p.ld0 : p.ld1;
-    const float mul = g == 0 ? p.scale : 1.0f;
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      const int row = row0 + 8 * r;
-      if (row >= p.S) continue;
-      __nv_bfloat16* out_row = base + ((long long)b * p.S + row) * ld + (long long)h * DH;
-#pragma unroll
-      for (int jj = 0; jj < 16; ++jj) {
-        const int i = 4 * jj + 2 * r;
-        const float v0 = g == 0 ? g0[i] : g1[i];
-        const float v1 = g == 0 ? g0[i + 1] : g1[i + 1];
-        *reinterpret_cast<uint32_t*>(out_row + 8 * jj + colq) = pack_bf16x2(v0 * mul, v1 * mul);
-      }
-    }
+  for (int r = 0; r < 2; ++r) {
+    const int row = row0 + 8 * r;
+    if (row >= p.S) continue;
+    store_row_bf16(p.g0 + ((long long)b * p.S + row) * p.ld0 + (long long)h * DH, g0, r, colq, p.scale);
+    if (MODE == 0) store_row_bf16(p.g1 + ((long long)b * p.S + row) * p.ld1 + (long long)h * DH, g1, r, colq, 1.0f);
   }
 }
 
@@ -248,13 +232,9 @@ extern "C" int b2f_attention_bwd(const void* q, int64_t ldq, const void* k, int6
        reinterpret_cast<uintptr_t>(dv) | reinterpret_cast<uintptr_t>(lse) | reinterpret_cast<uintptr_t>(delta)) & 15)
     return B2F_ERR_ALIGN;
   static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(attn_bwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
-    if (e != cudaSuccess) return cuda_err(e, "attention bwd smem attribute");
-    e = cudaFuncSetAttribute(attn_bwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, BWD_SMEM);
-    if (e != cudaSuccess) return cuda_err(e, "attention bwd smem attribute");
-    attr_set = true;
-  }
+  if (int rc = set_max_smem_once(attr_set, BWD_SMEM, "attention bwd smem attribute", attn_bwd_kernel<0>,
+                                 attn_bwd_kernel<1>))
+    return rc;
   // every operand as a stationary tile (128-row boxes) and as a streamed block (64-row boxes)
   CUtensorMap tQ, tK, tV, tO, sQ, sK, sV, sO;
   const void* src[4] = {q, k, v, dout};

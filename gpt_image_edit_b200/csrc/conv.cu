@@ -163,11 +163,7 @@ conv3x3_kernel(const __grid_constant__ CUtensorMap tmIn, const __grid_constant__
 
 int launch_conv(const CUtensorMap& tmIn, const CUtensorMap& tmW, ConvParams p, cudaStream_t stream) {
   static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv3x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM_BYTES);
-    if (e != cudaSuccess) return cuda_err(e, "conv smem attribute");
-    attr_set = true;
-  }
+  if (int rc = set_max_smem_once(attr_set, SMEM_BYTES, "conv smem attribute", conv3x3_kernel)) return rc;
   p.num_n_blocks = (p.Cout + BLOCK_N - 1) / BLOCK_N;
   const int num_tiles = p.num_m_blocks * p.num_n_blocks;
   prof_begin(KC_CONV, stream);

@@ -8,29 +8,6 @@ namespace b2f {
 
 namespace {
 
-__device__ __forceinline__ void unpack8(const uint4& q, float* f) {
-  const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 t = unpack_bf16x2(w[j]);
-    f[2 * j] = t.x;
-    f[2 * j + 1] = t.y;
-  }
-}
-__device__ __forceinline__ uint4 pack8(const float* f) {
-  uint4 q;
-  q.x = pack_bf16x2(f[0], f[1]);
-  q.y = pack_bf16x2(f[2], f[3]);
-  q.z = pack_bf16x2(f[4], f[5]);
-  q.w = pack_bf16x2(f[6], f[7]);
-  return q;
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 // ------------------------------------------------------------------------------------------------
 // AdaLN modulate:  y = bf16( bf16( bf16(LN(x)) * bf16(1 + scale[b]) ) + shift[b] )
 // LN: no affine, eps, biased variance, fp32 statistics (torch.nn.functional.layer_norm on bf16).
@@ -57,12 +34,6 @@ struct LnModParams {
   float* row_scale;
   long long row_scale_bs;
 };
-
-__device__ __forceinline__ float warp_max(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, o));
-  return v;
-}
 
 // One warp per row, rows taken grid-stride.  The row stays PACKED in registers (MAXC uint4 per lane, 48 registers
 // for D = 3072) and is unpacked again in each of the three passes (sum, centred sum of squares, output): with the

@@ -14,6 +14,7 @@
 
 #include "flux_ctx.h"
 #include "host_common.h"
+#include "ptx.cuh"
 
 namespace b2f {
 
@@ -21,16 +22,6 @@ namespace {
 
 constexpr int kThreads = 256;
 constexpr int kRowsPerCta = 8;   // rows of d elements per CTA of the residual pass: fixes the partials' order
-
-__device__ __forceinline__ void unpack8(const uint4& u, float* f) {
-  const __nv_bfloat162* p = reinterpret_cast<const __nv_bfloat162*>(&u);
-#pragma unroll
-  for (int i = 0; i < 4; ++i) {
-    const float2 v = __bfloat1622float2(p[i]);
-    f[2 * i] = v.x;
-    f[2 * i + 1] = v.y;
-  }
-}
 
 // Fixed-shape tree over kThreads doubles in shared memory; the result lands in s[0].
 __device__ __forceinline__ void tree_sum(double* s) {

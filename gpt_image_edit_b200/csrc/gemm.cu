@@ -183,16 +183,6 @@ __device__ __forceinline__ void epilogue_group(const int epi, float (&v)[8], con
   *reinterpret_cast<uint4*>(out) = o;
 }
 
-__device__ __forceinline__ void unpack_bf16x8(const uint4 q, float (&v)[8]) {
-  const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 f = unpack_bf16x2(w[j]);
-    v[2 * j] = f.x;
-    v[2 * j + 1] = f.y;
-  }
-}
-
 // One 128-column head of a fused QKV projection for one token, from its row of the staged tile x = bf16(acc + bias):
 //   y = bf16(x * rsqrt(mean(x^2) + eps));  z = bf16(y * w);
 //   out = bf16(z * cos + rot(z) * sin)        (diffusers RMSNorm + apply_rotary_emb, SURVEY.md A.2)
@@ -205,7 +195,9 @@ __device__ __forceinline__ void epilogue_head_norm_rope(const GemmParams& p, con
 #pragma unroll 4
   for (int g = 0; g < BLOCK_N / 8; ++g) {
     float x[8];
-    unpack_bf16x8(*reinterpret_cast<const uint4*>(srow + g * 16), x);
+    // uint4(...) unpacks a register copy (here and below): unpacking through a reference to the staged bytes changes
+    // this tile's register allocation
+    unpack8(uint4(*reinterpret_cast<const uint4*>(srow + g * 16)), x);
 #pragma unroll
     for (int j = 0; j < 8; ++j) ss = fmaf(x[j], x[j], ss);
   }
@@ -216,7 +208,7 @@ __device__ __forceinline__ void epilogue_head_norm_rope(const GemmParams& p, con
   for (int g = 0; g < BLOCK_N / 8; ++g) {
     const int c = g * 8;
     float x[8];
-    unpack_bf16x8(*reinterpret_cast<const uint4*>(srow + g * 16), x);
+    unpack8(uint4(*reinterpret_cast<const uint4*>(srow + g * 16)), x);
     const uint4 wq = __ldg(reinterpret_cast<const uint4*>(w + c));
     const uint32_t ww[4] = {wq.x, wq.y, wq.z, wq.w};
     const float4 c0 = __ldg(reinterpret_cast<const float4*>(cs + c)), c1 = __ldg(reinterpret_cast<const float4*>(cs + c + 4));
@@ -321,7 +313,7 @@ __device__ __forceinline__ void epilogue_rows(const GemmParams& p, const TileOut
       const long long row = row0 + STEP * r;
       if (row >= p.M) break;
       float v[8];
-      unpack_bf16x8(*reinterpret_cast<const uint4*>(stg + (rb + STEP * r) * PITCH + cg * 16), v);
+      unpack8(uint4(*reinterpret_cast<const uint4*>(stg + (rb + STEP * r) * PITCH + cg * 16)), v);
       epilogue_group(o.epi, v, rq[r], gq, o.base + row * o.ld + n);
     }
   }
@@ -896,17 +888,11 @@ int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, GemmParams p, cu
                 const LoraParams<LORA>& lx = LoraParams<LORA>{}, const Fp8Params<FP8>& fx = Fp8Params<FP8>{}) {
   static_assert(!LORA || MODE == 0, "the LoRA K-extension is forward-only");
   static_assert(!FP8 || MODE == 0, "FP8 is a mode of the forward GEMM");
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_bf16_kernel<MODE, LORA, FP8>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         PP_SMEM_BYTES);
-    if (e != cudaSuccess) return cuda_err(e, "gemm smem attribute");
-    if (MODE == 0 && !LORA && !FP8) {
-      e = cudaFuncSetAttribute(gemm_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WIDE_SMEM_BYTES);
-      if (e != cudaSuccess) return cuda_err(e, "gemm smem attribute");
-    }
-    attr_set = true;
-  }
+  static bool attr_set = false, wide_attr_set = false;
+  if (int rc = set_max_smem_once(attr_set, PP_SMEM_BYTES, "gemm smem attribute", gemm_bf16_kernel<MODE, LORA, FP8>))
+    return rc;
+  if (MODE == 0 && !LORA && !FP8)
+    if (int rc = set_max_smem_once(wide_attr_set, WIDE_SMEM_BYTES, "gemm smem attribute", gemm_wide_kernel)) return rc;
   p.m_blocks_per_batch = (p.M + BLOCK_M - 1) / BLOCK_M;
   p.num_m_blocks = p.batch * p.m_blocks_per_batch;
   const int tile_n = MODE == 0 && !LORA && !FP8 ? tile_width(p) : BLOCK_N;

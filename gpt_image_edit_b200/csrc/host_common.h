@@ -51,6 +51,19 @@ inline int cuda_err(cudaError_t e, const char* what) {
   return B2F_ERR_CUDA;
 }
 
+// Raises the dynamic shared-memory limit of every kernel in `kernels` to `bytes`, once: `done` is set only when every
+// call succeeded, so a launcher whose call failed tries again on its next launch.
+template <class... Kernels>
+int set_max_smem_once(bool& done, int bytes, const char* what, Kernels*... kernels) {
+  if (done) return B2F_OK;
+  for (const void* k : {reinterpret_cast<const void*>(kernels)...}) {
+    const cudaError_t e = cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e != cudaSuccess) return cuda_err(e, what);
+  }
+  done = true;
+  return B2F_OK;
+}
+
 // Workspace carving: sizes and pointers rounded up to 256 bytes (a null pointer stays null).
 inline size_t al256(size_t n) { return (n + 255) & ~size_t(255); }
 template <class T = uint8_t>

@@ -9,24 +9,6 @@ namespace b2f {
 
 namespace {
 
-__device__ __forceinline__ void unpack8l(const uint4& q, float* f) {
-  const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 t = unpack_bf16x2(w[j]);
-    f[2 * j] = t.x;
-    f[2 * j + 1] = t.y;
-  }
-}
-__device__ __forceinline__ uint4 pack8l(const float* f) {
-  uint4 q;
-  q.x = pack_bf16x2(f[0], f[1]);
-  q.y = pack_bf16x2(f[2], f[3]);
-  q.z = pack_bf16x2(f[4], f[5]);
-  q.w = pack_bf16x2(f[6], f[7]);
-  return q;
-}
-
 // Qwen2RMSNorm: y = w * bf16(x_f32 * rsqrt(mean(x^2) + eps)); one warp per row, D % 256 == 0.
 template <int MAXC>
 __global__ void __launch_bounds__(128) rmsnorm_kernel(const __nv_bfloat16* x, long long ldx,
@@ -41,7 +23,7 @@ __global__ void __launch_bounds__(128) rmsnorm_kernel(const __nv_bfloat16* x, lo
 #pragma unroll
   for (int c = 0; c < MAXC; ++c)
     if (c < nchunk) {
-      unpack8l(*reinterpret_cast<const uint4*>(x + r * ldx + c * 256 + lane * 8), v[c]);
+      unpack8(*reinterpret_cast<const uint4*>(x + r * ldx + c * 256 + lane * 8), v[c]);
 #pragma unroll
       for (int j = 0; j < 8; ++j) ss += v[c][j] * v[c][j];
     }
@@ -52,10 +34,10 @@ __global__ void __launch_bounds__(128) rmsnorm_kernel(const __nv_bfloat16* x, lo
   for (int c = 0; c < MAXC; ++c)
     if (c < nchunk) {
       float g[8], o[8];
-      unpack8l(__ldg(reinterpret_cast<const uint4*>(w + c * 256 + lane * 8)), g);
+      unpack8(__ldg(reinterpret_cast<const uint4*>(w + c * 256 + lane * 8)), g);
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = g[j] * bf16r(v[c][j] * rs);
-      *reinterpret_cast<uint4*>(y + r * ldy + c * 256 + lane * 8) = pack8l(o);
+      *reinterpret_cast<uint4*>(y + r * ldy + c * 256 + lane * 8) = pack8(o);
     }
 }
 
@@ -101,11 +83,11 @@ __global__ void __launch_bounds__(256) swiglu_kernel(const __nv_bfloat16* gu, lo
   const long long r = i / vec;
   const int c = int(i - r * vec) * 8;
   float g[8], u[8], o[8];
-  unpack8l(*reinterpret_cast<const uint4*>(gu + r * ld + c), g);
-  unpack8l(*reinterpret_cast<const uint4*>(gu + r * ld + I + c), u);
+  unpack8(*reinterpret_cast<const uint4*>(gu + r * ld + c), g);
+  unpack8(*reinterpret_cast<const uint4*>(gu + r * ld + I + c), u);
 #pragma unroll
   for (int j = 0; j < 8; ++j) o[j] = bf16r(g[j] / (1.0f + __expf(-g[j]))) * u[j];
-  *reinterpret_cast<uint4*>(out + r * ldo + c) = pack8l(o);
+  *reinterpret_cast<uint4*>(out + r * ldo + c) = pack8(o);
 }
 
 // out[i, :] = table[idx[i], :]   (gather)   or   out[idx[i], :] = src[i, :]   (scatter)
@@ -136,15 +118,15 @@ __global__ void __launch_bounds__(256) geglu_kernel(const __nv_bfloat16* gu, lon
   const long long r = i / vec;
   const int c = int(i - r * vec) * 8;
   float g[8], u[8], o[8];
-  unpack8l(*reinterpret_cast<const uint4*>(gu + r * ld + c), g);
-  unpack8l(*reinterpret_cast<const uint4*>(gu + r * ld + I + c), u);
+  unpack8(*reinterpret_cast<const uint4*>(gu + r * ld + c), g);
+  unpack8(*reinterpret_cast<const uint4*>(gu + r * ld + I + c), u);
 #pragma unroll
   for (int j = 0; j < 8; ++j) {
     const float x = g[j];
     const float t = tanhf(0.7978845608028654f * (x + 0.044715f * x * x * x));
     o[j] = bf16r(0.5f * x * (1.0f + t)) * u[j];
   }
-  *reinterpret_cast<uint4*>(out + r * ldo + c) = pack8l(o);
+  *reinterpret_cast<uint4*>(out + r * ldo + c) = pack8(o);
 }
 
 // nn.LayerNorm with affine weight and bias (CLIP text encoder): fp32 statistics, one rounding.
@@ -162,7 +144,7 @@ __global__ void __launch_bounds__(128) layernorm_kernel(const __nv_bfloat16* x, 
 #pragma unroll
   for (int c = 0; c < MAXC; ++c)
     if (c < nchunk) {
-      unpack8l(*reinterpret_cast<const uint4*>(x + r * ldx + c * 256 + lane * 8), v[c]);
+      unpack8(*reinterpret_cast<const uint4*>(x + r * ldx + c * 256 + lane * 8), v[c]);
 #pragma unroll
       for (int j = 0; j < 8; ++j) sum += v[c][j];
     }
@@ -186,11 +168,11 @@ __global__ void __launch_bounds__(128) layernorm_kernel(const __nv_bfloat16* x, 
   for (int c = 0; c < MAXC; ++c)
     if (c < nchunk) {
       float g[8], bb[8], o[8];
-      unpack8l(__ldg(reinterpret_cast<const uint4*>(w + c * 256 + lane * 8)), g);
-      unpack8l(__ldg(reinterpret_cast<const uint4*>(b + c * 256 + lane * 8)), bb);
+      unpack8(__ldg(reinterpret_cast<const uint4*>(w + c * 256 + lane * 8)), g);
+      unpack8(__ldg(reinterpret_cast<const uint4*>(b + c * 256 + lane * 8)), bb);
 #pragma unroll
       for (int j = 0; j < 8; ++j) o[j] = (v[c][j] - mean) * rs * g[j] + bb[j];
-      *reinterpret_cast<uint4*>(y + r * ldy + c * 256 + lane * 8) = pack8l(o);
+      *reinterpret_cast<uint4*>(y + r * ldy + c * 256 + lane * 8) = pack8(o);
     }
 }
 
@@ -205,14 +187,14 @@ __global__ void __launch_bounds__(256) embed_kernel(const __nv_bfloat16* tok, lo
   const long long r = i / vec;
   const int c = int(i - r * vec) * 8;
   float a[8];
-  unpack8l(*reinterpret_cast<const uint4*>(tok + ids[r] * ld_tok + c), a);
+  unpack8(*reinterpret_cast<const uint4*>(tok + ids[r] * ld_tok + c), a);
   if (pos) {
     float b[8];
-    unpack8l(*reinterpret_cast<const uint4*>(pos + (r % period) * ld_pos + c), b);
+    unpack8(*reinterpret_cast<const uint4*>(pos + (r % period) * ld_pos + c), b);
 #pragma unroll
     for (int j = 0; j < 8; ++j) a[j] += b[j];
   }
-  *reinterpret_cast<uint4*>(out + r * ldo + c) = pack8l(a);
+  *reinterpret_cast<uint4*>(out + r * ldo + c) = pack8(a);
 }
 
 }  // namespace

@@ -14,29 +14,6 @@ namespace b2f {
 
 namespace {
 
-__device__ __forceinline__ void unpack8(const uint4& q, float* f) {
-  const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 t = unpack_bf16x2(w[j]);
-    f[2 * j] = t.x;
-    f[2 * j + 1] = t.y;
-  }
-}
-__device__ __forceinline__ uint4 pack8(const float* f) {
-  uint4 q;
-  q.x = pack_bf16x2(f[0], f[1]);
-  q.y = pack_bf16x2(f[2], f[3]);
-  q.z = pack_bf16x2(f[4], f[5]);
-  q.w = pack_bf16x2(f[6], f[7]);
-  return q;
-}
-__device__ __forceinline__ float warp_sum(float v) {
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-  return v;
-}
-
 constexpr int CHUNK_ROWS = 32;   // token rows per block of the column-reduction kernels
 
 // ------------------------------------------------------------------------------------------------

@@ -9,24 +9,6 @@ namespace b2f {
 
 namespace {
 
-__device__ __forceinline__ void unpack8v(const uint4& q, float* f) {
-  const uint32_t w[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const float2 t = unpack_bf16x2(w[j]);
-    f[2 * j] = t.x;
-    f[2 * j + 1] = t.y;
-  }
-}
-__device__ __forceinline__ uint4 pack8v(const float* f) {
-  uint4 q;
-  q.x = pack_bf16x2(f[0], f[1]);
-  q.y = pack_bf16x2(f[2], f[3]);
-  q.z = pack_bf16x2(f[4], f[5]);
-  q.w = pack_bf16x2(f[6], f[7]);
-  return q;
-}
-
 // ---------------------------------------------------------------- GroupNorm statistics
 // x: [N, P, C] (P = H*W pixels).  stats: double [N, 32, 2] (sum, sum of squares), zeroed by caller.
 // Thread t of a block owns the channel octet (t % (C/8)) and strides over pixels; per-thread fp32
@@ -52,7 +34,7 @@ __global__ void __launch_bounds__(GN_THREADS) gn_stats_kernel(const __nv_bfloat1
   if (prow < rows_per_iter) {
     for (long long pp = p0 + prow; pp < p1; pp += rows_per_iter) {
       float f[8];
-      unpack8v(*reinterpret_cast<const uint4*>(base + pp * C), f);
+      unpack8(*reinterpret_cast<const uint4*>(base + pp * C), f);
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         s[j] += f[j];
@@ -97,9 +79,9 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const __nv_bfloat16* x, c
   const double cnt = (double)P * cpg;
   float f[8], ga[8], be[8], o[8];
   const long long off = ((long long)n * P) * C + i * 8;
-  unpack8v(*reinterpret_cast<const uint4*>(x + off), f);
-  unpack8v(__ldg(reinterpret_cast<const uint4*>(gamma + oct * 8)), ga);
-  unpack8v(__ldg(reinterpret_cast<const uint4*>(beta + oct * 8)), be);
+  unpack8(*reinterpret_cast<const uint4*>(x + off), f);
+  unpack8(__ldg(reinterpret_cast<const uint4*>(gamma + oct * 8)), ga);
+  unpack8(__ldg(reinterpret_cast<const uint4*>(beta + oct * 8)), be);
   // an octet of channels touches at most 8/cpg groups (one for the real widths, cpg >= 8, two for
   // cpg = 4): derive mean / rstd once per distinct group, in double, then stay in fp32
   int g_prev = -1;
@@ -118,7 +100,7 @@ __global__ void __launch_bounds__(256) gn_apply_kernel(const __nv_bfloat16* x, c
     if (silu) v = v / (1.0f + __expf(-v));
     o[j] = v;
   }
-  *reinterpret_cast<uint4*>(y + off) = pack8v(o);
+  *reinterpret_cast<uint4*>(y + off) = pack8(o);
 }
 
 // ---------------------------------------------------------------- nearest 2x upsample (NHWC)
@@ -155,7 +137,7 @@ __global__ void __launch_bounds__(256) nchw_to_nhwc_pad_kernel(const T* in, __nv
     const int c = o * 8 + j;
     f[j] = c < C ? (float)in[((long long)n * C + c) * hw + p] : 0.f;
   }
-  reinterpret_cast<uint4*>(out)[i] = pack8v(f);
+  reinterpret_cast<uint4*>(out)[i] = pack8(f);
 }
 
 // uint8 NHWC [N, H, W, C] image -> NHWC bf16 in [-1, 1], channels zero-padded to Cpad: the reference's host-side
@@ -174,7 +156,7 @@ __global__ void __launch_bounds__(256) u8_nhwc_to_nhwc_pad_kernel(const uint8_t*
     const int c = o * 8 + j;
     f[j] = c < C ? ((float)in[pix * C + c] / 255.0f - 0.5f) / 0.5f : 0.f;
   }
-  reinterpret_cast<uint4*>(out)[i] = pack8v(f);
+  reinterpret_cast<uint4*>(out)[i] = pack8(f);
 }
 
 // ---------------------------------------------------------------- row softmax, bf16 out
@@ -182,7 +164,7 @@ __global__ void __launch_bounds__(256) u8_nhwc_to_nhwc_pad_kernel(const uint8_t*
 // are read and written as 8-wide vectors over [0, round_up(L, 8)): the columns [L, round_up(L, 8)) of the last vector
 // are left out of the max and the sum and written as zeros (the VAE's attention contracts P.V over the padded length).
 __device__ __forceinline__ void load8(const __nv_bfloat16* row, int i, float* f) {
-  unpack8v(reinterpret_cast<const uint4*>(row)[i], f);
+  unpack8(reinterpret_cast<const uint4*>(row)[i], f);
 }
 __device__ __forceinline__ void load8(const float* row, int i, float* f) {
   const float4 a = reinterpret_cast<const float4*>(row)[2 * i], b = reinterpret_cast<const float4*>(row)[2 * i + 1];
@@ -234,7 +216,7 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(const T* s, long long
     load8(row, i, f);
 #pragma unroll
     for (int j = 0; j < 8; ++j) f[j] = i * 8 + j < L ? exp2f((f[j] - mx) * k) * inv : 0.f;
-    reinterpret_cast<uint4*>(prow)[i] = pack8v(f);
+    reinterpret_cast<uint4*>(prow)[i] = pack8(f);
   }
 }
 
